@@ -1,10 +1,10 @@
-"""Benchmark of the volumetric-render hot path (BASELINE.json: rays/s @ 64 samples/ray).
+"""Benchmark of the volumetric-render hot path (rays/s @ 64 samples/ray).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config c2|c3|c4|c5]
                   [--precision tc_fp16x3|tc_fp16|fp32] [--dense]
 
-Default (`--config c2`, the configuration BASELINE.json's metric is quoted on): a "step" = one pass of the hot path over
-one synthetic batch: at N=1 ONE 512x512 all-hit view of the synth-313 body (BASELINE.json configs[1]: single B200,
+Default (`--config c2`, the configuration the headline metric is quoted on): a "step" = one pass of the hot path over
+one synthetic batch: at N=1 ONE 512x512 all-hit view of the synth-313 body (single H100,
 262 144 rays x 64 samples, eval, no jitter, random-init trained-like decoder).  At N>1 a step is N such views, each
 ray-sharded over the N ranks with one NCCL all-gather per view (issued on a side stream, overlapping the next view) --
 per-GPU work is fixed (262 144 rays per step) => "scaling": "weak".
@@ -14,11 +14,11 @@ per-GPU work is fixed (262 144 rays per step) => "scaling": "weak".
 `e2e`    : the same metric through the public API make_renderer(cfg, net).render(batch) with the batch in PINNED HOST
            memory: H2D of rays/near/far/pose per step, prepare_sp_input, weight pack, render, D2H of rgb_map + depth_map
            (at N>1: of the GATHERED frame, on the view's owner rank v % N, each GPU using its own PCIe link) inside the timed region.
-`--impl reference`: the reference's own CPU implementation of the path (the oracle port of /root/reference's
+`--impl reference`: the reference's own CPU implementation of the path (the oracle port of the reference's
            if_clight_renderer + latent_xyzc + raw2outputs, validated bit-exact against the unmodified reference in the
            build container), all host threads, each step a bounded sample (--ref-rays rays) of the same workload.
 
-Other BASELINE.json configurations (their own JSON line, same keys; committed under profiles/):
+Other configurations (their own JSON line, same keys):
   --config c3   one N_rand = 1024 training chunk, 64 + 128 samples, forward + backward (gradient path on)
   --config c4   144 novel views of the reference's spiral path (render_utils.gen_path), 512x512, rays generated on the
                 device per view, ray-sharded over the N ranks, one gather per frame
@@ -42,7 +42,7 @@ H = W = 512
 S = 64
 FLOP_PER_SAMPLE_AS_WRITTEN = 859904     # SURVEY.md 8d: 2 x 429 952 MAC, layers of latent_xyzc.py:20-28
 FLOP_PER_SAMPLE_FOLDED = 532224         # exact fold of feature_fc o latent_fc o view_fc[:, :256]
-# tensor-core FLOPs the kernel actually ISSUES per sample (dense UMMA tiles incl. bias K-steps, the
+# tensor-core FLOPs the kernel actually ISSUES per sample (dense MMA tiles incl. bias K-steps, the
 # alpha/rgb rows and, in the 3-pass mode, the A_lo*W_hi and A_hi*W_lo correction passes; layer 3 takes the
 # lo half of its input only on the 16-row density block)
 FLOP_PER_SAMPLE_ISSUED = {"tc_fp16": 2 * 16 * (23 * 256 + 2 * 17 * 256 + 22 * 144 + 9 * 16),
@@ -58,13 +58,14 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "tf_burst": d.get("bf16_tflops", 1590.0),
-                "tf_sustained": d.get("bf16_tflops_sustained", 1400.0), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+        return {"hbm_gbs": d.get("hbm_gbs", 3350.0), "tf_burst": d.get("bf16_tflops", 989.0),
+                "tf_sustained": d.get("bf16_tflops_sustained", 989.0), "src": "measured"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense fp16 / bf16 TFLOP/s -- not reached figures
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "fallback (H100 SXM data sheet)"}
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md), in-process through NVML (pynvml) from a
+    """SM clock and throttle reasons sampled DURING the timed region, in-process through NVML (pynvml) from a
     background thread.  The `nvidia-smi -lms` loop it replaces holds a driver lock for tens of ms per query: invisible to the
     3-launch steps of c2, but it stalled the ~400 launches of a c3 step every 50 ms (measured: 60-130 ms steps among 6.5 ms ones)."""
     REASONS = (("hw_slowdown", "nvmlClocksEventReasonHwSlowdown"), ("hw_thermal_slowdown", "nvmlClocksEventReasonHwThermalSlowdown"),
@@ -123,7 +124,7 @@ class ClockSampler:
 
 
 def host_info():
-    """Core count and CPU model of the box the CPU arm ran on (BASELINE.md section 4)."""
+    """Core count and CPU model of the box the CPU arm ran on (the CPU arm of the benchmark)."""
     model = None
     try:
         for line in open("/proc/cpuinfo"):
@@ -284,7 +285,7 @@ class Product:
             "tensor_tflops_issued": (tflops_exec * issued / flop_exec),
             "tensor_issued_frac_of_sustained": (tflops_exec * issued / flop_exec) / peaks["tf_sustained"],
             "achieved_if_counted_as_written": tflops_written,
-            "kernel": ("render_tc_list_kernel<%d> (CTA pairs, tcgen05 cta_group::2)" % (3 if precision == "tc_fp16x3" else 1))
+            "kernel": ("render_tc_list_kernel<%d> (two warpgroups per CTA, wgmma)" % (3 if precision == "tc_fp16x3" else 1))
                       if precision != "fp32" else "render_f32_kernel (fp32 FFMA pipe, no tensor cores)",
             "kernel_ms": kernel_ms, "kernel_ms_source": src,
             "kernel_share_of_step": (kernel_ms * kernel_launches / total_ms) if kernel_ms else None,
@@ -308,7 +309,7 @@ def time_steps(args, dev, world, step_fn, before_step=None):
             dist.barrier()
         torch.cuda.synchronize(dev)
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
     for _ in range(args.warmup):
         step_fn()
     barrier()
@@ -326,6 +327,26 @@ def time_steps(args, dev, world, step_fn, before_step=None):
     barrier()
     step_ms = [a.elapsed_time(b) for a, b in ev]
     return sum(step_ms), step_ms
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: what the timed path computed in its last step, one float32 DIR/<name>.npy per output array.
+
+    A ray that accumulates no weight (acc_map == 0) has no surface: its depth is at infinity, so its disparity is stored as 0
+    (raw2outputs itself returns 1 / max(1e-10, 0 / 0) = NaN there, and acc_map marks those rays).  Any other non-finite value
+    is an error of the render, not something to store."""
+    import numpy as np
+    out = {k: v.detach().float().cpu().contiguous().numpy() for k, v in arrays.items()}
+    if "disp_map" in out and "acc_map" in out:
+        disp = out["disp_map"].copy()
+        disp[(out["acc_map"] == 0) & np.isnan(disp)] = 0.0
+        out["disp_map"] = disp
+    bad = [k for k, a in out.items() if not np.isfinite(a).all()]
+    if bad:
+        raise RuntimeError("--dump-outputs: non-finite values in %s" % ", ".join(bad))
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 def max_over_ranks(vals, dev, world):
@@ -370,11 +391,13 @@ def run_c2(args, rank, world, local_rank):
     vol = net.encode_sparse_voxels(sp_input)
     gatherer = nbdist.FrameGatherer(H * W, world, rank, dev)
 
+    last = {}
+
     def device_step():
         for _ in range(n_views):
             out = gatherer.begin()
             ren.render_rays(local["ray_o"], local["ray_d"], local["near"], local["far"], vol, sp_input, out=out)
-            gatherer.finish()
+            last["frame"] = gatherer.finish()
         if world > 1:     # the step ends when the last frame is assembled: the compute stream waits for the side stream
             torch.cuda.current_stream(dev).wait_stream(gatherer.side)
 
@@ -400,6 +423,9 @@ def run_c2(args, rank, world, local_rank):
     launches = ren.launches - launches0[0]
     stats = [int(v) for v in ren.stats.tolist()]
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        gatherer.drain()
+        dump_outputs(args.dump_outputs, nbdist.slab_views(last["frame"]))
 
     # ---- e2e through the public API with host buffers: per view H2D of this rank's rays (+ the frame's pose tensors) from
     # pinned memory, Renderer.render, the gather, and the D2H of the GATHERED frame on the view's owner (rank v % N)
@@ -477,7 +503,7 @@ def run_c2(args, rank, world, local_rank):
                               "unused downstream, SURVEY 8b)",
                    "parallelism": ("ray-sharded x%d (interleaved 256-ray chunks), one all-gather per view on a side stream, "
                                    "frame assembled on every rank" % world) if world > 1 else "single GPU",
-                   "l2": "256 MiB written between timed steps (untimed) to flush the 126 MB L2",
+                   "l2": "256 MiB written between timed steps (untimed) to flush the 50 MB L2",
                    "volume": "fp16 channels-last 69 MB, packed once (cached across views of the frame)"
                              if precision == "tc_fp16" else "fp32 channels-last 137 MB, packed once (cached across views)"},
         "roofline": roofline,
@@ -937,7 +963,7 @@ def run_c3(args, rank, world, local_rank):
     line = {
         "metric": "train_rays_per_s_fwd_bwd", "value": value, "unit": "rays/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": ("tf32x2 (hi+lo TF32 pairs, 3 tcgen05 passes, fp32 accumulate)" if args.train_precision == "tc_tf32x3"
+        "dtype": ("tf32x2 (hi+lo TF32 pairs, 3 wgmma passes, fp32 accumulate)" if args.train_precision == "tc_tf32x3"
                   else "f32 (exact FFMA kernels)"), "data": "synthetic",
         "config": {"workload": "BASELINE configs[2]: one N_rand = 1024 training chunk of the synth-313 frame, %d coarse%s samples, "
                                "net.train(), perturb = 1, loss = mse(rgb_map) (+ mse(rgb0)), forward + backward through nb_render_fwd / "
@@ -966,7 +992,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="c2", choices=["c2", "c3", "c4", "c5"],
-                    help="BASELINE.json configuration: c2 (default) 512x512 view; c3 training chunk; c4 144 spiral views; c5 8 poses")
+                    help="configuration: c2 (default) 512x512 view; c3 training chunk; c4 144 spiral views; c5 8 poses")
     ap.add_argument("--precision", default="auto", choices=["auto", "tc_fp16x3", "tc_fp16", "fp32"])
     ap.add_argument("--ref-rays", type=int, default=4096, help="rays per step of the CPU arm / baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -976,6 +1002,9 @@ def main():
     ap.add_argument("--c5-size", type=int, default=1024, help="c5: image side")
     ap.add_argument("--train-precision", default="tc_tf32x3", choices=["tc_tf32x3", "fp32"], help="c3: precision of the gradient path")
     ap.add_argument("--importance", type=int, default=128, help="c3: importance samples of the fine pass (0 = coarse only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="c2: after the timed steps, write the last step's rgb_map / disp_map / acc_map / depth_map as DIR/<name>.npy "
+                         "(float32; rays with acc_map == 0 have disparity 0)")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = {"c2": 20, "c3": 20, "c4": 2, "c5": 3}[args.config]

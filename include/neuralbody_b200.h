@@ -1,4 +1,4 @@
-/* neuralbody_b200 -- C ABI of the B200-native volumetric-render hot path.
+/* neuralbody_b200 -- C ABI of the H100-native (sm_90a) volumetric-render hot path.
  *
  * The reference (zju3dv/neuralbody @ 3c516b9) is pure Python over PyTorch and has no FFI
  * of its own; its plugin boundary for this path is
@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NB_ABI_VERSION 4
+#define NB_ABI_VERSION 5
 
 #define NB_OK               0
 #define NB_ERR_BAD_ARG     (-1)
@@ -37,9 +37,9 @@ extern "C" {
 
 /* arithmetic of the decoder MLP inside nb_render_fwd */
 #define NB_PRECISION_FP32      0   /* exact: fp32 FFMA everywhere (GPU-side oracle, fallback)            */
-#define NB_PRECISION_TC_FP16   1   /* tcgen05 tensor cores: fp16 operands, fp32 accumulate in TMEM       */
-#define NB_PRECISION_TC_FP16X3 2   /* tcgen05, density path as hi+lo fp16 pairs, 3 MMA passes: ~fp32-accurate */
-#define NB_PRECISION_TC_TF32X3 3   /* training: sample list + tcgen05 kind::tf32 GEMM chains, hi+lo TF32 pairs, 3 passes (fp32-grade);
+#define NB_PRECISION_TC_FP16   1   /* wgmma tensor cores: fp16 operands, fp32 accumulate                 */
+#define NB_PRECISION_TC_FP16X3 2   /* wgmma, density path as hi+lo fp16 pairs, 3 MMA passes: ~fp32-accurate */
+#define NB_PRECISION_TC_TF32X3 3   /* training: sample list + wgmma tf32 GEMM chains, hi+lo TF32 pairs, 3 passes (fp32-grade);
                                       writes the activation record nb_render_bwd consumes; needs `save` and `raw` */
 
 #define NB_NUM_LEVELS   4          /* SparseConvNet returns 4 dense volumes, latent_xyzc.py:179-204     */
@@ -74,7 +74,7 @@ int    nb_pack_volume(const nb_volume_level levels[NB_NUM_LEVELS], int batch, in
  * All pointers device fp32, Conv1d layout (out, in[, 1]).  The pack step performs the exact
  * fold  view_fc[:, :256] o latent_fc o (feature_fc (+) latent[latent_index])  (no activation
  * between those layers) in fp64, and emits fp32 K-major matrices for the exact kernel and fp16
- * tcgen05-canonical (UMMA K-major, no-swizzle) matrices for the tensor-core kernel.
+ * canonical (K-major, no-swizzle) matrices of the wgmma shared-memory descriptor for the tensor-core kernel.
  */
 typedef struct nb_decoder_weights {
     const float *fc0_w, *fc0_b;         /* (256,352) (256) */
@@ -264,23 +264,8 @@ size_t nb_render_bwd_workspace_bytes_for(const nb_render_args* fwd);
 int    nb_render_bwd(const nb_render_bwd_args* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Diagnostics.  A two-layer tcgen05 micro-pipeline on one 128-row tile (see csrc/nb_tc_probe.cu):
- * validates descriptor layouts, TMEM-resident activations and the bias-as-K-step trick in
- * isolation.  a0: device fp16 [128][64] row-major; w0_packed: device fp16 128x80 in the packed
- * K-major layout (columns 64/65 = bias hi/lo); w1_packed: 64x128 packed; d0_out fp32 [128][128];
- * d1_out fp32 [128][64].  variant bit0 swaps the descriptor's LBO/SBO, bit1 the fp16 pair order. */
-int nb_debug_tc_probe(const void* a0, const void* w0_packed, const void* w1_packed, float* d0_out, float* d1_out,
-                      int variant, void* stream);
-/* The same idea for a CTA PAIR (tcgen05 cta_group::2, see csrc/nb_tc_probe2.cu): one 256-row tile, 128 rows per CTA of a
- * 2-cluster, every B operand split by N halves across the two CTAs.  a0: device fp16 [256][64]; w0_halves: fp16 [2][128 x 80]
- * packed (rank r holds rows 128 r .. of the 256 x 80 matrix, columns 64/65 = bias hi/lo); w1_halves: fp16 [2][72 x 128] packed;
- * d0_out fp32 [256][256]; d1_out fp32 [256][144] (= relu(d0[:, :128]) w1^T, plus a second accumulation of each half's local
- * rows 64..71 into columns 64..79). */
-int nb_debug_tc_probe2(const void* a0, const void* w0_halves, const void* w1_halves, float* d0_out, float* d1_out, void* stream);
-/* Timing probe (csrc/nb_tc_bench.cu): n_mma back-to-back tcgen05.mma of M = 128 (one CTA) or M = 256 (CTA pair, variant bit 1), N
- * columns, K = 16, A from shared memory or (variant bit 0) TMEM.  out: device i64[2] = cycles until the last issue returned /
- * until the commit arrived.  tools/mma_rate.py prints the table. */
-int nb_debug_mma_rate(int variant, int n_mma, int N, long long* out, void* stream);
+ * Diagnostics.
+ */
 /* The training path's GEMM in isolation (csrc/nb_train.cu): c (M,N) = epilogue(a b^T), fp32 in and out, 3 x TF32 passes.
  * a: (M,K) if a_k_contiguous else (K,M); b: (N,K) if b_k_contiguous else (K,N); N % 16 == 0, leading dimensions % 4 == 0.
  * splits > 1 splits the reduction over CTAs and ACCUMULATES into c (zero it first).  bias (N) / mask (M,N) may be NULL. */

@@ -13,7 +13,7 @@ NB_NUM_LEVELS = 4
 
 EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_volume_bytes", "nb_packed_volume_level_offset",
            "nb_pack_volume", "nb_packed_weights_bytes", "nb_pack_weights", "nb_render_fwd",
-           "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_debug_tc_probe", "nb_debug_tc_probe2", "nb_debug_mma_rate", "nb_render_bwd", "nb_render_save_bytes",
+           "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_render_bwd", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf"]
 
 
@@ -124,11 +124,7 @@ def load(path=None):
     lib.nb_gen_rays_sharded.argtypes = [C.POINTER(nb_camera)] + [C.c_int] * 4 + [C.c_void_p] * 6
     lib.nb_sample_pdf.restype = C.c_int
     lib.nb_sample_pdf.argtypes = [C.POINTER(nb_importance_args), C.c_void_p]
-    lib.nb_debug_tc_probe.restype = C.c_int
-    lib.nb_debug_tc_probe.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_void_p]
-    lib.nb_debug_tc_probe2.restype = C.c_int
-    lib.nb_debug_tc_probe2.argtypes = [C.c_void_p] * 6
-    if lib.nb_abi_version() != 4:
+    if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):
         _lib = lib

@@ -371,7 +371,7 @@ int nb_pack_volume(const nb_volume_level levels[NB_NUM_LEVELS], int batch, int d
     for (int l = 0; l < NB_NUM_LEVELS; ++l) {
         const size_t nvox = (size_t)levels[l].D * levels[l].H * levels[l].W;
         const size_t tiles = ((nvox + 31) / 32) * ((levels[l].C + 31) / 32) * batch;
-        const int grid = (int)(tiles < 148 * 16 ? tiles : 148 * 16);
+        const int grid = (int)(tiles < kGridSMs * 16 ? tiles : kGridSMs * 16);
         char* dst = (char*)out_blob + nb_packed_volume_level_offset(dims, batch, dtype, l);
         unsigned* vb = (unsigned*)((char*)out_blob + occ_offset(dims, batch, dtype, l, 0));
         unsigned* cb = (unsigned*)((char*)out_blob + occ_offset(dims, batch, dtype, l, 1));
@@ -380,7 +380,7 @@ int nb_pack_volume(const nb_volume_level levels[NB_NUM_LEVELS], int batch, int d
         else
             pack_volume_kernel<float><<<grid, 256, 0, st>>>(levels[l].data, (float*)dst, levels[l].C, nvox, batch, vb, vox_words(dims[l]));
         const size_t ncellp = cell_words(dims[l]) * 32 * batch;
-        const int cgrid = (int)((ncellp + 255) / 256 < 148 * 8 ? (ncellp + 255) / 256 : 148 * 8);
+        const int cgrid = (int)((ncellp + 255) / 256 < kGridSMs * 8 ? (ncellp + 255) / 256 : kGridSMs * 8);
         cell_occupancy_kernel<<<cgrid, 256, 0, st>>>(vb, cb, levels[l].D, levels[l].H, levels[l].W, vox_words(dims[l]),
                                                      cell_words(dims[l]), batch);
     }
@@ -411,9 +411,9 @@ int nb_pack_weights(const nb_decoder_weights* w, void* out_blob, size_t out_byte
     fold_T_kernel<<<(n1 + 127) / 128, 128, 0, st>>>(*w, T, u);
     const int n2 = kColor * kHidden + w->batch * kColor;
     fold_Wc_kernel<<<(n2 + 127) / 128, 128, 0, st>>>(*w, T, u, f32, f16, bc);
-    relayout_kernel<<<148, 256, 0, st>>>(*w, f32, f16);
+    relayout_kernel<<<kGridSMs, 256, 0, st>>>(*w, f32, f16);
     sigma_empty_kernel<<<1, kHidden, 0, st>>>(*w, f32);
-    stream_kernel<<<148, 256, 0, st>>>(*w, f32, bc, f16, (__half*)(base + frame_step_byte_offset(w->batch)));
+    stream_kernel<<<kGridSMs, 256, 0, st>>>(*w, f32, bc, f16, (__half*)(base + frame_step_byte_offset(w->batch)));
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_pack_weights: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     return NB_OK;

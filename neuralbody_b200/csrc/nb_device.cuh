@@ -1,4 +1,4 @@
-// Device helpers shared by the exact-fp32 and the tcgen05 render kernels:
+// Device helpers shared by the exact-fp32 and the tensor-core render kernels:
 // sample generation, world->SMPL->grid transform, trilinear corner set-up,
 // positional encoding and the alpha-compositing warp scan.
 //

@@ -10,6 +10,10 @@ namespace nb {
 
 void set_error(const char* fmt, ...);
 
+// Grid-size unit of the persistent / grid-stride kernels: the SM count of the H100 SXM.  (Launches that must match the
+// device's SM count exactly query cudaDevAttrMultiProcessorCount instead.)
+constexpr int kGridSMs = 132;
+
 // Kernel-side view of one nb_render_fwd call (passed by value as a __grid_constant__).
 struct RenderParams {
     int batch, n_rays, n_samples;

@@ -48,7 +48,7 @@ constexpr size_t oSigmaEmpty = oWc + (size_t)kColor * kHidden;   // [1] (+3 pad)
 constexpr size_t kF32Floats = oSigmaEmpty + 4;
 
 // ---- fp16 section: the tensor-core kernel's weight STREAM, in consumption order.
-// One "step" = the B operand of one K=16 tcgen05.mma: an N x 16 tile in the canonical K-major
+// One "step" = the B operand of one K=16 MMA: an N x 16 tile in the canonical K-major
 // no-swizzle layout: element (n, kk) at half-offset ((kk/8) * (N/8) + n/8) * 64 + (n%8) * 8 + (kk%8),
 // i.e. 8x8 core matrices (8 rows x 16 B = 128 B contiguous); stride-byte-offset (next 8 rows) = 128 B,
 // leading-byte-offset (next 8-wide K chunk) = N*16 B.
@@ -89,18 +89,17 @@ __host__ __device__ inline int feat_tc_to_orig(int j) {
 __host__ __device__ inline int class_segments(int c) { return c == 0 ? 6 : c == 1 ? 5 : c == 2 ? 4 : 2; }
 __host__ __device__ inline int class_ksteps(int c) { return c == 0 ? 22 : c == 1 ? 20 : c == 2 ? 16 : 8; }
 
-// The tensor-core decoder runs on CTA PAIRS (tcgen05 cta_group::2): every B operand is split by N halves across the two CTAs'
-// shared memory, so each CTA streams only ITS half of every step -- half the bytes per SM.  A step of an N-wide layer is
-// therefore stored as two (N/2) x 16 tiles (same canonical K-major layout, N/2 rows), arranged so that what ONE CTA loads for
-// one ring slot is one contiguous run:
+// The tensor-core decoder multiplies every layer as two N halves (one wgmma per half and K-step), so a step of an N-wide
+// layer is stored as two (N/2) x 16 tiles (same canonical K-major layout, N/2 rows), arranged so that the tiles of one half
+// and plane are contiguous runs:
 //   N = 256 layers: group g of gs K-steps = [half 0: gs hi tiles, gs lo tiles][half 1: gs hi tiles, gs lo tiles]  (4 KB tiles);
 //                   bias step = [half 0 tile][half 1 tile]
 //   L3 (N = 128)  : the folded colour layer: [half 0: steps 0..20][half 1: steps 0..20] (64 x 16 tiles); the per-frame step 21
 //                   is [B][half][tile].  alpha_fc (1 x 256) and rgb_fc (3 x 128) are NOT in the stream: the epilogue applies them
-//                   in fp32 to the accumulators it converts anyway (a 1- or 3-wide layer costs the tensor pipe a full
-//                   instruction slot per K-step -- measured ~200 cycles each -- for a few hundred FMAs per row).
+//                   in fp32 to the accumulators it converts anyway (a 1- or 3-wide layer would cost the tensor pipe a full
+//                   instruction per K-step for a few hundred FMAs per row).
 constexpr int kHalfTile256 = 128 * 16;                     // halves in one (N/2 = 128) x 16 tile
-constexpr int kHalfTile3 = (kN3 / 2) * 16;                 // 72 x 16
+constexpr int kHalfTile3 = (kN3 / 2) * 16;                 // 64 x 16
 constexpr int kHalfTile4 = (kN4 / 2) * 16;                 // 8 x 16
 // half-offset (from the layer base) of the first tile CTA `half` loads for the group starting at K-step g0
 __host__ __device__ inline size_t pair_group_offset(int g0, int half, int nks) {

@@ -505,7 +505,7 @@ extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
     const size_t smem = ((size_t)bwd::TP * bwd::LDX + (size_t)bwd::TP * bwd::LDY + (size_t)bwd::KC * kFeat) * 4;
     cudaFuncSetAttribute(bwd::decoder_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const size_t ntiles = (npts + bwd::TP - 1) / bwd::TP;
-    bwd::decoder_dgrad_kernel<<<(unsigned)(ntiles < 148 ? ntiles : 148), bwd::NT, smem, s>>>(Q);
+    bwd::decoder_dgrad_kernel<<<(unsigned)(ntiles < kGridSMs ? ntiles : kGridSMs), bwd::NT, smem, s>>>(Q);
 
     // scratch after the per-point region
     float* extra = Q.ws + npts * kGradDim;

@@ -4,7 +4,7 @@
 // (lib/networks/renderer/if_clight_renderer.py:107-120): sampling, world->SMPL->grid,
 // 4-level trilinear gather from the channels-last packed volume, the decoder MLP in
 // fp32 FFMA, positional encodings, and the alpha composite.  No activation ever leaves
-// shared memory.  This is the GPU-side oracle and the fallback for shapes the tcgen05
+// shared memory.  This is the GPU-side oracle and the fallback for shapes the tensor-core
 // kernel does not take; its roofline is the fp32 FFMA pipe, not the tensor cores.
 //
 // CTA = 256 threads, persistent over "groups" (one or more whole rays = <=64 sample
@@ -422,7 +422,7 @@ int launch_render_f32(const RenderParams& p_in, int volume_dtype, cudaStream_t s
     p.n_groups = p.groups_per_frame * p.batch;
     const size_t smem = f32::smem_bytes(p.rays_per_group, S);
     if (smem > 227 * 1024) { set_error("n_samples=%d needs %zu B of shared memory (> 227 KB)", S, smem); return NB_ERR_UNSUPPORTED; }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = kGridSMs;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = p.n_groups < sms ? p.n_groups : sms;
@@ -442,7 +442,7 @@ int launch_render_f32(const RenderParams& p_in, int volume_dtype, cudaStream_t s
 
 int launch_density_f32(const RenderParams& p, int volume_dtype, const float* pts, int n_points, float* sigma, cudaStream_t stream) {
     const size_t smem = ((size_t)f32::TP * f32::LDX + (size_t)f32::TP * f32::LDY + 2 * f32::KC * 256 + f32::TP * 3) * 4;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = kGridSMs;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int tiles = ((n_points + f32::TP - 1) / f32::TP) * p.batch;

@@ -7,28 +7,14 @@
 //                                Layer 0 consumes the features coarse level first, so a class-c tile runs only the leading
 //                                2 / 4 / 5 / 6 of its six 64-channel K segments (gather AND MMAs): exact, the skipped
 //                                segments are all zeros.
-//   2. render_tc_list_kernel     the decoder MLP (latent_xyzc.py:91-126) over the list, 128 entries per tile, as a
-//                                warp-specialised tcgen05 pipeline (roles below).
+//   2. render_tc_list_kernel     the decoder MLP (latent_xyzc.py:91-126) over the list, 128 entries per tile, on the Hopper
+//                                tensor cores (wgmma, see below).
 //   3. composite_kernel          raw2outputs (nerf_net_utils.py:6-51), one warp per ray.
 //
-// Decoder pipeline, one persistent CTA per SM.  The two CTAs of a cluster (one TPC) work as a PAIR on 2 x 128 list rows: every
-// MMA is a tcgen05 cta_group::2 instruction of M = 256 issued by the leader CTA, whose B operand (the layer's weights) is split
-// by N halves across the two CTAs' shared memory -- each SM streams only HALF of the weight bytes from L2 (the per-SM ingest of
-// the 1 MB-per-tile weight stream, not the tensor pipe, bounded the single-CTA version) and reads half of them per MMA.
-//   warps  0..15  producers   trilinear gather of the 352 features into a ring of 64-channel layer-0 operand segments
-//   warps 16..19  epilogue    TMEM accumulator -> relu -> (hi, lo) fp16 operand of the next layer, IN PLACE (see below)
-//   warp  20      MMA issuer  leader: the warp walks the schedule, one elected lane issues every tcgen05.mma for the pair (a
-//                             warp-uniform loop: 1-2 SASS instructions per MMA); peer: relays its bulk-copy completions
-//   warp  21      loader      one thread streams this CTA's half of the pre-packed weights through a shared-memory ring
-// (the warp scheduler favours high warp ids, so the latency-critical roles sit above the 16 throughput warps).
-//
-// TMEM (512 columns) is two 256-column regions R0 | R1 that swap roles every layer: layer l accumulates into one region
-// while its A operand (the previous layer's activations) is read from the other.  The epilogue converts an accumulator
-// in place -- the 16 fp32 columns of K-step k become 8 columns of fp16 hi pairs + 8 columns of fp16 lo pairs -- and
-// signals after 32, 64, 128, 192 and 256 columns, so the issuer starts layer l+1 on the first converted columns while the
-// epilogue is still converting the rest: conversion and MMA overlap instead of alternating (what stays exposed of an epilogue
-// is the latency of its first hand-over).  h2 is converted to its hi halves only (rounded to nearest): the colour layer is a
-// 1-pass layer, and sigma = alpha_fc . relu(acc) and the 3-wide rgb head are fp32 dot products in the epilogue registers.
+// Precision: the density path (layers 0-2) runs in the 3-pass mode as A_hi W_hi + A_lo W_hi + A_hi W_lo with fp16 (hi, lo)
+// pairs of both operands and fp32 accumulation (~fp32-accurate), or as A_hi W_hi only in the 1-pass mode.  h2 is converted to
+// its hi halves only (rounded to nearest): the colour layer is a 1-pass layer, and sigma = alpha_fc . relu(acc) and the 3-wide
+// rgb head are fp32 dot products on the accumulator registers.
 //
 // Results do not depend on the (non-deterministic) order of the blocks in the list: a tile row is evaluated
 // independently of its neighbours.  The list and the raw (rgb logits, sigma) records cross HBM once each way.
@@ -39,104 +25,12 @@ namespace nb {
 namespace tcl {
 
 using tcr::Quad;
-using tcr::Tracer;
 
-constexpr int TP = 128;
-// weight ring: NB_NUM_SLOTS slots of NB_SLOT_KB KB (64 KB in all; a 5th / 6th layer-0 segment buffer would be worth more, but
-// does not fit).  A 32 KB slot takes the hi AND lo tiles of a 4-K-step group of an N = 256 layer (12 MMAs per hand-off); 16 KB
-// slots take one plane each (8 / 4 MMAs per hand-off) and let the loader run three hand-offs ahead instead of one.
-#ifndef NB_SLOT_KB
-#define NB_SLOT_KB 32
-#endif
-#ifndef NB_NUM_SLOTS
-#define NB_NUM_SLOTS (64 / NB_SLOT_KB)
-#endif
-// NB_H_FIRST_SPLIT = 1: the first 64-column quarter of an activation region is handed over in two halves (K-steps 0-1, 2-3), so
-// the next layer starts after 32 converted columns: what is exposed of every epilogue is the latency of its FIRST hand-over.
-#ifndef NB_H_FIRST_SPLIT
-#define NB_H_FIRST_SPLIT 1
-#endif
-#ifndef NB_SEG_BUFS
-#define NB_SEG_BUFS 4
-#endif
-constexpr int NUM_SLOTS = NB_NUM_SLOTS;
-constexpr int SLOT_BYTES = NB_SLOT_KB * 1024;
-static_assert(SLOT_BYTES == 32768 || SLOT_BYTES == 16384, "weight slot size");
-constexpr bool SPLIT_PLANES = SLOT_BYTES < 32768;                  // hi and lo tiles of a group travel in separate slots
-#ifndef NB_PROD_WAIT_NS
-#define NB_PROD_WAIT_NS 100
-#endif
-#ifndef NB_GATHER_AHEAD
-#define NB_GATHER_AHEAD 1
-#endif
-constexpr bool GATHER_AHEAD = NB_GATHER_AHEAD;                     // producers gather a segment into registers BEFORE they wait for its buffer
-constexpr unsigned PROD_WAIT_NS = NB_PROD_WAIT_NS;                 // sleep between the producers' probes for a free segment buffer
-constexpr int CHUNK_BYTES = 2048;
-constexpr int SEG_CHUNKS = 8;
+constexpr int TP = 128;                                            // list rows per tile
+constexpr int NT = 256;                                            // two warpgroups
 constexpr int NUM_SEGS = 6;
-// a layer-0 operand chunk (128 rows x 8 k) is 2048 B; the chunks of a segment are laid 2064 B apart (the K-direction
-// core-matrix stride LBO is a free descriptor field), which rotates successive chunks by 4 banks: the 4 rows (two apart) x 8
-// channel quads a producer warp stores per instruction then cover every bank exactly twice (256 B = two wavefronts)
-constexpr int SEG_CHUNK_STRIDE = CHUNK_BYTES + 16;
-constexpr int SEG_BUFS_3PASS = NB_SEG_BUFS;                        // (hi + lo) segment buffers in the 3-pass mode; hi-only mode: twice as many
-constexpr int SEG_RING_BYTES = 2 * SEG_BUFS_3PASS * SEG_CHUNKS * SEG_CHUNK_STRIDE;  // 96.75 KB at 3 buffers
-constexpr int MAX_SEG_BUFS = 2 * SEG_BUFS_3PASS;
-constexpr int PE_CHUNKS = 12;
-// NB_EPI_LOW = 1 (A/B builds): the epilogue warps take the LOWEST warp ids instead of sitting above the producers
-#ifndef NB_EPI_LOW
-#define NB_EPI_LOW 0
-#endif
-constexpr int PROD_WARPS = 16, EPI_WARPS = 4, PROD_WARP0 = NB_EPI_LOW ? 4 : 0, EPI_WARP0 = NB_EPI_LOW ? 0 : 16, MMA_WARP = 20, LOAD_WARP = 21;
-constexpr int NT = (LOAD_WARP + 1) * 32;                          // 704
-constexpr int PTS_PER_GROUP = TP / (PROD_WARPS * 4);
 constexpr int MAXS = 1024;                                         // samples per classification block
-constexpr int CLUSTER = 2;                     // a CTA pair (same TPC) executes every MMA together: tcgen05 cta_group::2, M = 256
 constexpr uint32_t ID_MASK = 0x0FFFFFFFu;                          // list entry .w = frame sample id | level bits << 28
-#ifndef NB_CORNER_BATCH
-#define NB_CORNER_BATCH 4
-#endif
-constexpr int CORNER_BATCH = NB_CORNER_BATCH;                      // corner loads in flight per thread and batch
-constexpr int L3_SPLIT = SPLIT_PLANES ? 8 : 11;                    // layer-3 K-steps per ring slot (2 KB per step and CTA)
-constexpr int HSPLIT = NB_H_FIRST_SPLIT ? 1 : 0;                   // extra hand-over barrier for the first half of quarter 0
-constexpr int HEAD_FLOATS = kHidden + 4 + 3 * kColor + 4;           // alpha_fc (256 + bias) and rgb_fc (3 x 128 + bias), fp32, resident
-constexpr int HALF_TILE_BYTES = kHalfTile256 * 2;                  // one K-step of an N = 256 layer, this CTA's 128 rows (4 KB)
-constexpr int L3_TILE_BYTES = kHalfTile3 * 2;                      // one K-step of layer 3, this CTA's 64 rows (2 KB)
-
-// shared-memory map (bytes)
-constexpr int OFF_SEG = 0;
-constexpr int OFF_ONES = OFF_SEG + SEG_RING_BYTES;
-constexpr int OFF_PE = OFF_ONES + 2 * CHUNK_BYTES;
-constexpr int OFF_RING = OFF_PE + PE_CHUNKS * CHUNK_BYTES;
-constexpr int OFF_HEAD = OFF_RING + NUM_SLOTS * SLOT_BYTES;        // [alpha_w 256 | alpha_b 4 | rgb_w 3 x 128 | rgb_b 4] floats
-constexpr int OFF_XF = OFF_HEAD + HEAD_FLOATS * 4;                 // FrameXf
-constexpr int OFF_SCHED = OFF_XF + 128;                            // tile schedule of the frame (class counts and first tiles)
-constexpr int OFF_BAR = OFF_SCHED + 64;
-// W_FULL[slot]: this CTA's bulk copy landed (transaction bytes + the loader's arrival) AND, on the leader, the peer's did (a
-// second arrival, relayed by the peer: a bulk copy can only signal an mbarrier of its destination CTA).  SEG_FULL / H_READY
-// (leader only): producers / epilogue warps of BOTH CTAs arrive (the peer's remotely).  W_EMPTY / SEG_EMPTY / ACC_FULL: the
-// leader's tcgen05.commit, multicast to both CTAs.
-enum { BAR_W_FULL = 0, BAR_W_EMPTY = NUM_SLOTS, BAR_SEG_FULL = 2 * NUM_SLOTS, BAR_SEG_EMPTY = 2 * NUM_SLOTS + MAX_SEG_BUFS,
-       BAR_ACC_FULL = 2 * NUM_SLOTS + 2 * MAX_SEG_BUFS /* x2, see below */, BAR_H_READY = BAR_ACC_FULL + 2 /* one per hand-over */,
-       NUM_BARS = BAR_H_READY + 4 + HSPLIT };
-// hand-over barrier of the columns holding K-step k of an activation region: one per 64 columns (4 K-steps); with HSPLIT the
-// first quarter is two hand-overs (K-steps 0-1 -> [0], 2-3 -> [1], then one per quarter)
-__host__ __device__ constexpr int h_bar_of_kstep(int k) { return HSPLIT ? (k < 2 ? 0 : k < 4 ? 1 : (k >> 2) + 1) : (k >> 2); }
-__host__ __device__ constexpr bool h_last_kstep(int k) { return (k & 3) == 3 || (HSPLIT && k == 1); }   // k closes its hand-over
-// ACC_FULL alternates between two barriers (layers 0 / 2 -> [0], layers 1 / 3 -> [1]): the issuer can run a whole layer 0 of
-// the next tile ahead of the epilogue, and with one barrier it could complete two phases before the epilogue looked at the first.
-constexpr int OFF_TMEM = OFF_BAR + NUM_BARS * 8;
-constexpr int SMEM_BYTES = OFF_TMEM + 16;
-static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-static_assert(OFF_RING % 128 == 0 && OFF_PE % 128 == 0 && OFF_HEAD % 16 == 0, "operand alignment");
-
-// TMEM: two 256-column regions; K-step k of an activation operand occupies columns [16k, 16k+8) (hi) and [16k+8, 16k+16) (lo)
-constexpr uint32_t TM_R0 = 0, TM_R1 = 256;     // (layer 3 accumulates its 128 colour columns into R1[0,128))
-// weight-ring pushes of one tile (the loader issues them, the peer's relay forwards their completions): layer 0 of a class with
-// `l0_ksteps` K-steps, layers 1 / 2, layer 3
-__host__ __device__ constexpr int pushes_per_tile(int l0_ksteps, int passes) {
-    const int planes = (SPLIT_PLANES && passes == 3) ? 2 : 1;
-    return ((l0_ksteps + 3) / 4) * planes + 1 + 2 * ((kKsL12 / 4) * planes + 1) + (kStepsL3 + L3_SPLIT - 1) / L3_SPLIT;
-}
 
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
@@ -250,64 +144,73 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 }
 
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
+// One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  Two warpgroups each own 64 rows of a tile and
+// issue the wgmma for them; the B operand (the layer's weights) is streamed through a two-slot shared-memory ring by bulk
+// copies (thread 0 issues, an mbarrier with transaction count signals), one push = two K-steps of both N halves.
+//   activations   the ACT planes hold the current layer's A operand as fp16 (hi plane, and in the 3-pass mode the lo plane):
+//                 during layer 0 a ring of four gathered 64-channel feature segments, then h0 / h1 / h2 (written by the
+//                 epilogue straight from the accumulator registers), and in layer 3 the per-point tile in the lo plane.
+//   gather        every thread gathers: segment s + 1 is gathered while the MMAs of segment s run.
+//   accumulators  fp32 in registers (two m64n128 halves per warpgroup), started from the fp32 bias of the layer.
+constexpr int CHUNK_STRIDE = TP * 16 + 16;                         // K-chunk stride (LBO) of an ACT plane: 16 bytes of padding
+                                                                   // rotate successive chunks by 4 banks for the gather's stores
+constexpr int ACT_CHUNKS = kHidden / 8;
+constexpr int PLANE_BYTES = ACT_CHUNKS * CHUNK_STRIDE;             // 66048
+constexpr int SEG_BUFS = 4;                                        // layer-0 segment ring inside the ACT planes
+constexpr int SLOT_BYTES = 32768, NUM_SLOTS = 2;
+constexpr int TILE256 = kHalfTile256 * 2;                          // one K-step, one N half (128 rows) of an N = 256 layer: 4 KB
+constexpr int TILE3 = kHalfTile3 * 2;                              // one K-step, one N half (64 rows) of layer 3: 2 KB
+constexpr int L3_PUSH = 8;                                         // layer-3 K-steps per push
+constexpr int HEAD_FLOATS = kHidden + 4 + 3 * kColor + 4 + 3 * kHidden;   // alpha_fc, rgb_fc, then the biases of fc_0..fc_2, fp32
+constexpr int H_ALPHA = 0, H_RGBW = kHidden + 4, H_RGBB = H_RGBW + 3 * kColor, H_B0 = H_RGBB + 4;
+constexpr int OFF_HI = 0, OFF_LO = PLANE_BYTES;
+constexpr int OFF_RING = 2 * PLANE_BYTES;
+constexpr int OFF_HEAD = OFF_RING + NUM_SLOTS * SLOT_BYTES;
+constexpr int OFF_XF = OFF_HEAD + HEAD_FLOATS * 4;
+constexpr int OFF_SCHED = OFF_XF + 128;
+constexpr int OFF_ROWS = OFF_SCHED + 64;                           // the tile's list entries (float4 per row)
+constexpr int OFF_BAR = OFF_ROWS + TP * 16;
+constexpr int SMEM_BYTES = OFF_BAR + NUM_SLOTS * 8;
+static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+static_assert(OFF_RING % 128 == 0 && OFF_HEAD % 16 == 0 && OFF_ROWS % 16 == 0 && OFF_BAR % 8 == 0, "alignment");
+
+// weight pushes of a tile whose layer 0 runs l0_ksteps K-steps: layer 0 and layers 1 / 2 two K-steps each, layer 3 in groups of L3_PUSH
+__host__ __device__ constexpr int pushes_per_tile(int l0_ksteps) {
+    return l0_ksteps / 2 + 2 * (kKsL12 / 2) + (kStepsL3 + L3_PUSH - 1) / L3_PUSH;
+}
+
+__device__ __forceinline__ uint32_t act_off(int row, int k) {      // byte offset of element (row, k) in an ACT plane
+    return (uint32_t)((k >> 3) * CHUNK_STRIDE + (row >> 3) * 128 + (row & 7) * 16 + (k & 7) * 2);
+}
+
 template <int NP, typename VT>
 __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_constant__ RenderParams P) {
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + OFF_TMEM);
     FrameXf* xf = reinterpret_cast<FrameXf*>(smem + OFF_XF);
+    float* head = reinterpret_cast<float*>(smem + OFF_HEAD);
+    float4* rows = reinterpret_cast<float4*>(smem + OFF_ROWS);
     const int tid = threadIdx.x, lane = tid & 31;
-    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // (the shuffle tells ptxas the role dispatch is warp-uniform)
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    const int wg = warp >> 2;                                       // warpgroup: rows [64 wg, 64 wg + 64) of a tile
     const int S = P.n_samples;
-    constexpr int NUM_SEG_BUFS = (NP == 3) ? SEG_BUFS_3PASS : 2 * SEG_BUFS_3PASS;
-    constexpr int SEG_BYTES = SEG_RING_BYTES / NUM_SEG_BUFS;
+    const uint32_t s_hi = tc::smem_u32(smem + OFF_HI), s_lo = tc::smem_u32(smem + OFF_LO), s_ring = tc::smem_u32(smem + OFF_RING);
 
-    if (warp == MMA_WARP) tc::tmem_alloc_pair<512>(tmem_slot);        // the same warp of both CTAs
-    if (tid == LOAD_WARP * 32) {
-        const bool lead = tc::cluster_ctarank() == 0;
-        for (int i = 0; i < NUM_SLOTS; ++i) {
-            tc::mbar_init(&bars[BAR_W_FULL + i], lead ? 2 : 1);      // the leader's also counts the peer's relayed completion
-            tc::mbar_init(&bars[BAR_W_EMPTY + i], 1);
-        }
-        for (int i = 0; i < NUM_SEG_BUFS; ++i) { tc::mbar_init(&bars[BAR_SEG_FULL + i], CLUSTER * PROD_WARPS); tc::mbar_init(&bars[BAR_SEG_EMPTY + i], 1); }
-        tc::mbar_init(&bars[BAR_ACC_FULL], 1);
-        tc::mbar_init(&bars[BAR_ACC_FULL + 1], 1);
-        for (int i = 0; i < 4 + HSPLIT; ++i) tc::mbar_init(&bars[BAR_H_READY + i], CLUSTER * EPI_WARPS);
+    if (tid == 0) {
+        for (int i = 0; i < NUM_SLOTS; ++i) tc::mbar_init(&bars[i], 1);
         tc::fence_mbar_init();
     }
-    const int pwarp = warp - PROD_WARP0, ptid = tid - PROD_WARP0 * 32;       // producer-relative ids
-    const bool is_producer = pwarp >= 0 && pwarp < PROD_WARPS;
-    if (is_producer) {
-        if (ptid < TP) {
-            unsigned char* o = smem + OFF_ONES;
-            *reinterpret_cast<uint4*>(o + (ptid >> 3) * 128 + (ptid & 7) * 16) = make_uint4(0x3C003C00u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(o + CHUNK_BYTES + (ptid >> 3) * 128 + (ptid & 7) * 16) = make_uint4(0u, 0u, 0u, 0u);
+    load_frame_xf(P, xf, tid);
+    for (int i = tid; i < HEAD_FLOATS; i += NT) {
+        float v;
+        if (i < H_RGBW) v = __ldg(P.wf32 + oAlphaW + i);                       // [alpha_w | alpha_b]
+        else if (i < H_B0) v = __ldg(P.wf32 + oRgbW + (i - H_RGBW));            // [rgb_w | rgb_b]
+        else {
+            const int j = i - H_B0, l = j / kHidden, n = j % kHidden;
+            v = __ldg(P.wf32 + (l == 0 ? oB0 : l == 1 ? oB1 : oB2) + n);
         }
-        load_frame_xf(P, xf, ptid);
-        // the two narrow heads, fp32: alpha_fc (latent_xyzc.py:104) and rgb_fc (:124) are applied by the epilogue
-        float* head = reinterpret_cast<float*>(smem + OFF_HEAD);
-        for (int i = ptid; i < HEAD_FLOATS; i += PROD_WARPS * 32) {
-            const int j = i - (kHidden + 4);
-            head[i] = i < kHidden + 4 ? __ldg(P.wf32 + oAlphaW + i) : __ldg(P.wf32 + oRgbW + j);     // [alpha_w | alpha_b] / [rgb_w | rgb_b]
-        }
-        tc::fence_proxy_async();
+        head[i] = v;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    tc::cluster_sync_all();                        // both CTAs' mbarriers are initialised before anything arrives on them
-    const uint32_t crank = tc::cluster_ctarank();
-    const bool leader = crank == 0;                // the leader's MMA thread issues for the pair
-    constexpr uint16_t CMASK = (1u << CLUSTER) - 1;
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t leader_bars = tc::map_to_cta(bars, 0);             // shared::cluster address of the leader's barrier array
-    auto arrive_at_leader = [&](int bar) { tc::mbar_arrive_remote(leader_bars + 8u * (uint32_t)bar); };
-    if (tid == 0 && P.stats) atomicMax(P.frame_clock + 0, ~global_ns());     // min(start) over the CTAs, as max(~start)
-    // The frame's work: per sample class c (heaviest first) ceil(count_c / 128) tiles, rounded up to whole clusters so that the
-    // CTAs of a cluster -- which walk the tiles in lockstep on one shared weight stream -- always work on the same class
-    // (padding tiles have 0 rows).  Every role derives the same static schedule from the four list lengths.
-    // (the schedule lives in shared memory, not in registers: it is read once per tile, and the producers' gather needs every
-    // register it can get for loads in flight)
     struct Sched { unsigned int cnt[4]; int start[4]; int n_tiles; };
     Sched* sched = reinterpret_cast<Sched*>(smem + OFF_SCHED);
     if (tid == 0) {
@@ -316,13 +219,13 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             const unsigned int n = P.list_count[c];                         // written by classify_compact_kernel (previous launch)
             sched->cnt[c] = n;
             sched->start[c] = acc;
-            acc += (int)(((n + TP - 1) / TP + CLUSTER - 1) / CLUSTER * CLUSTER);
+            acc += (int)((n + TP - 1) / TP);
         }
         sched->n_tiles = acc;
+        if (P.stats) atomicMax(P.frame_clock + 0, ~global_ns());            // min(start) over the CTAs, as max(~start)
     }
     __syncthreads();
     const int n_tiles = sched->n_tiles;
-    const int tile0 = (int)(blockIdx.x / CLUSTER) * CLUSTER;
     struct TileRef { int cls, nrows; const float4* ent; };
     auto tile_ref = [&](int tile) {
         TileRef r;
@@ -336,566 +239,344 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         return r;
     };
 
-    // ================================================================== PRODUCERS
-    if (is_producer) {
-        const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
-        const int grp = pwarp * 4 + (lane >> 3);
-        const int t = lane & 7;
-        uint32_t gseg = 0;                             // segments produced so far (ring position)
-        Tracer tr;
-        tr.init((pwarp == 0 && lane == 0) ? P.trace : nullptr, 0);
-        const uint32_t seg_base = tc::smem_u32(smem + OFF_SEG);
-        // An 8-lane group owns the ADJACENT tile rows 2 grp and 2 grp + 1 (a warp: 8 consecutive rows); lane t owns channels
-        // 4t..4t+3 of every 32-channel unit, so one corner of one row is one contiguous 128-byte (fp32) run.  Consecutive list
-        // entries are the same depth sample of neighbouring rays, a few millimetres apart: at the coarser levels the two rows
-        // usually sit in the same trilinear cell, and the second row then reuses the corner vectors the first one loaded --
-        // the L1 wavefronts of the corner loads, not their latency, bound the gather.
-        const uint32_t so0 = (uint32_t)((t >> 1) * SEG_CHUNK_STRIDE + (grp >> 2) * 128 + (grp & 3) * 32 + (t & 1) * 8);
-        uint32_t real_tiles = 0, real_ksteps = 0;
-        for (int tbase = tile0; tbase < n_tiles; tbase += gridDim.x) {
-            const TileRef tref = tile_ref(tbase + (int)crank);
-            const int nrows = tref.nrows, nseg = class_segments(tref.cls);
-            real_tiles += nrows > 0;
-            real_ksteps += nrows > 0 ? class_ksteps(tref.cls) : 0;
-            // the list entries of this thread's rows: grid coordinates + per-level occupancy bits
-            float gx[PTS_PER_GROUP], gy[PTS_PER_GROUP], gz[PTS_PER_GROUP];
-            uint32_t lvl_bits = 0;                     // bit (4 pp + l): row pp has an occupied cell at level l
+    // ---- the weight stream.  Push j of a tile goes to slot (pc + j) % 2, pc = pushes of the earlier tiles.
+    const unsigned char* seq = reinterpret_cast<const unsigned char*>(P.wf16);
+    auto issue_push = [&](int l0_ksteps, int j, uint32_t gidx) {      // (thread 0)
+        const uint32_t slot = gidx % NUM_SLOTS;
+        unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
+        uint64_t* bar = &bars[slot];
+        const int n0 = l0_ksteps / 2;
+        if (j < n0 + kKsL12) {                                          // layers 0..2: K-steps ks0, ks0 + 1 of both N halves
+            const int layer = j < n0 ? 0 : j < n0 + kKsL12 / 2 ? 1 : 2;
+            const int ks0 = 2 * (layer == 0 ? j : layer == 1 ? j - n0 : j - n0 - kKsL12 / 2);
+            const int nks = layer == 0 ? kKsL0 : kKsL12;
+            const unsigned char* base = seq + 2 * (layer == 0 ? sL0 : layer == 1 ? sL1 : sL2);
+            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * (NP == 3 ? 2 : 1) * 2 * TILE256));
 #pragma unroll
-            for (int pp = 0; pp < PTS_PER_GROUP; ++pp) {
-                const int row = 2 * grp + pp;
-                gx[pp] = gy[pp] = gz[pp] = -4.f;
-                if (row < nrows) {
-                    const float4 e = __ldg(tref.ent + row);
-                    world_to_grid(*xf, e.x, e.y, e.z, gx[pp], gy[pp], gz[pp]);
-                    lvl_bits |= (__float_as_uint(e.w) >> 28) << (4 * pp);
-                }
-            }
-            tr.ev(1);                                   // tile begin
-            // per level and row: byte offset of the cell's low corner (clamped into the volume, see below) and the 8 corner weights
-            uint32_t cbase[PTS_PER_GROUP];
-            float cw[PTS_PER_GROUP][8];
-            bool occ0 = false, occ1 = false, same_cell = false;
-            uint32_t dX = 0, dY = 0, dZ = 0;           // byte strides of the level's x / y / z neighbours
-            const unsigned char* lvl_ptr = nullptr;    // this lane's channels of voxel 0 of the level
-            int cur_lvl = -1;
-            for (int seg = 0; seg < nseg; ++seg, ++gseg) {
-                const uint32_t buf = gseg % NUM_SEG_BUFS;
-                // The gather itself needs no buffer: a segment is gathered and converted INTO REGISTERS first (16 packed words per
-                // thread), and only the 8 shared-memory stores wait for the ring slot.  With four buffers for six segments the
-                // last two of a tile used to start their L2-latency-bound gather (6-7 K cycles) only when the issuer had consumed
-                // segments 0 / 1 -- 3.4 K cycles of every 14 K-cycle layer 0 were exposed (profiles/r02_trace_timeline_h_split.txt)
-                // while the producers sat idle for 6 K cycles before.  This way the ring is one segment deeper than its buffers.
-                if (!GATHER_AHEAD) { tc::mbar_wait_backoff(&bars[BAR_SEG_EMPTY + buf], ((gseg / NUM_SEG_BUFS) & 1) ^ 1, PROD_WAIT_NS); tr.ev(10 + seg); }
-                // this thread's (row, channel quad) slot of the hi plane; the lo plane follows SEG_CHUNKS chunk strides later
-                const uint32_t dst = seg_base + buf * SEG_BYTES + so0;
-                const int nunits = (seg == NUM_SEGS - 1) ? 1 : 2;
-                uint2 hi_w[2][PTS_PER_GROUP], lo_w[2][PTS_PER_GROUP];      // [unit][row]: 4 channels as fp16 (hi, lo) pairs
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int uu = 0; uu < 2; ++uu) {
-                    if (uu >= nunits) continue;
-                    const int unit = 2 * seg + uu;              // coarse level first (nb_layout.h feat_tc_to_orig)
-                    int lvl, c0;
-                    if (unit < 4) { lvl = 3; c0 = unit * 32; }
-                    else if (unit < 8) { lvl = 2; c0 = (unit - 4) * 32; }
-                    else if (unit < 10) { lvl = 1; c0 = (unit - 8) * 32; }
-                    else { lvl = 0; c0 = 0; }
-                    if (lvl != cur_lvl) {
-                        cur_lvl = lvl;
-                        const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-                        lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
-                        dX = (uint32_t)(C * sizeof(VT)); dY = dX * W; dZ = dY * H;
-                        int cell[PTS_PER_GROUP];
+                for (int pl = 0; pl < (NP == 3 ? 2 : 1); ++pl)
+                    tc::bulk_g2s(dst + (2 * h + pl) * 2 * TILE256, base + 2 * pair_step_offset(ks0, pl, h, nks), 2 * TILE256, bar);
+        } else {                                                        // layer 3: steps [g0, g0 + n) of both N halves
+            const int g0 = (j - n0 - kKsL12) * L3_PUSH;
+            const int n = min(L3_PUSH, kStepsL3 - g0), common = min(n, kStepsL3 - 1 - g0);
+            const bool last = g0 + n == kStepsL3;
+            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * n * TILE3));
 #pragma unroll
-                        for (int pp = 0; pp < PTS_PER_GROUP; ++pp) {
-                            Corners cn;
-                            corner_setup(unnormalize(gx[pp], W), unnormalize(gy[pp], H), unnormalize(gz[pp], D), W, H, D, cn);
-                            cell[pp] = (cn.z0 * (H + 2) + cn.y0) * (W + 2) + cn.x0;
-                            // The 8 corners are addressed as (clamped low corner) + constant strides.  A cell that straddles the
-                            // volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted inside by one and
-                            // its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
-                            auto axis = [](int i0, int size, float (&w)[2]) {
-                                if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
-                                if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
-                                if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
-                                return i0;
-                            };
-                            const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
-                            cbase[pp] = (uint32_t)((zc * H + yc) * W + xc) * dX;
-#pragma unroll
-                            for (int c = 0; c < 8; ++c)
-                                cw[pp][c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
-                            if (cn.x0 == -2) cell[pp] = -1 - pp;          // out of the volume altogether (never marked occupied)
-                        }
-                        occ0 = (lvl_bits >> lvl) & 1;
-                        occ1 = (lvl_bits >> (4 + lvl)) & 1;
-                        // same cell => the same 8 corner voxels: row 1 reuses row 0's loads
-                        same_cell = occ0 && occ1 && cell[0] == cell[1];
-                    }
-                    // corner c of the cell = base + (c & 1) dX + ((c >> 1) & 1) dY + (c >> 2) dZ
-                    auto corner_off = [&](uint32_t base, int c) { return base + ((c & 1) ? dX : 0u) + ((c & 2) ? dY : 0u) + ((c & 4) ? dZ : 0u); };
-                    float acc[PTS_PER_GROUP][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-                    const unsigned char* ub = lvl_ptr + (size_t)c0 * sizeof(VT);
-                    if (occ0) {
-#pragma unroll
-                        for (int h = 0; h < 8; h += CORNER_BATCH) {          // corners in batches (register budget)
-                            typename Quad<VT>::raw v[CORNER_BATCH];
-#pragma unroll
-                            for (int c = 0; c < CORNER_BATCH; ++c) v[c] = Quad<VT>::load_bytes(ub + corner_off(cbase[0], h + c));
-#pragma unroll
-                            for (int c = 0; c < CORNER_BATCH; ++c)
-                                if (cw[0][h + c] != 0.f) Quad<VT>::fma(acc[0], v[c], cw[0][h + c]);
-                            if (same_cell) {
-#pragma unroll
-                                for (int c = 0; c < CORNER_BATCH; ++c)
-                                    if (cw[1][h + c] != 0.f) Quad<VT>::fma(acc[1], v[c], cw[1][h + c]);
-                            }
-                        }
-                    }
-                    if (occ1 && !same_cell) {
-#pragma unroll
-                        for (int h = 0; h < 8; h += CORNER_BATCH) {
-                            typename Quad<VT>::raw v[CORNER_BATCH];
-#pragma unroll
-                            for (int c = 0; c < CORNER_BATCH; ++c) v[c] = Quad<VT>::load_bytes(ub + corner_off(cbase[1], h + c));
-#pragma unroll
-                            for (int c = 0; c < CORNER_BATCH; ++c)
-                                if (cw[1][h + c] != 0.f) Quad<VT>::fma(acc[1], v[c], cw[1][h + c]);
-                        }
-                    }
-#pragma unroll
-                    for (int pp = 0; pp < PTS_PER_GROUP; ++pp) {
-                        const float (&a)[4] = acc[pp];
-                        if (NP == 3) {
-                            // (hi, lo) split with a truncated hi: the residual is exact and costs one LOP3 + half an FADD2 a value
-                            hi_w[uu][pp].x = tc::cvt_rz_f16x2(a[0], a[1]); hi_w[uu][pp].y = tc::cvt_rz_f16x2(a[2], a[3]);
-                            float r0, r1, r2, r3;
-                            tc::trunc_residual2(a[0], a[1], r0, r1);
-                            tc::trunc_residual2(a[2], a[3], r2, r3);
-                            lo_w[uu][pp].x = tc::cvt_f16x2(r0, r1); lo_w[uu][pp].y = tc::cvt_f16x2(r2, r3);
-                        } else {
-                            hi_w[uu][pp].x = tc::cvt_f16x2(a[0], a[1]); hi_w[uu][pp].y = tc::cvt_f16x2(a[2], a[3]);
-                        }
-                    }
-                }
-                if (GATHER_AHEAD) { tc::mbar_wait_backoff(&bars[BAR_SEG_EMPTY + buf], ((gseg / NUM_SEG_BUFS) & 1) ^ 1, PROD_WAIT_NS); tr.ev(10 + seg); }
-#pragma unroll
-                for (int uu = 0; uu < 2; ++uu) {
-                    if (uu >= nunits) continue;
-#pragma unroll
-                    for (int pp = 0; pp < PTS_PER_GROUP; ++pp) {
-                        const uint32_t so = dst + (uint32_t)(uu * 4 * SEG_CHUNK_STRIDE + pp * 16);   // K-major core-matrix layout
-                        tcr::sts_v2(so, hi_w[uu][pp]);
-                        if (NP == 3) tcr::sts_v2(so + SEG_CHUNKS * SEG_CHUNK_STRIDE, lo_w[uu][pp]);
-                    }
-                }
-                tc::fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) arrive_at_leader(BAR_SEG_FULL + buf);
-                tr.ev(20 + seg);
+            for (int h = 0; h < 2; ++h) {
+                unsigned char* d = dst + h * (SLOT_BYTES / 2);
+                tc::bulk_g2s(d, seq + 2 * (sL3 + pair_l3_offset(g0, h)), common * TILE3, bar);
+                if (last)                                               // the per-frame step 21 (it carries the frame's bias)
+                    tc::bulk_g2s(d + common * TILE3, reinterpret_cast<const unsigned char*>(P.wframe) + ((size_t)P.frame * 2 + h) * TILE3,
+                                 TILE3, bar);
             }
         }
-        if (ptid == 0 && P.stats) {
-            atomicAdd(P.stats + 0, (unsigned long long)real_tiles);
-            atomicAdd(P.stats + 4, (unsigned long long)real_ksteps);
-            if (blockIdx.x == 0) atomicAdd(P.stats + 1, (unsigned long long)sched->cnt[0] + sched->cnt[1] + sched->cnt[2] + sched->cnt[3]);
+    };
+
+    // this thread's accumulator fragment: rows r0 and r0 + 8 of the tile, columns 8 c + cq + {0, 1} of each 128-column half
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    float acc0[64], acc1[64];                                      // N halves [0, 128) and [128, 256)
+    auto init_bias = [&](const float* b) {
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            const float2 v0 = *reinterpret_cast<const float2*>(b + 8 * c + cq), v1 = *reinterpret_cast<const float2*>(b + 128 + 8 * c + cq);
+            acc0[4 * c] = v0.x; acc0[4 * c + 1] = v0.y; acc0[4 * c + 2] = v0.x; acc0[4 * c + 3] = v0.y;
+            acc1[4 * c] = v1.x; acc1[4 * c + 1] = v1.y; acc1[4 * c + 2] = v1.x; acc1[4 * c + 3] = v1.y;
         }
-    }
-    // ================================================================== LOADER (each CTA streams ITS half of every weight step)
-    else if (warp == LOAD_WARP) {
-        if (lane == 0) {
-            uint32_t cnt = 0;
-            Tracer tr;
-            tr.init(P.trace, 3);
-            const unsigned char* seq = reinterpret_cast<const unsigned char*>(P.wf16);
-            auto push = [&](const unsigned char* src, uint32_t bytes, const unsigned char* src2 = nullptr, uint32_t bytes2 = 0) {
-                const uint32_t slot = cnt % NUM_SLOTS, round = cnt / NUM_SLOTS;
-                unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
-                tr.ev(2);
-                tc::mbar_wait(&bars[BAR_W_EMPTY + slot], (round & 1) ^ 1);
-                tr.ev(3);
-                tc::mbar_arrive_expect_tx(&bars[BAR_W_FULL + slot], bytes + bytes2);
-                tc::bulk_g2s(dst, src, bytes, &bars[BAR_W_FULL + slot]);
-                if (bytes2) tc::bulk_g2s(dst + bytes, src2, bytes2, &bars[BAR_W_FULL + slot]);
-                ++cnt;
-            };
-            for (int tbase = tile0; tbase < n_tiles; tbase += gridDim.x) {
-                tr.ev(1);
-                const int l0_ksteps = class_ksteps(tile_ref(tbase).cls);      // both CTAs of the pair: same class
-                for (int layer = 0; layer < 3; ++layer) {
-                    const int nks = layer == 0 ? kKsL0 : kKsL12;
-                    const unsigned char* base = seq + 2 * (layer == 0 ? sL0 : layer == 1 ? sL1 : sL2);
-                    for (int g0 = 0; g0 < (layer == 0 ? l0_ksteps : nks); g0 += 4) {
-                        const int gs = (nks - g0) < 4 ? (nks - g0) : 4;
-                        // this CTA's gs hi tiles (+ gs lo tiles in the 3-pass mode) are contiguous in the stream: one slot, or two
-                        const unsigned char* grp = base + 2 * pair_group_offset(g0, (int)crank, nks);
-                        if (SPLIT_PLANES) {
-                            push(grp, gs * HALF_TILE_BYTES);
-                            if (NP == 3) push(grp + gs * HALF_TILE_BYTES, gs * HALF_TILE_BYTES);
-                        } else {
-                            push(grp, (NP == 3 ? 2 : 1) * gs * HALF_TILE_BYTES);
-                        }
-                    }
-                    push(base + 2 * pair_bias_offset((int)crank, nks), HALF_TILE_BYTES);
-                }
-                const unsigned char* l3 = seq + 2 * (sL3 + pair_l3_offset(0, (int)crank));
-                const unsigned char* fr = reinterpret_cast<const unsigned char*>(P.wframe) + ((size_t)P.frame * 2 + crank) * L3_TILE_BYTES;
-                for (int g0 = 0; g0 < kStepsL3; g0 += L3_SPLIT) {     // steps 0..20 from the common stream, the per-frame step 21 last
-                    const int common = min(L3_SPLIT, kStepsL3 - 1 - g0), last = g0 + L3_SPLIT >= kStepsL3;
-                    if (common > 0) push(l3 + (size_t)g0 * L3_TILE_BYTES, common * L3_TILE_BYTES, last ? fr : nullptr, last ? L3_TILE_BYTES : 0);
-                    else push(fr, L3_TILE_BYTES);
-                }
+    };
+    const uint32_t wg_rows = (uint32_t)(wg * 8 * 128);              // this warpgroup's first 8-row group in an ACT plane
+    // two K-steps of a 256 -> 256 layer from the slot at `slot`: A K-step ka, ka + 1 (ACT chunk 2 ka)
+    auto mma256 = [&](uint32_t slot, int ka) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            const uint64_t a_hi = tc::make_smem_desc(s_hi + wg_rows + 2 * (ka + j) * CHUNK_STRIDE, CHUNK_STRIDE, 128);
+            const uint64_t a_lo = tc::make_smem_desc(s_lo + wg_rows + 2 * (ka + j) * CHUNK_STRIDE, CHUNK_STRIDE, 128);
+            const uint64_t b0h = tc::make_smem_desc(slot + 0 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
+            const uint64_t b0l = tc::make_smem_desc(slot + 1 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
+            const uint64_t b1h = tc::make_smem_desc(slot + 2 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
+            const uint64_t b1l = tc::make_smem_desc(slot + 3 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
+            tc::wgmma_m64n128k16_f16(acc0, a_hi, b0h, true);
+            tc::wgmma_m64n128k16_f16(acc1, a_hi, b1h, true);
+            if (NP == 3) {                                          // A_lo W_hi + A_hi W_lo
+                tc::wgmma_m64n128k16_f16(acc0, a_lo, b0h, true);
+                tc::wgmma_m64n128k16_f16(acc1, a_lo, b1h, true);
+                tc::wgmma_m64n128k16_f16(acc0, a_hi, b0l, true);
+                tc::wgmma_m64n128k16_f16(acc1, a_hi, b1l, true);
             }
         }
-    }
-    // ================================================================== MMA ISSUER (leader) / COPY RELAY (peer)
-    else if (warp == MMA_WARP) {
-        if (lane == 0 && !leader) {
-            // The leader must know that THIS CTA's half of a weight slot has landed, but a bulk copy can only signal an mbarrier
-            // of its destination CTA: this thread watches the local W_FULL barriers in push order and forwards each completion
-            // as the second arrival of the leader's W_FULL barrier of the same slot.
-            uint32_t cnt = 0;
-            for (int tbase = tile0; tbase < n_tiles; tbase += gridDim.x) {
-                const int pushes = pushes_per_tile(class_ksteps(tile_ref(tbase).cls), NP);
-                for (int i = 0; i < pushes; ++i, ++cnt) {
-                    const uint32_t slot = cnt % NUM_SLOTS;
-                    tc::mbar_wait(&bars[BAR_W_FULL + slot], (cnt / NUM_SLOTS) & 1);
-                    arrive_at_leader(BAR_W_FULL + slot);
-                }
-            }
-        }
-        if (leader) {
-            // THE WHOLE WARP walks the schedule and waits on the barriers; the MMAs and commits sit in elect_one() blocks (see
-            // nb_tc_ptx.cuh): every value of the loop is warp-uniform, so an MMA costs the warp 1-2 instructions instead of the
-            // ~14 of the single-lane form.  The issuer shares its scheduler with four gathering producer warps, and with the
-            // single-lane form its own instruction stream -- 200+ cycles per MMA while the gather ran, 400 in the rolled layer-3
-            // loop (profiles/r02_trace_timeline_final.txt) -- not the tensor pipe bounded layers 1 and 3.
-            uint32_t cnt = 0, hphase = 0, gseg = 0;
-            constexpr uint32_t FULL = 0xffffffffu;
-            constexpr uint32_t ID256 = tc::make_idesc_f16(256, 256), ID3 = tc::make_idesc_f16(256, kN3);   // M = 256: the pair's two tiles
-            constexpr uint32_t DHI = tc::desc_hi(128);                          // 8-row groups 128 B apart, every operand
-            // low descriptor words (start address | K-chunk stride) of the operand arrays; tiles / K-steps are 16-byte-unit adds
-            const uint32_t seg_lo = tc::desc_lo(tc::smem_u32(smem + OFF_SEG), SEG_CHUNK_STRIDE);
-            const uint32_t pe_lo = tc::desc_lo(tc::smem_u32(smem + OFF_PE), CHUNK_BYTES);
-            const uint32_t ones_lo = tc::desc_lo(tc::smem_u32(smem + OFF_ONES), CHUNK_BYTES);
-            const uint32_t ring256_lo = tc::desc_lo(tc::smem_u32(smem + OFF_RING), 128 * 16);      // 128-row half tiles of an N = 256 layer
-            const uint32_t ring3_lo = tc::desc_lo(tc::smem_u32(smem + OFF_RING), (kN3 / 2) * 16);  // 64-row half tiles of layer 3
-            constexpr uint32_t SLOT_U = SLOT_BYTES >> 4, T256_U = HALF_TILE_BYTES >> 4, T3_U = L3_TILE_BYTES >> 4;
-            constexpr uint32_t SEG_U = (uint32_t)SEG_BYTES >> 4, SEG_LO_U = (SEG_CHUNKS * SEG_CHUNK_STRIDE) >> 4;
-            constexpr uint32_t KS_SEG_U = (2 * SEG_CHUNK_STRIDE) >> 4, KS_A_U = (2 * CHUNK_BYTES) >> 4;
-            static_assert((2 * SEG_CHUNK_STRIDE) % 16 == 0 && SEG_BYTES % 16 == 0 && (SEG_CHUNKS * SEG_CHUNK_STRIDE) % 16 == 0, "descriptor units");
-            const uint32_t tm = __shfl_sync(FULL, tmem, 0);                     // (read from shared memory: tell ptxas it is uniform)
-            Tracer tr;
-            tr.init(lane == 0 ? P.trace : nullptr, 1);
-            // The tensor pipe queues only a few instructions, so whatever the issuer does between two MMAs beyond ~the queue's
-            // worth of cycles is a bubble.  Hence ONE barrier per weight slot, and the barriers of the NEXT group are probed
-            // (non-blocking, made warp-uniform by a vote) right after the current group's MMAs; only a failed probe is waited for.
-            bool slot_seen = false;                          // the next slot's phase was already observed complete
-            auto probe_slot = [&]() {
-                slot_seen = __all_sync(FULL, tc::mbar_test(&bars[BAR_W_FULL + cnt % NUM_SLOTS], (cnt / NUM_SLOTS) & 1));
-            };
-            auto wait_slot = [&]() {                         // -> the slot's offset in descriptor units
-                const uint32_t slot = cnt % NUM_SLOTS;
-                if (!slot_seen) { tr.ev(40); tc::mbar_wait(&bars[BAR_W_FULL + slot], (cnt / NUM_SLOTS) & 1); tr.ev(42); }
-                slot_seen = false;
-                tc::tc_fence_after();
-                return slot * SLOT_U;
-            };
-            // (inside an elect block) both CTAs' loaders reuse the slot once the MMAs issued so far are done
-            auto commit_slot = [&]() { tc::mma_commit_pair(&bars[BAR_W_EMPTY + cnt % NUM_SLOTS], CMASK); };
-            // the epilogues of BOTH CTAs have converted columns [64 g, 64 g + 64) of the current activation region (K-steps 4g..4g+3)
-            uint32_t h_seen = 0;                             // bit g: chunk g's phase was already observed complete
-            auto probe_h = [&](int g) {
-                if (__all_sync(FULL, tc::mbar_test(&bars[BAR_H_READY + g], (hphase >> g) & 1))) h_seen |= 1u << g;
-            };
-            auto wait_h = [&](int g) {
-                if (!((h_seen >> g) & 1)) { tr.ev(44); tc::mbar_wait_cluster(&bars[BAR_H_READY + g], (hphase >> g) & 1); tr.ev(45); }
-                h_seen &= ~(1u << g);
-                hphase ^= 1u << g;
-                tc::tc_fence_after();
-            };
-            // one layer-0 segment of NKS K-steps against its hi weight tiles at `b` (A_hi W_hi, A_lo W_hi) / its lo tiles (A_hi W_lo)
-            auto l0_hi = [&](auto nks_c, uint32_t a_hi, uint32_t b, bool first) {
-                constexpr int NKS = decltype(nks_c)::value;
-#pragma unroll
-                for (int ks = 0; ks < NKS; ++ks) {
-                    tc::mma_ss_pair_w(tm + TM_R0, a_hi + ks * KS_SEG_U, b + ks * T256_U, DHI, ID256, ks != 0 || !first);
-                    if (NP == 3) tc::mma_ss_pair_w(tm + TM_R0, a_hi + SEG_LO_U + ks * KS_SEG_U, b + ks * T256_U, DHI, ID256, true);
-                }
-            };
-            auto l0_lo = [&](auto nks_c, uint32_t a_hi, uint32_t b) {
-                constexpr int NKS = decltype(nks_c)::value;
-#pragma unroll
-                for (int ks = 0; ks < NKS; ++ks) tc::mma_ss_pair_w(tm + TM_R0, a_hi + ks * KS_SEG_U, b + ks * T256_U, DHI, ID256, true);
-            };
-            // the bias step of an N = 256 layer (a column of ones x [hi(b), lo(b)]) and the layer's accumulator barrier
-            auto bias_and_commit = [&](uint32_t rout, int acc_bar) {
-                const uint32_t b = ring256_lo + wait_slot();
-                if (tc::elect_one()) {
-                    tc::mma_ss_pair_w(tm + rout, ones_lo, b, DHI, ID256, true);
-                    commit_slot();
-                    tc::mma_commit_pair(&bars[BAR_ACC_FULL + acc_bar], CMASK);
-                }
-                ++cnt;
-            };
-            // K-steps [k0, k1) of a 256 -> 256 layer against the hi weight tiles of its group: A_hi W_hi (+ A_lo W_hi)
-            auto hi_steps = [&](uint32_t rin, uint32_t rout, uint32_t b, int k0, int k1) {
-#pragma unroll
-                for (int k = k0; k < k1; ++k) {
-                    const uint32_t a = tm + rin + 16 * k;
-                    tc::mma_ts_pair_w(tm + rout, a, b + (k & 3) * T256_U, DHI, ID256, k != 0);
-                    if (NP == 3) tc::mma_ts_pair_w(tm + rout, a + 8, b + (k & 3) * T256_U, DHI, ID256, true);
-                }
-            };
-            // a 256 -> 256 layer: A = activations in region `rin` (TMEM), accumulator = region `rout`
-            auto layer256 = [&](uint32_t rin, uint32_t rout, int code) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    wait_h(h_bar_of_kstep(4 * g));
-                    if (g == 0) tr.ev(30 + code);
-                    uint32_t b = ring256_lo + wait_slot();                      // [4 hi tiles | 4 lo tiles], or one plane per slot
-                    if (HSPLIT && g == 0) {                                     // quarter 0 arrives in two halves
-                        if (tc::elect_one()) hi_steps(rin, rout, b, 0, 2);
-                        wait_h(1);
-                    }
-                    if (tc::elect_one()) {
-                        hi_steps(rin, rout, b, (HSPLIT && g == 0) ? 2 : 4 * g, 4 * g + 4);
-                        if (SPLIT_PLANES || NP != 3) commit_slot();
-                    }
-                    if (g < 3) probe_h(h_bar_of_kstep(4 * g + 4));              // (the probes ride under the MMAs just queued)
-                    if (NP == 3) {
-                        if (SPLIT_PLANES) { ++cnt; b = ring256_lo + wait_slot() - 4 * T256_U; }   // the lo tiles' own slot
-                        if (tc::elect_one()) {
-#pragma unroll
-                            for (int i = 0; i < 4; ++i)                         // A_hi W_lo
-                                tc::mma_ts_pair_w(tm + rout, tm + rin + 16 * (4 * g + i), b + (4 + i) * T256_U, DHI, ID256, true);
-                            commit_slot();
-                        }
-                    }
-                    ++cnt;
-                    probe_slot();
-                }
-                bias_and_commit(rout, code & 1);
-                tr.ev(20 + code);
-            };
-            for (int tbase = tile0; tbase < n_tiles; tbase += gridDim.x) {
-                tr.ev(1);
-                // ---- layer 0: A = gathered feature segments (shared memory of each CTA), accumulator R0.  R0 held the previous
-                // tile's h2, whose last reader (its layer 3) was issued before: the tensor pipe executes in issue order.
-                const int nseg = __shfl_sync(FULL, class_segments(tile_ref(tbase).cls), 0);
-                for (int seg = 0; seg < nseg; ++seg, ++gseg) {
-                    const uint32_t buf = gseg % NUM_SEG_BUFS;
-                    tc::mbar_wait_cluster(&bars[BAR_SEG_FULL + buf], (gseg / NUM_SEG_BUFS) & 1);
-                    tc::tc_fence_after();
-                    tr.ev(10 + seg);
-                    const uint32_t a_hi = seg_lo + buf * SEG_U;                 // (3-pass: the lo plane follows SEG_LO_U units later)
-                    const bool short_seg = seg == NUM_SEGS - 1;                 // level 0: 32 channels = 2 K-steps
-                    uint32_t b = ring256_lo + wait_slot();
-                    if (SPLIT_PLANES && NP == 3) {                              // hi tiles, then the lo tiles from their own slot
-                        if (tc::elect_one()) {
-                            if (short_seg) l0_hi(std::integral_constant<int, 2>{}, a_hi, b, false);
-                            else l0_hi(std::integral_constant<int, 4>{}, a_hi, b, seg == 0);
-                            commit_slot();
-                        }
-                        ++cnt;
-                        b = ring256_lo + wait_slot();
-                        if (tc::elect_one()) {
-                            if (short_seg) l0_lo(std::integral_constant<int, 2>{}, a_hi, b);
-                            else l0_lo(std::integral_constant<int, 4>{}, a_hi, b);
-                            commit_slot();
-                            tc::mma_commit_pair(&bars[BAR_SEG_EMPTY + buf], CMASK);
-                        }
-                    } else if (tc::elect_one()) {
-                        if (short_seg) { l0_hi(std::integral_constant<int, 2>{}, a_hi, b, false); if (NP == 3) l0_lo(std::integral_constant<int, 2>{}, a_hi, b + 2 * T256_U); }
-                        else { l0_hi(std::integral_constant<int, 4>{}, a_hi, b, seg == 0); if (NP == 3) l0_lo(std::integral_constant<int, 4>{}, a_hi, b + 4 * T256_U); }
-                        commit_slot();
-                        tc::mma_commit_pair(&bars[BAR_SEG_EMPTY + buf], CMASK);
-                    }
-                    ++cnt;
-                    probe_slot();
-                }
-                bias_and_commit(TM_R0, 0);
-                tr.ev(20);
-                layer256(TM_R0, TM_R1, 1);       // layer 1: h0 (R0) -> R1
-                layer256(TM_R1, TM_R0, 2);       // layer 2: h1 (R1) -> R0
-                // ---- layer 3 (the folded colour layer, N = 128): A = h2 (R0) for K-steps 0..15, the per-point tile (shared memory)
-                // for 16..21; accumulator R1[0,128); L3_SPLIT steps per weight slot.  (R1 held h1, last read by layer 2.)
-                uint32_t b3 = ring3_lo + wait_slot();
-#pragma unroll
-                for (int k = 0; k < kStepsL3; ++k) {     // unrolled: every condition below is a compile-time constant
-                    if (k && k % L3_SPLIT == 0) b3 = ring3_lo + wait_slot();
-                    if (k < 16 && (k == 0 || h_last_kstep(k - 1))) {
-                        wait_h(h_bar_of_kstep(k));
-                        if (k == 0) tr.ev(33);
-                    }
-                    const bool slot_ends = k % L3_SPLIT == L3_SPLIT - 1 || k == kStepsL3 - 1;
-                    if (tc::elect_one()) {
-                        if (k < 16) tc::mma_ts_pair_w(tm + TM_R1, tm + TM_R0 + 16 * k, b3 + (k % L3_SPLIT) * T3_U, DHI, ID3, k != 0);
-                        else tc::mma_ss_pair_w(tm + TM_R1, pe_lo + (k - 16) * KS_A_U, b3 + (k % L3_SPLIT) * T3_U, DHI, ID3, true);   // [PE(xyz) | PE(view) | 1 | 1]
-                        if (slot_ends) commit_slot();
-                        if (k == kStepsL3 - 1) tc::mma_commit_pair(&bars[BAR_ACC_FULL + 1], CMASK);
-                    }
-                    if (slot_ends) ++cnt;
-                    if (k < 14 && h_last_kstep(k + 1)) probe_h(h_bar_of_kstep(k + 2));        // the hand-over needed two K-steps from now
-                }
-                probe_slot();
-                tr.ev(23);
-            }
-        }
-    }
-    // ================================================================== EPILOGUE (thread = tile row)
-    else {
-        const int row = tid - EPI_WARP0 * 32;
-        const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-        unsigned char* PE = smem + OFF_PE;
-        const float* head = reinterpret_cast<const float*>(smem + OFF_HEAD);     // [alpha_w 256 | alpha_b 4 | rgb_w 384 | rgb_b 4]
-        uint32_t acnt = 0;                       // accumulators consumed so far: layer l of a tile uses barrier l & 1
-        Tracer tr;
-        tr.init(row == 0 ? P.trace : nullptr, 2);
-        auto wait_acc = [&]() { tc::mbar_wait(&bars[BAR_ACC_FULL + (acnt & 1)], (acnt >> 1) & 1); ++acnt; tc::tc_fence_after(); };
-        // accumulator region `reg` -> relu -> fp16 operand of the next layer, in place: the 16 fp32 columns of K-step k become
-        // 8 columns of hi pairs [16k, 16k+8) and (3-pass mode) 8 columns of lo pairs [16k+8, 16k+16).  H_READY[g] is signalled
-        // after every 4 K-steps, so the issuer can start the next layer on the first converted quarter.  SIGMA: this is h2 --
-        // also accumulate alpha_fc . relu(x) in fp32 (latent_xyzc.py:104), exactly, instead of a 1-wide tensor-core layer.
-        auto convert_region = [&](uint32_t reg, bool sigma_too) {
-            uint32_t va[16], vb[16];
-            const uint32_t base = lane_base + reg;
-            float sig = 0.f;
-            auto convert_store = [&](const uint32_t (&v)[16], int k) {
-                uint32_t h[8];
-                if (sigma_too) {
-                    const float4* aw = reinterpret_cast<const float4*>(head + 16 * k);      // same address in every lane: broadcast
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const float4 w4 = aw[q];
-                        sig = fmaf(fmaxf(__uint_as_float(v[4 * q + 0]), 0.f), w4.x, sig);
-                        sig = fmaf(fmaxf(__uint_as_float(v[4 * q + 1]), 0.f), w4.y, sig);
-                        sig = fmaf(fmaxf(__uint_as_float(v[4 * q + 2]), 0.f), w4.z, sig);
-                        sig = fmaf(fmaxf(__uint_as_float(v[4 * q + 3]), 0.f), w4.w, sig);
-                    }
-                }
-                if (NP == 3 && !sigma_too) {
-                    uint32_t l[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const float x0 = __uint_as_float(v[2 * i]), x1 = __uint_as_float(v[2 * i + 1]);
-                        h[i] = tc::cvt_rz_relu_f16x2(x0, x1);
-                        float r0, r1;
-                        tc::trunc_residual2(x0, x1, r0, r1);
-                        l[i] = tc::cvt_relu_f16x2(r0, r1);      // negative x: hi = 0 and the (negative) residual clamps to 0
-                    }
-                    tc::tmem_st8(base + 16 * k, h);
-                    tc::tmem_st8(base + 16 * k + 8, l);
-                } else {
-                    // 1-pass mode, and h2 in every mode: layer 3 (the colour path) multiplies the hi halves only, so h2 is
-                    // rounded to nearest and its lo columns are left alone (the conversion is the epilogue's critical path)
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) h[i] = tc::cvt_relu_f16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-                    tc::tmem_st8(base + 16 * k, h);
-                }
-            };
-            auto chunk_done = [&](int k) {
-                if (h_last_kstep(k)) {
-                    tc::tmem_st_wait();
-                    tc::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) arrive_at_leader(BAR_H_READY + h_bar_of_kstep(k));   // one arrival per warp, 4 + 4 warps of the pair
-                }
-            };
-            tc::tmem_ld16(base, va);
-            tc::tmem_ld_wait(va);
-#pragma unroll
-            for (int k = 0; k < 16; k += 2) {
-                tc::tmem_ld16(base + 16 * (k + 1), vb);
-                convert_store(va, k);
-                chunk_done(k);
-                tc::tmem_ld_wait(vb);
-                if (k + 2 < 16) tc::tmem_ld16(base + 16 * (k + 2), va);
-                convert_store(vb, k + 1);
-                chunk_done(k + 1);
-                if (k + 2 < 16) tc::tmem_ld_wait(va);
-            }
-            return sig;
+    };
+
+    uint32_t pc = 0;                                                // pushes consumed by the earlier tiles
+    unsigned long long real_tiles = 0, real_ksteps = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const TileRef tref = tile_ref(tile);
+        const int nrows = tref.nrows, nseg = class_segments(tref.cls), l0_ksteps = class_ksteps(tref.cls);
+        const int n_push = pushes_per_tile(l0_ksteps);
+        real_tiles += nrows > 0;
+        real_ksteps += nrows > 0 ? l0_ksteps : 0;
+        if (tid == 0) { issue_push(l0_ksteps, 0, pc); issue_push(l0_ksteps, 1, pc + 1); }
+        if (tid < TP) rows[tid] = tid < nrows ? __ldg(tref.ent + tid) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
+        __syncthreads();
+        int jp = 0;                                                 // pushes of this tile consumed
+        // wait for push jp, issue `mma(slot address)`, commit
+        auto consume = [&](auto&& mma) {
+            const uint32_t g = pc + (uint32_t)jp;
+            tc::mbar_wait(&bars[g % NUM_SLOTS], (g / NUM_SLOTS) & 1);
+            tc::wgmma_fence();
+            mma(s_ring + (g % NUM_SLOTS) * SLOT_BYTES);
+            tc::wgmma_commit();
+            ++jp;
+        };
+        // the MMAs of the push before the last one are complete in both warpgroups: its slot takes push jp
+        auto retire = [&]() {
+            tc::wgmma_wait<1>();
+            tc::acc_fence(acc0); tc::acc_fence(acc1);
+            tc::fence_proxy_async();
+            __syncthreads();
+            if (tid == 0 && jp >= 2 && jp < n_push) issue_push(l0_ksteps, jp, pc + (uint32_t)jp);
+        };
+        auto drain = [&]() {
+            tc::wgmma_wait<0>();
+            tc::acc_fence(acc0); tc::acc_fence(acc1);
+            __syncthreads();
         };
 
-        for (int tbase = tile0; tbase < n_tiles; tbase += gridDim.x) {
-            const TileRef tref = tile_ref(tbase + (int)crank);
-            float4 gm = make_float4(0.f, 0.f, 0.f, 0.f);
-            int smp = -1;
-            if (row < tref.nrows) {
-                gm = __ldg(tref.ent + row);
-                smp = (int)(__float_as_uint(gm.w) & ID_MASK);
-            }
-            const size_t ri = (size_t)P.frame * P.n_rays + (smp >= 0 ? smp / S : 0);
-            tr.ev(1);
-            {
-                // the per-point tile of layer 3: [PE(xyz) 63 | 0 | PE(view) 27 | 0 | 1 | 1 | 0 | 0].  The previous tile's layer 3
-                // has read it: this thread waited for that layer's ACC_FULL, which is committed after all of its MMAs.
-                __half* peh = reinterpret_cast<__half*>(PE);
-                auto put = [&](int k, float v) {
-                    peh[((k >> 3) * 16 + (row >> 3)) * 64 + (row & 7) * 8 + (k & 7)] = __float2half_rn(v);
-                };
-                positional_embed_anchored<10, 5>(gm.x, gm.y, gm.z, [&](int j, float v) { put(j, v); });
-                put(63, 0.f);
-                const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
-                const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
-                positional_embed_anchored<4, 4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { put(64 + j, v); });
-                put(91, 0.f); put(92, 1.f); put(93, 1.f); put(94, 0.f); put(95, 0.f);
-                tc::fence_proxy_async();     // ordered before this thread's first H_READY arrival, which the issuer waits for
-            }
-            tr.ev(2);
-            wait_acc(); tr.ev(10);
-            convert_region(TM_R0, false);        // h0
-            tr.ev(20);
-            wait_acc(); tr.ev(11);
-            convert_region(TM_R1, false);        // h1
-            tr.ev(21);
-            wait_acc(); tr.ev(12);
-            const float sigma = convert_region(TM_R0, true) + head[kHidden];     // h2, and sigma = alpha_fc . h2 + bias
-            tr.ev(22);
-            wait_acc(); tr.ev(13);
-            // ---- the colour head: rgb = rgb_fc . relu(layer-3 accumulator) + bias (latent_xyzc.py:122-124), fp32, straight from TMEM
-            float cr = head[kHidden + 4 + 3 * kColor + 0], cg = head[kHidden + 4 + 3 * kColor + 1], cb = head[kHidden + 4 + 3 * kColor + 2];
-            {
-                const float* rw = head + kHidden + 4;
-                uint32_t va[16], vb[16];
-                const uint32_t base = lane_base + TM_R1;
-                auto accumulate = [&](const uint32_t (&v)[16], int k) {
+        // ---- layer-0 gather: segment seg (64 channels of one level, coarse level first) -> segment buffer seg % SEG_BUFS
+        auto gather = [&](int seg) {
+            const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
+            const int grp = tid >> 3, t = tid & 7;
+            const int lvl = seg < 2 ? 3 : seg < 4 ? 2 : seg < 5 ? 1 : 0;
+            const int cbase0 = seg < 2 ? seg * 64 : seg < 4 ? (seg - 2) * 64 : 0;
+            const int nunits = seg == NUM_SEGS - 1 ? 1 : 2;
+            const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+            const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
+            const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
+            const int kb = 64 * (seg % SEG_BUFS);
+            for (int pp = 0; pp < TP / 32; ++pp) {
+                const int row = 4 * grp + pp;
+                const float4 e = rows[row];
+                const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
+                float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+                if (occ) {
+                    float gx, gy, gz;
+                    world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+                    Corners cn;
+                    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+                    // The 8 corners are addressed as (clamped low corner) + constant strides.  A cell that straddles the
+                    // volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted inside by one and
+                    // its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
+                    auto axis = [](int i0, int size, float (&w)[2]) {
+                        if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
+                        if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
+                        if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
+                        return i0;
+                    };
+                    const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
+                    const uint32_t cb = (uint32_t)((zc * H + yc) * W + xc) * dX;
+                    float cw[8];
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const float4 w0 = *reinterpret_cast<const float4*>(rw + 16 * k + 4 * q);
-                        const float4 w1 = *reinterpret_cast<const float4*>(rw + kColor + 16 * k + 4 * q);
-                        const float4 w2 = *reinterpret_cast<const float4*>(rw + 2 * kColor + 16 * k + 4 * q);
-                        const float x0 = fmaxf(__uint_as_float(v[4 * q + 0]), 0.f), x1 = fmaxf(__uint_as_float(v[4 * q + 1]), 0.f);
-                        const float x2 = fmaxf(__uint_as_float(v[4 * q + 2]), 0.f), x3 = fmaxf(__uint_as_float(v[4 * q + 3]), 0.f);
-                        cr = fmaf(x3, w0.w, fmaf(x2, w0.z, fmaf(x1, w0.y, fmaf(x0, w0.x, cr))));
-                        cg = fmaf(x3, w1.w, fmaf(x2, w1.z, fmaf(x1, w1.y, fmaf(x0, w1.x, cg))));
-                        cb = fmaf(x3, w2.w, fmaf(x2, w2.z, fmaf(x1, w2.y, fmaf(x0, w2.x, cb))));
+                    for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
+#pragma unroll
+                    for (int uu = 0; uu < 2; ++uu) {
+                        if (uu >= nunits) continue;
+                        const unsigned char* ub = lvl_ptr + (size_t)(cbase0 + 32 * uu) * sizeof(VT);
+#pragma unroll
+                        for (int h = 0; h < 8; h += 4) {
+                            typename Quad<VT>::raw v[4];
+#pragma unroll
+                            for (int c = 0; c < 4; ++c)
+                                v[c] = Quad<VT>::load_bytes(ub + cb + (((h + c) & 1) ? dX : 0u) + (((h + c) & 2) ? dY : 0u) + (((h + c) & 4) ? dZ : 0u));
+#pragma unroll
+                            for (int c = 0; c < 4; ++c)
+                                if (cw[h + c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw[h + c]);
+                        }
                     }
-                };
-                tc::tmem_ld16(base, va);
-                tc::tmem_ld_wait(va);
-                for (int k = 0; k < 8; k += 2) {
-                    tc::tmem_ld16(base + 16 * (k + 1), vb);
-                    accumulate(va, k);
-                    tc::tmem_ld_wait(vb);
-                    if (k + 2 < 8) tc::tmem_ld16(base + 16 * (k + 2), va);
-                    accumulate(vb, k + 1);
-                    if (k + 2 < 8) tc::tmem_ld_wait(va);
+                }
+#pragma unroll
+                for (int uu = 0; uu < 2; ++uu) {
+                    if (uu >= nunits) continue;
+                    const float (&a)[4] = acc[uu];
+                    const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
+                    uint2 hw, lw;
+                    if (NP == 3) {
+                        // (hi, lo) split with a truncated hi: the residual is exact
+                        hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
+                        float q0, q1, q2, q3;
+                        tc::trunc_residual2(a[0], a[1], q0, q1);
+                        tc::trunc_residual2(a[2], a[3], q2, q3);
+                        lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
+                        tcr::sts_v2(s_lo + off, lw);
+                    } else {
+                        hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
+                    }
+                    tcr::sts_v2(s_hi + off, hw);
                 }
             }
-            if (smp >= 0) P.raw_ws[smp] = make_float4(cr, cg, cb, sigma);
-            tr.ev(23);
-            // R1 is next written by the next tile's layer 1, issued after this thread's next H_READY arrival (fenced there)
-        }
-    }
+            tc::fence_proxy_async();
+        };
 
-    tc::tc_fence_before();
-    __syncthreads();
-    if (tid == 0 && P.stats) atomicMax(P.frame_clock + 1, global_ns());
-    tc::cluster_sync_all();                        // no CTA exits (or frees its TMEM) while the pair's MMAs may still touch it
-    if (warp == MMA_WARP) {
-        __syncwarp();
-        tc::tmem_dealloc_pair<512>(tmem);
+        // ---- epilogue of a 256-wide layer: relu -> fp16 (hi, lo) operand of the next layer in the ACT planes (own rows only).
+        // h2 (`last`) is rounded to nearest, hi only: layer 3 is a 1-pass layer.  Returns this thread's share of alpha_fc . h2.
+        auto convert = [&](bool last) {
+            float sig0 = 0.f, sig1 = 0.f;
+            auto one = [&](const float (&a)[64], int nh) {
+#pragma unroll
+                for (int c = 0; c < 16; ++c) {
+                    const int col = 128 * nh + 8 * c + cq;
+#pragma unroll
+                    for (int hr = 0; hr < 2; ++hr) {
+                        const float x0 = a[4 * c + 2 * hr], x1 = a[4 * c + 2 * hr + 1];
+                        const uint32_t off = act_off(r0 + 8 * hr, col);
+                        uint32_t hv;
+                        if (last) {
+                            const float2 aw = *reinterpret_cast<const float2*>(head + H_ALPHA + col);
+                            float& sg = hr ? sig1 : sig0;
+                            sg = fmaf(fmaxf(x0, 0.f), aw.x, sg);
+                            sg = fmaf(fmaxf(x1, 0.f), aw.y, sg);
+                            hv = tc::cvt_relu_f16x2(x0, x1);
+                        } else if (NP == 3) {
+                            hv = tc::cvt_rz_relu_f16x2(x0, x1);
+                            float q0, q1;
+                            tc::trunc_residual2(x0, x1, q0, q1);
+                            const uint32_t lv = tc::cvt_relu_f16x2(q0, q1);   // negative x: hi = 0 and the residual clamps to 0
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(s_lo + off), "r"(lv) : "memory");
+                        } else {
+                            hv = tc::cvt_relu_f16x2(x0, x1);
+                        }
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(s_hi + off), "r"(hv) : "memory");
+                    }
+                }
+            };
+            one(acc0, 0);
+            one(acc1, 1);
+            return make_float2(sig0, sig1);
+        };
+
+        // ================= layer 0
+        init_bias(head + H_B0);
+        gather(0);
+        __syncthreads();
+        for (int seg = 0; seg < nseg; ++seg) {
+            const int nks = seg == NUM_SEGS - 1 ? 2 : 4;
+            const int ka = 4 * (seg % SEG_BUFS);
+            for (int q = 0; q < nks; q += 2) {
+                consume([&](uint32_t slot) { mma256(slot, ka + q); });
+                if (q + 2 >= nks && seg + 1 < nseg) gather(seg + 1);    // under the MMAs just issued
+                retire();
+            }
+        }
+        drain();
+        convert(false);                                             // h0
+        init_bias(head + H_B0 + kHidden);
+        tc::fence_proxy_async();
+        __syncthreads();
+        // ================= layers 1, 2
+        float2 sig = make_float2(0.f, 0.f);
+        for (int layer = 1; layer <= 2; ++layer) {
+            for (int q = 0; q < kKsL12; q += 2) {
+                consume([&](uint32_t slot) { mma256(slot, q); });
+                retire();
+            }
+            drain();
+            if (layer == 1) {
+                convert(false);                                     // h1
+                init_bias(head + H_B0 + 2 * kHidden);
+            } else {
+                sig = convert(true);                                // h2, and this thread's share of sigma
+            }
+            if (layer == 2) {
+                // the per-point tile of layer 3 in the lo plane: [PE(xyz) 63 | 0 | PE(view) 27 | 0 | 1 | 1 | 0 | 0]
+                const int prow = 64 * wg + (tid & 63);
+                const float4 e = rows[prow];
+                auto put = [&](int k, float v) {
+                    const __half hv = __float2half_rn(v);
+                    asm volatile("st.shared.b16 [%0], %1;" ::"r"(s_lo + act_off(prow, k)), "h"(*reinterpret_cast<const unsigned short*>(&hv)) : "memory");
+                };
+                if ((tid & 127) < 64) {
+                    positional_embed_anchored<10, 5>(e.x, e.y, e.z, [&](int j, float v) { put(j, v); });
+                    put(63, 0.f);
+                } else {
+                    const int smp = (int)(__float_as_uint(e.w) & ID_MASK);
+                    const size_t ri = (size_t)P.frame * P.n_rays + (prow < nrows ? smp / S : 0);
+                    const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
+                    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+                    positional_embed_anchored<4, 4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { put(64 + j, v); });
+                    put(91, 0.f); put(92, 1.f); put(93, 1.f); put(94, 0.f); put(95, 0.f);
+                }
+            }
+            tc::fence_proxy_async();
+            __syncthreads();
+        }
+        // ================= layer 3 (the folded colour layer, N = 128 as two halves of 64): A = h2 (hi plane) for K-steps
+        // 0..15, the per-point tile (lo plane) for 16..21
+        float c3a[32], c3b[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) { c3a[i] = 0.f; c3b[i] = 0.f; }
+#pragma unroll
+        for (int g0 = 0; g0 < kStepsL3; g0 += L3_PUSH) {
+            consume([&](uint32_t slot) {
+#pragma unroll
+                for (int k = 0; k < L3_PUSH; ++k) {
+                    const int ks = g0 + k;
+                    if (ks >= kStepsL3) break;
+                    const uint32_t a = ks < 16 ? s_hi + 2 * ks * CHUNK_STRIDE : s_lo + 2 * (ks - 16) * CHUNK_STRIDE;
+                    const uint64_t ad = tc::make_smem_desc(a + wg_rows, CHUNK_STRIDE, 128);
+                    tc::wgmma_m64n64k16_f16(c3a, ad, tc::make_smem_desc(slot + k * TILE3, 64 * 16, 128), true);
+                    tc::wgmma_m64n64k16_f16(c3b, ad, tc::make_smem_desc(slot + SLOT_BYTES / 2 + k * TILE3, 64 * 16, 128), true);
+                }
+            });
+            tc::wgmma_wait<1>();
+            tc::acc_fence(c3a); tc::acc_fence(c3b);
+            __syncthreads();
+            if (tid == 0 && jp >= 2 && jp < n_push) issue_push(l0_ksteps, jp, pc + (uint32_t)jp);
+        }
+        tc::wgmma_wait<0>();
+        tc::acc_fence(c3a); tc::acc_fence(c3b);
+        // ---- the colour head: rgb = rgb_fc . relu(layer-3 accumulator) + bias, and sigma = alpha_fc . h2 + bias, fp32
+        float cr[2] = {0.f, 0.f}, cg[2] = {0.f, 0.f}, cbl[2] = {0.f, 0.f};
+        auto color = [&](const float (&a)[32], int nh) {
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                const int col = 64 * nh + 8 * c + cq;
+                const float2 w0 = *reinterpret_cast<const float2*>(head + H_RGBW + col);
+                const float2 w1 = *reinterpret_cast<const float2*>(head + H_RGBW + kColor + col);
+                const float2 w2 = *reinterpret_cast<const float2*>(head + H_RGBW + 2 * kColor + col);
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    const float x0 = fmaxf(a[4 * c + 2 * hr], 0.f), x1 = fmaxf(a[4 * c + 2 * hr + 1], 0.f);
+                    cr[hr] = fmaf(x1, w0.y, fmaf(x0, w0.x, cr[hr]));
+                    cg[hr] = fmaf(x1, w1.y, fmaf(x0, w1.x, cg[hr]));
+                    cbl[hr] = fmaf(x1, w2.y, fmaf(x0, w2.x, cbl[hr]));
+                }
+            }
+        };
+        color(c3a, 0);
+        color(c3b, 1);
+        float sg[2] = {sig.x, sig.y};
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+                cr[hr] += __shfl_xor_sync(0xffffffffu, cr[hr], o);
+                cg[hr] += __shfl_xor_sync(0xffffffffu, cg[hr], o);
+                cbl[hr] += __shfl_xor_sync(0xffffffffu, cbl[hr], o);
+                sg[hr] += __shfl_xor_sync(0xffffffffu, sg[hr], o);
+            }
+            const int row = r0 + 8 * hr;
+            if ((lane & 3) == 0 && row < nrows) {
+                const int smp = (int)(__float_as_uint(rows[row].w) & ID_MASK);
+                P.raw_ws[smp] = make_float4(cr[hr] + head[H_RGBB], cg[hr] + head[H_RGBB + 1], cbl[hr] + head[H_RGBB + 2],
+                                            sg[hr] + head[H_ALPHA + kHidden]);
+            }
+        }
+        pc += (uint32_t)n_push;
+        __syncthreads();                                            // rows / ACT planes / slots are free for the next tile
+    }
+    if (tid == 0 && P.stats) {
+        atomicAdd(P.stats + 0, real_tiles);
+        atomicAdd(P.stats + 4, real_ksteps);
+        if (blockIdx.x == 0) atomicAdd(P.stats + 1, (unsigned long long)sched->cnt[0] + sched->cnt[1] + sched->cnt[2] + sched->cnt[3]);
+        atomicMax(P.frame_clock + 1, global_ns());
     }
 }
 
@@ -936,19 +617,8 @@ static cudaError_t launch_list(const RenderParams& p, int grid, cudaStream_t str
     cudaError_t e = cudaFuncSetAttribute(render_tc_list_kernel<NP, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
     // what the 228 KB array does not spend on shared memory is the L1 the producers' gather lives on: ask for the smallest carve-out
-    e = cudaFuncSetAttribute(render_tc_list_kernel<NP, VT>, cudaFuncAttributePreferredSharedMemoryCarveout, (SMEM_BYTES + 1024) * 100 / (228 * 1024) + 1);
-    if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CLUSTER; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, render_tc_list_kernel<NP, VT>, p);
+    render_tc_list_kernel<NP, VT><<<grid, NT, SMEM_BYTES, stream>>>(p);
+    return cudaGetLastError();
 }
 
 static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -998,7 +668,7 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
     p.groups_per_frame = (p.n_rays + p.rays_per_group - 1) / p.rays_per_group;
     p.n_groups = p.groups_per_frame * p.batch;
     if (p.n_rays == 0) return NB_OK;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = kGridSMs;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t per_frame = tcl::align256((size_t)p.n_rays * S * sizeof(float4));
@@ -1008,10 +678,8 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
     cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
     if (e != cudaSuccess) { set_error("render_tc_list: memset failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     // the tile count of a frame is only known on the device: size the grid for the worst case (every sample occupied)
-    const long long max_tiles = ((long long)p.n_rays * S + tcl::TP - 1) / tcl::TP + 4 * tcl::CLUSTER;
-    int grid = (int)(max_tiles < sms ? max_tiles : sms);
-    grid = (grid + tcl::CLUSTER - 1) / tcl::CLUSTER * tcl::CLUSTER;     // whole clusters; tiles past the end are no-ops
-    if (grid > sms) grid = sms / tcl::CLUSTER * tcl::CLUSTER;
+    const long long max_tiles = ((long long)p.n_rays * S + tcl::TP - 1) / tcl::TP + 4;
+    const int grid = (int)(max_tiles < sms ? max_tiles : sms);         // one persistent CTA per SM; tiles past the end are no-ops
     for (int b = 0; b < p.batch; ++b) {
         p.frame = b;
         p.list_a = list;

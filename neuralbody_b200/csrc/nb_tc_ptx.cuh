@@ -1,7 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the tensor-core render kernel uses:
-// mbarrier, bulk async copy (TMA engine, SASS UBLKCP), tcgen05 alloc / mma / commit / ld / st.
-// Field layouts follow the PTX ISA "tcgen05 matrix/instruction descriptor" tables (cross-checked
-// against the bit-field unions in cute/arch/mma_sm100_desc.hpp).
+// Thin inline-PTX wrappers for the sm_90a features the tensor-core kernels use: mbarrier, bulk async copy (TMA engine,
+// SASS UBLKCP) and warpgroup MMA (wgmma.mma_async, SASS HGMMA).  Field layouts follow the PTX ISA "matrix descriptor"
+// table of the asynchronous warpgroup-level matrix instructions.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -78,7 +77,7 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity
     }
 }
 
-// generic-proxy smem writes -> visible to the async proxy (UMMA / bulk copies)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------- bulk async copy global -> shared (1-D TMA)
@@ -89,246 +88,87 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
-// multicast variant: the bytes land at the same CTA-relative offsets in every CTA of `cta_mask`, and each of those
-// CTAs' own mbarrier (same offset) receives the complete_tx
-__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar,
-                                                   uint16_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-        : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- TMEM allocation (one warp, .sync.aligned)
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"):
+// ---------------------------------------------------------------- warpgroup MMA (wgmma, sm_90a)
+// Shared-memory matrix descriptor, K-major, no swizzle ("interleave"):
 //   bits [0,14)  start address >> 4          bits [16,30) leading-dimension byte offset >> 4
-//   bits [32,46) stride-dimension byte offset >> 4        bits [46,48) = 0b01 (sm_100 descriptor version)
-//   bits [61,64) swizzle mode (0 = none)
+//   bits [32,46) stride-dimension byte offset >> 4        bits [49,52) base offset (0)   bits [62,64) swizzle (0 = none)
 // Canonical layout (units of 16 B): ((8 rows, n), 2 K-chunks) : ((1, SBO), LBO): a core matrix is 8 rows x 16 B
-// stored contiguously (128 B); SBO = distance between 8-row groups, LBO = distance between the two 8-element
-// K chunks of one K=16 MMA step.
+// stored contiguously (128 B); SBO = distance between 8-row groups, LBO = distance between the 8-element (fp16) or
+// 4-element (tf32) K chunks of one MMA K-step.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
+// the start-address field of a descriptor advanced by `bytes` (in-range addresses never carry out of the field)
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
-// Instruction descriptor for kind::f16: fp16 A/B (K-major), fp32 accumulate, dense.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (0 = f16)  [10,13) B fmt (0 = f16)  [15] A major (0 = K)  [16] B major (0 = K)
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// ---------------------------------------------------------------- MMA issue (one thread)
-// D[tmem] (+)= A[smem] * B[smem]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+// D (+)= A[smem] * B[smem]^T for one warpgroup: A is 64 x K, B is N x K, both K-major; D in registers (fp32).
+// Accumulator fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4 c + e] holds row 16 w + l / 4 + 8 (e / 2),
+// column 8 c + 2 (l % 4) + (e % 2).
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%2"
+        "7,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%5"
+        "2,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
         : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T   (A: lane = row, 32-bit column c holds K elements 2c, 2c+1)
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// all previously issued MMAs of this thread complete -> arrive(1) on the mbarrier
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// same, arriving on the mbarrier at this offset in every CTA of `cta_mask` (releases a multicast weight slot cluster-wide)
-__device__ __forceinline__ void mma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%2"
+        "7,%28,%29,%30,%31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
+        : "memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (ranks 0 / 1, same TPC) execute ONE MMA of M = 256: each CTA's tensor core computes its own 128 rows
-// (A and the accumulator are CTA-local, at the same shared-memory / TMEM addresses in both CTAs) against the WHOLE B operand,
-// of which each CTA holds one half of the N rows in its own shared memory (rank 0: rows [0, N/2), rank 1: rows [N/2, N)).
-// Only the leader (rank 0) issues; completion is signalled to both CTAs with a multicast commit.
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {       // the same warp id in BOTH CTAs calls this
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void mma_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+__device__ __forceinline__ void wgmma_m64n256k8_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%2"
+        "7,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%5"
+        "2,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%7"
+        "7,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,"
+        "%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,"
+        "%122,%123,%124,%125,%126,%127"
+        "}, %128, %129, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
         : "memory");
-}
-__device__ __forceinline__ void mma_ts_pair(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// all MMAs this thread issued so far have completed in both CTAs -> arrive(1) on the mbarrier at this offset in every CTA of the mask
-__device__ __forceinline__ void mma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-// ---- the same instructions for a WARP-UNIFORM issue loop: the whole warp walks the schedule and waits on the barriers, and
-// the MMAs / commits sit in `if (elect_one()) { ... }` blocks.  ptxas recognises elect.sync + branch as "one thread of a
-// converged warp" and then keeps warp-uniform operand values in uniform registers: an MMA is the bare UTCHMMA plus at most one
-// UIADD3 per operand that moves.  Under a plain `if (lane == 0)` the same code is a divergent region, where every
-// uniform-register operand is wrapped in an ELECT / R2UR.BROADCAST / BRA.U.ANY loop (~14 SASS instructions per MMA): the
-// issuer's own instruction stream, not the tensor pipe, then bounds the short layers.
-// elect.sync is deterministic for a given member mask (PTX ISA), so the MMAs and the commits that track them come from one lane.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// The shared-memory descriptor travels as its two 32-bit words, so stepping to the next tile of an operand is ONE 32-bit add
-// on the low word (start address >> 4 in bits [0,14): sums of in-range addresses never carry out of the field).
-__host__ __device__ constexpr uint32_t desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14); }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ void mma_ss_pair_w(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi_word, uint32_t idesc,
-                                              bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 ad, bd;\n\tmov.b64 ad, {%1, %3};\n\tmov.b64 bd, {%2, %3};\n\tsetp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], ad, bd, %4, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_lo), "r"(b_lo), "r"(desc_hi_word), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma_ts_pair_w(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t desc_hi_word, uint32_t idesc,
-                                              bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\tmov.b64 bd, {%2, %3};\n\tsetp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], bd, %4, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "r"(b_lo), "r"(desc_hi_word), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// shared::cluster address of `local` (a shared::cta address of this CTA) in the CTA of rank `cta`
-__device__ __forceinline__ uint32_t map_to_cta(const void* local, uint32_t cta) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(local)), "r"(cta));
-    return r;
-}
-// arrive(1) on an mbarrier of another CTA of the cluster.  Default semantics (release at CTA scope), as CUTLASS's cross-CTA
-// arrives use: what the arriving thread hands over lives in ITS OWN SM (shared memory fenced to the async proxy, TMEM ordered
-// by tcgen05.wait / fence) and is consumed by that same SM's tensor core; the explicit .release.cluster form costs a
-// MEMBAR.ALL.GPU on every arrival (measured: it doubled the epilogue's time per 64-column chunk).
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a LOCAL mbarrier that CTAs of the whole cluster arrive on.  Same instruction as mbar_wait (acquire at CTA scope,
-// as CUTLASS's 2-SM pipelines use): the waiter -- the MMA-issuing thread -- reads nothing through the generic proxy, and
-// the .acquire.cluster form makes ptxas append a CCTL.IVALL to every successful wait, i.e. it flushes the SM's L1 (which
-// the producers' gather lives on) some 45 times per tile.
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
-
-// ---------------------------------------------------------------- TMEM <-> registers (warp w owns lanes 32*(w%4)..+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// same wait, with the loaded registers as in/out operands: no consumer of them (the register-only cvt asm included) can be
-// scheduled above the wait
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[8]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7])
-                 :
-                 : "memory");
 }
 
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
+__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+    asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) :: "memory");
 }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t (&r)[4]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
-                 : "memory");
+
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+    asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) :: "memory");
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-                 "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
+
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+    asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127]) :: "memory");
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+
 
 // relu + round-to-nearest fp16 + pack in one instruction: lo half = relu(lo), hi half = relu(hi)
 __device__ __forceinline__ uint32_t cvt_relu_f16x2(float lo, float hi) {
@@ -353,14 +193,10 @@ __device__ __forceinline__ uint32_t cvt_rz_f16x2(float lo, float hi) {
     asm("cvt.rz.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
-// (x0 - trunc10(x0), x1 - trunc10(x1)): the exact fp32 residuals of the round-toward-zero fp16 split, as one FADD2
+// (x0 - trunc10(x0), x1 - trunc10(x1)): the exact fp32 residuals of the round-toward-zero fp16 split
 __device__ __forceinline__ void trunc_residual2(float x0, float x1, float& r0, float& r1) {
-    const float h0 = __uint_as_float(__float_as_uint(x0) & 0xFFFFE000u), h1 = __uint_as_float(__float_as_uint(x1) & 0xFFFFE000u);
-    uint64_t a, b, r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(x0), "f"(x1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(h0), "f"(h1));
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(r0), "=f"(r1) : "l"(r));
+    r0 = __fsub_rn(x0, __uint_as_float(__float_as_uint(x0) & 0xFFFFE000u));
+    r1 = __fsub_rn(x1, __uint_as_float(__float_as_uint(x1) & 0xFFFFE000u));
 }
 
 }  // namespace tc

@@ -1,5 +1,5 @@
 // Training path on the tensor cores (NB_PRECISION_TC_TF32X3): forward with an activation record + backward of the fused
-// render over the COMPACT SAMPLE LIST, as chains of tcgen05 GEMMs.
+// render over the COMPACT SAMPLE LIST, as chains of wgmma GEMMs.
 //
 // Upstream a training step is Trainer.train (lib/train/trainers/trainer.py:46-53) -> NetworkWrapper -> Renderer.render on a
 // 1024-ray chunk (BASELINE config 3) and PyTorch autograd through raw2outputs (nerf_net_utils.py:6-51), the eight Conv1d
@@ -18,10 +18,10 @@
 //             ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu).
 //
 // gemm_tf32x3_kernel: C[128 x <=256 tile] = epilogue(A B^T), fp32 in HBM on both sides.  Operands are split on the way into
-// shared memory into hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi, and three tcgen05.mma kind::tf32
-// passes (hi hi + lo hi + hi lo) accumulate in fp32 in TMEM: ~2^-21 relative error per product, i.e. fp32-grade, which the
+// shared memory into hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi, and three wgmma tf32 passes
+// (hi hi + lo hi + hi lo) accumulate in fp32 in registers (two warpgroups, 64 rows each, N = 256 per instruction): ~2^-21 relative error per product, i.e. fp32-grade, which the
 // forward's 1e-3 parity gate on depth needs (one 11-bit rounding anywhere on the density path breaks it,
-// profiles/r01_precision_emulation.txt); TF32 rather than fp16 pairs because gradients underflow fp16's range.
+// tests/test_precision_model.py); TF32 rather than fp16 pairs because gradients underflow fp16's range.
 #include "nb_device.cuh"
 #include "nb_tc_ptx.cuh"
 #include "nb_train.h"
@@ -34,8 +34,8 @@ constexpr int GT = 256;                      // threads
 #ifndef NB_TRN_KCH
 #define NB_TRN_KCH 16
 #endif
-constexpr int KCH = NB_TRN_KCH;              // reduction elements per stage (KCH / 8 MMAs of K = 8 per pass); 16 -> two CTAs per SM
-constexpr int CTAS_PER_SM = KCH <= 16 ? 2 : 1;
+constexpr int KCH = NB_TRN_KCH;              // reduction elements per stage (KCH / 8 MMAs of K = 8 per pass)
+constexpr int CTAS_PER_SM = 1;               // the 128 x 256 fp32 accumulator lives in registers: 128 per thread
 // K-major no-swizzle operand planes: a core matrix is 8 rows x 16 B.  Row groups sit SBO = 144 B apart (not 128) and the
 // 4-element K chunks LBO = rows/8 * 144 + 16 B apart: both strides are free descriptor fields, and these values make the
 // transposing 4-byte stores of a row-contiguous operand and the 16-byte stores of a K-contiguous one bank-conflict-free.
@@ -51,24 +51,13 @@ constexpr int A_ROWS = 128, B_ROWS = 256;
 constexpr int A_PLANE = (KCH / 4) * lbo_bytes(A_ROWS);    // 9280 at KCH = 16
 constexpr int B_PLANE = (KCH / 4) * lbo_bytes(B_ROWS);    // 18496
 constexpr int STAGE_BYTES = 2 * A_PLANE + 2 * B_PLANE;    // hi + lo of both operands: 55552
-constexpr int GEMM_SMEM = 2 * STAGE_BYTES;                // 111104: two CTAs per SM (one's epilogue and hand-offs hide behind the other's MMAs)
+constexpr int GEMM_SMEM = 2 * STAGE_BYTES;                // 111104: two stages (one is stored while the other's MMAs run)
 static_assert(CTAS_PER_SM * (GEMM_SMEM + 2048) <= 232448, "shared memory budget");
 constexpr int KC_TPR = KCH / 4;                           // K-contiguous operand: threads per row
 constexpr int KC_ROWS = GT / KC_TPR;                      //   rows per pass of the CTA
 constexpr int RC_NKC = KCH / 4;                           // row-contiguous operand: 4-element K chunks per stage (one warp each)
 constexpr int RC_WPK = (GT / 32) / RC_NKC;                //   warps sharing a K chunk (they split the 32-row blocks)
 template <int R> struct TileRegs { static constexpr int N = R * KCH / 1024; };   // float4 per thread and R x KCH tile
-
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {   // D f32, A/B tf32 (format 2), K-major both
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
 
 // Operand element (row, k):  KC (K contiguous): p[row * ld + k];  RC (rows contiguous): p[k * ld + row].
 // A 256-thread CTA moves one R x 32 tile per call, 16 bytes per load.
@@ -135,8 +124,6 @@ __device__ __forceinline__ void store_tile(unsigned char* __restrict__ hi_plane,
 template <bool A_KC, bool B_KC>
 __global__ void __launch_bounds__(GT, CTAS_PER_SM) gemm_tf32x3_kernel(const __grid_constant__ GemmArgs G) {
     extern __shared__ __align__(1024) unsigned char smem[];
-    __shared__ uint64_t bars[2];
-    __shared__ uint32_t tmem_slot;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int M = G.dyn_m ? (int)__ldg(G.dyn_m) : G.M;
     const int Ktot = G.dyn_k ? (int)__ldg(G.dyn_k) : G.K;
@@ -149,20 +136,13 @@ __global__ void __launch_bounds__(GT, CTAS_PER_SM) gemm_tf32x3_kernel(const __gr
         kend = min(Ktot, kbeg + per);
     }
     if (kbeg >= kend) return;
-    const int nt = min(B_ROWS, G.N - n0);               // N is a multiple of 16
+    const int nt = min(B_ROWS, G.N - n0);               // N is a multiple of 16; rows past nt are zero-filled in shared memory
     const int nchunks = (kend - kbeg + KCH - 1) / KCH;
-
-    if (warp == 0) tc::tmem_alloc<256>(&tmem_slot);
-    if (tid == 32) { tc::mbar_init(&bars[0], 1); tc::mbar_init(&bars[1], 1); tc::fence_mbar_init(); }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t taddr = tmem_slot;
-    const uint32_t idesc = make_idesc_tf32(128, nt);
     constexpr int LBO_A = lbo_bytes(A_ROWS), LBO_B = lbo_bytes(B_ROWS);
+    const int wg = warp >> 2;                            // warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile
 
     // Two register sets: the loads of chunk c + 2 are issued when chunk c has been stored, so they have two MMA batches to
-    // arrive (one set was not enough: ncu showed the CTA stalled on the L2 latency of every chunk, tensor pipe 34 % busy).
+    // arrive; two shared-memory stages: the MMAs of chunk c run while chunk c + 1 is split and stored.
     float4 va0[TileRegs<A_ROWS>::N], vb0[TileRegs<B_ROWS>::N], va1[TileRegs<A_ROWS>::N], vb1[TileRegs<B_ROWS>::N];
     load_tile<A_ROWS, A_KC>(G.a, G.lda, m0, M, kbeg, kend, va0, tid);
     load_tile<B_ROWS, B_KC>(G.b, G.ldb, n0, G.N, kbeg, kend, vb0, tid);
@@ -170,11 +150,17 @@ __global__ void __launch_bounds__(GT, CTAS_PER_SM) gemm_tf32x3_kernel(const __gr
         load_tile<A_ROWS, A_KC>(G.a, G.lda, m0, M, kbeg + KCH, kend, va1, tid);
         load_tile<B_ROWS, B_KC>(G.b, G.ldb, n0, G.N, kbeg + KCH, kend, vb1, tid);
     }
-    uint32_t phase[2] = {0u, 0u};
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     auto chunk = [&](float4 (&va)[TileRegs<A_ROWS>::N], float4 (&vb)[TileRegs<B_ROWS>::N], int c) {
         const int s = c & 1;
         unsigned char* st = smem + s * STAGE_BYTES;
-        if (c >= 2) { tc::mbar_wait(&bars[s], phase[s]); phase[s] ^= 1u; }       // the MMAs of chunk c - 2 have read this stage
+        if (c >= 2) {                                    // the MMAs of chunk c - 2 (both warpgroups) have read this stage
+            tc::wgmma_wait<1>();
+            tc::acc_fence(acc);
+            __syncthreads();
+        }
         store_tile<A_ROWS, A_KC>(st, st + A_PLANE, va, tid);
         store_tile<B_ROWS, B_KC>(st + 2 * A_PLANE, st + 2 * A_PLANE + B_PLANE, vb, tid);
         if (c + 2 < nchunks) {
@@ -183,83 +169,63 @@ __global__ void __launch_bounds__(GT, CTAS_PER_SM) gemm_tf32x3_kernel(const __gr
         }
         tc::fence_proxy_async();
         __syncthreads();
-        if (tid == 0) {
-            tc::tc_fence_after();
-            const uint32_t a_hi = tc::smem_u32(st), a_lo = a_hi + A_PLANE, b_hi = a_hi + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+        const uint32_t a_hi = tc::smem_u32(st) + 8 * wg * SBO, a_lo = a_hi + A_PLANE;
+        const uint32_t b_hi = tc::smem_u32(st) + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+        tc::wgmma_fence();
 #pragma unroll
-            for (int pass = 0; pass < 3; ++pass) {       // lo hi + hi lo + hi hi
-                const uint32_t ab = pass == 0 ? a_lo : a_hi, bb = pass == 1 ? b_lo : b_hi;
+        for (int pass = 0; pass < 3; ++pass) {           // lo hi + hi lo + hi hi
+            const uint32_t ab = pass == 0 ? a_lo : a_hi, bb = pass == 1 ? b_lo : b_hi;
 #pragma unroll
-                for (int j = 0; j < KCH / 8; ++j) {
-                    const uint64_t da = tc::make_smem_desc(ab + 2 * j * LBO_A, LBO_A, SBO);
-                    const uint64_t db = tc::make_smem_desc(bb + 2 * j * LBO_B, LBO_B, SBO);
-                    mma_tf32_ss(taddr, da, db, idesc, !(c == 0 && pass == 0 && j == 0));
-                }
+            for (int j = 0; j < KCH / 8; ++j) {
+                const uint64_t da = tc::make_smem_desc(ab + 2 * j * LBO_A, LBO_A, SBO);
+                const uint64_t db = tc::make_smem_desc(bb + 2 * j * LBO_B, LBO_B, SBO);
+                tc::wgmma_m64n256k8_tf32(acc, da, db, true);
             }
-            tc::mma_commit(&bars[s]);
         }
+        tc::wgmma_commit();
     };
     for (int c = 0; c < nchunks; c += 2) {
         chunk(va0, vb0, c);
         if (c + 1 < nchunks) chunk(va1, vb1, c + 1);
     }
-    {
-        const int s = (nchunks - 1) & 1;
-        tc::mbar_wait(&bars[s], phase[s]);               // commits complete in order: the accumulator is final
-    }
-    tc::tc_fence_after();
+    tc::wgmma_wait<0>();
+    tc::acc_fence(acc);
 
-    // ---- epilogue: warp w reads TMEM lanes 32 (w % 4) .. +31 (= rows), 16 columns at a time; warps w and w + 4 alternate
-    const int q = warp & 3;
-    const int row = m0 + 32 * q + lane;
-    const bool row_ok = row < M;
-    const float* bias = G.bias;
-    if (bias && G.bias_frame_stride && row_ok)
-        bias += (size_t)((__float_as_uint(__ldg(&G.list[row].w)) & 0x0FFFFFFFu) / G.samples_per_frame) * G.bias_frame_stride;
-    for (int j = warp >> 2; j < nt / 16; j += 2) {
-        uint32_t r[16];
-        tc::tmem_ld16(taddr + ((uint32_t)(32 * q) << 16) + 16 * j, r);
-        tc::tmem_ld_wait(r);
-        if (!row_ok) continue;
-        const int col0 = n0 + 16 * j;
-        float v[16];
+    // ---- epilogue, straight from the accumulator registers: this thread holds rows r and r + 8, columns 8 j + 2 (lane % 4) + {0, 1}
+    const int rbase = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = __uint_as_float(r[e]);
-        if (bias) {
+    for (int h = 0; h < 2; ++h) {
+        const int row = rbase + 8 * h;
+        if (row >= M) continue;
+        const float* bias = G.bias;
+        if (bias && G.bias_frame_stride)
+            bias += (size_t)((__float_as_uint(__ldg(&G.list[row].w)) & 0x0FFFFFFFu) / G.samples_per_frame) * G.bias_frame_stride;
 #pragma unroll
-            for (int e = 0; e < 16; e += 4) {
-                const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + col0 + e));
-                v[e] += bv.x; v[e + 1] += bv.y; v[e + 2] += bv.z; v[e + 3] += bv.w;
+        for (int j = 0; j < B_ROWS / 8; ++j) {
+            const int cl = 8 * j + cq;
+            if (cl >= nt) continue;
+            const int col = n0 + cl;
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (bias) {
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + col));
+                v0 += bv.x; v1 += bv.y;
             }
-        }
-        if (col0 < G.relu_cols) {                        // relu_cols is a multiple of 16
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = fmaxf(v[e], 0.f);
-        }
-        if (G.mask) {
-            const float* mk = G.mask + (size_t)row * G.ldm + col0;
-#pragma unroll
-            for (int e = 0; e < 16; e += 4) {
-                const float4 mv = __ldg(reinterpret_cast<const float4*>(mk + e));
-                if (!(mv.x > 0.f)) v[e] = 0.f;
-                if (!(mv.y > 0.f)) v[e + 1] = 0.f;
-                if (!(mv.z > 0.f)) v[e + 2] = 0.f;
-                if (!(mv.w > 0.f)) v[e + 3] = 0.f;
+            if (col < G.relu_cols) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }   // relu_cols is a multiple of 16
+            if (G.mask) {
+                const float2 mv = __ldg(reinterpret_cast<const float2*>(G.mask + (size_t)row * G.ldm + col));
+                if (!(mv.x > 0.f)) v0 = 0.f;
+                if (!(mv.y > 0.f)) v1 = 0.f;
             }
-        }
-        float* dst = G.c + (size_t)row * G.ldc + col0;
-        if (G.atomic) {
-#pragma unroll
-            for (int e = 0; e < 16; ++e)
-                if (v[e] != 0.f) atomicAdd(dst + e, v[e]);
-        } else {
-#pragma unroll
-            for (int e = 0; e < 16; e += 4) *reinterpret_cast<float4*>(dst + e) = make_float4(v[e], v[e + 1], v[e + 2], v[e + 3]);
+            float* dst = G.c + (size_t)row * G.ldc + col;
+            if (G.atomic) {
+                if (v0 != 0.f) atomicAdd(dst, v0);
+                if (v1 != 0.f) atomicAdd(dst + 1, v1);
+            } else {
+                *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+            }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc<256>(taddr);
 }
 
 int launch_gemm(const GemmArgs& g, bool a_kc, bool b_kc, int max_m, int splits, cudaStream_t stream) {
@@ -645,7 +611,7 @@ int launch_train_fwd(const RenderParams& p_in, int volume_dtype, cudaStream_t st
         launch_classify(p, stream);
     }
     // 2. features + encodings, 3. the decoder as four GEMMs over the list
-    const int grid_pts = (int)((pmax + GP - 1) / GP < 148 * 8 ? (pmax + GP - 1) / GP : 148 * 8);
+    const int grid_pts = (int)((pmax + GP - 1) / GP < kGridSMs * 8 ? (pmax + GP - 1) / GP : kGridSMs * 8);
     if (volume_dtype == NB_DTYPE_F32) gather_kernel<float><<<grid_pts, 256, 0, stream>>>(p, sv);
     else gather_kernel<__half><<<grid_pts, 256, 0, stream>>>(p, sv);
     const float* wf = p.wf32;
@@ -662,7 +628,7 @@ int launch_train_fwd(const RenderParams& p_in, int volume_dtype, cudaStream_t st
     g.bias = sv.bias3; g.bias_frame_stride = kWS; g.list = sv.list; g.samples_per_frame = (unsigned int)p.n_rays * p.n_samples; g.relu_cols = kColor;
     if ((st = launch_gemm(g, true, true, (int)pmax, 1, stream)) != NB_OK) return st;
     // 4. rgb head + raw records, 5. raw2outputs
-    head_kernel<<<148 * 4, 256, 0, stream>>>(wf, sv, reinterpret_cast<float4*>(p.raw));
+    head_kernel<<<kGridSMs * 4, 256, 0, stream>>>(wf, sv, reinterpret_cast<float4*>(p.raw));
     for (int b = 0; b < p.batch; ++b) {
         p.frame = b;
         p.raw_ws = reinterpret_cast<float4*>(p.raw) + (size_t)b * p.n_rays * p.n_samples;
@@ -703,7 +669,7 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
 
     // 1. d(outputs) -> d(raw) per sample (dense), 2. the colour layer's output gradient over the list
     launch_composite_bwd(p, t.raw, t.d_rgb, t.d_depth, t.d_acc, reinterpret_cast<float*>(d_raw), 4, stream);
-    bwd_head_kernel<<<148 * 2, 256, 0, stream>>>(p.wf32, sv, d_raw, G3, G_(g.rgb_w), G_(g.rgb_b));
+    bwd_head_kernel<<<kGridSMs * 2, 256, 0, stream>>>(p.wf32, sv, d_raw, G3, G_(g.rgb_w), G_(g.rgb_b));
     // 3. dgrad chain (relu masks = the saved activations)
     GemmArgs a{};
     a.dyn_m = sv.count; a.relu_cols = 0;
@@ -719,7 +685,7 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
         // 4. trilinear backward
         cudaMemsetAsync(dblob, 0, gb.floats * 4, stream);
-        const int grid_pts = (int)((pmax + GP - 1) / GP < 148 * 8 ? (pmax + GP - 1) / GP : 148 * 8);
+        const int grid_pts = (int)((pmax + GP - 1) / GP < kGridSMs * 8 ? (pmax + GP - 1) / GP : kGridSMs * 8);
         scatter_kernel<<<grid_pts, 256, 0, stream>>>(p, sv, DF, dblob, gb);
         for (int l = 0; l < 4; ++l) {
             const size_t nvox = (size_t)p.lvl_D[l] * p.lvl_H[l] * p.lvl_W[l];

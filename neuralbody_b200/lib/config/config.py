@@ -102,13 +102,13 @@ def _defaults():
     c.num_train_frame = 60
     c.voxel_size = [0.005, 0.005, 0.005]
     c.big_box = False
-    # B200 renderer options (new)
-    c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" tcgen05, 3-pass hi/lo density path
-                                        # (meets the 1e-3 parity gate) | "tc_fp16" tcgen05 1-pass (fastest, ~4e-3 on depth)
+    # H100 renderer options (new)
+    c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
+                                        # (meets the 1e-3 parity gate) | "tc_fp16" wgmma 1-pass (fastest, ~4e-3 on depth)
     c.render_volume_dtype = "auto"      # "auto": fp16 volume for tc_fp16, fp32 otherwise
     c.render_skip_empty = True          # tensor-core modes: exact empty-sample skipping (bit-identical outputs)
     c.render_return_weights = True      # 'weights' (B,n,S) is unused downstream; may be skipped
-    c.render_train_precision = 'tc_tf32x3'   # calls autograd records: 'tc_tf32x3' (tcgen05 TF32 GEMM chains over the sample list) | 'fp32' (exact FFMA kernels)
+    c.render_train_precision = 'tc_tf32x3'   # calls autograd records: 'tc_tf32x3' (wgmma TF32 GEMM chains over the sample list) | 'fp32' (exact FFMA kernels)
     c.render_importance = 0             # f-4: > 0 adds a fine pass with this many importance samples (upstream's N_importance is a dead key for Neural Body, so the default stays single-pass)
     c.chunk = 0                         # 0 = all rays of the call in one launch
     return c

@@ -1,7 +1,7 @@
 """Drop-in for the reference's Neural Body renderer.
 
 Replaces lib/networks/renderer/if_clight_renderer.py (the file every Neural Body config
-selects through `renderer_module/renderer_path`; BASELINE.json calls it
+selects through `renderer_module/renderer_path`; the project brief calls it
 if_nerf_renderer.py): same class name, constructor and `render(batch)` contract
 (:94-122), same five output keys/shapes/dtypes (:84-92), same config keys read inside
 (`N_samples, perturb, raw_noise_std, white_bkgd` :13,16,82; `voxel_size`
@@ -78,7 +78,7 @@ class Renderer:
         return _PRECISIONS[name]
 
     def _train_precision(self, B, n, S):
-        """Precision of a call autograd records: 'tc_tf32x3' (default: sample list + tcgen05 TF32 GEMM chains, exact empty-sample
+        """Precision of a call autograd records: 'tc_tf32x3' (default: sample list + wgmma TF32 GEMM chains, exact empty-sample
         skipping in forward and backward) or 'fp32' (the exact FFMA kernels)."""
         name = str(self._opt("render_train_precision", "tc_tf32x3"))
         if name not in ("tc_tf32x3", "fp32"):

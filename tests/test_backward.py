@@ -39,7 +39,7 @@ def _rel_l2(a, b):
 @pytest.mark.gpu
 @pytest.mark.parametrize("train_precision", ["tc_tf32x3", "fp32"])
 def test_backward_matches_oracle_autograd(case, train_precision):
-    """Both training precisions: the tcgen05 TF32x3 GEMM chains over the sample list (default) and the exact FFMA kernels."""
+    """Both training precisions: the wgmma TF32x3 GEMM chains over the sample list (default) and the exact FFMA kernels."""
     import gpu_utils as Gu
     from neuralbody_b200.lib.config import cfg
     scene, t_rand, G, pg, vg, ret_ref, _ = case

@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(lib, name), "include/neuralbody_b200.h declares %s but the library does not export it" % name
     from neuralbody_b200 import capi
     assert sorted(capi.EXPORTS) == declared
-    assert capi.load().nb_abi_version() == 4
+    assert capi.load().nb_abi_version() == 5
 
 
 def test_struct_layouts_match_header(built_lib):

@@ -1,4 +1,4 @@
-"""GPU: the training path's tcgen05 GEMM in isolation (csrc/nb_train.cu::gemm_tf32x3_kernel) against fp64 matmuls:
+"""GPU: the training path's wgmma GEMM in isolation (csrc/nb_train.cu::gemm_tf32x3_kernel) against fp64 matmuls:
 both operand layouts, ragged M / K, N tiles, bias + relu + mask epilogues, split reductions with atomics, and the range of
 magnitudes gradients have (fp16 pairs would underflow there)."""
 import ctypes as C
