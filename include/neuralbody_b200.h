@@ -202,6 +202,31 @@ int nb_sample_pdf(const nb_importance_args* args, void* stream);
  * points: device (B, n_points, 3) world coordinates; sigma: device (B, n_points). */
 int nb_decode_density(const nb_render_args* frame, const float* points, int n_points, float* sigma, void* stream);
 
+/* Marching cubes over a dense fp32 grid: the mesh step of the mesh renderer (lib/networks/renderer/if_mesh_renderer.py:42-48,
+ * mcubes.marching_cubes(cube, cfg.mesh_th)).  A grid value is inside when it is > isovalue (equal counts as outside).
+ * Vertices are the crossed grid edges p -> p + e_a, at p + t e_a with t = (iso - v(p)) / (v(p + e_a) - v(p)) in fp64, in
+ * index coordinates; they follow grid-point order (x, y, z edge within a point).  Triangles follow the order of their
+ * cells' min corners and the table order of csrc/nb_mc_table.h within a cell; (b - a) x (c - a) points towards decreasing
+ * values.  The table separates the inside corners of every ambiguous face, so the mesh is closed wherever the surface
+ * stays off the grid boundary.  Deterministic: no atomics decide any output position.
+ * Usage: nb_mcubes_count, read counts on the host (one sync), allocate, nb_mcubes_emit with the same arguments and the
+ * same workspace on the same stream (skip it when the mesh is empty).  Grids with 5 * cells >= 2^31 or 3 * points >= 2^31
+ * (32-bit offsets) return NB_ERR_UNSUPPORTED before anything is enqueued; a grid with a dimension of 1 has no cell and an
+ * empty mesh. */
+typedef struct nb_mcubes_args {
+    const float* grid;        /* device (nx, ny, nz) fp32, C order */
+    int nx, ny, nz;
+    double isovalue;          /* cfg.mesh_th */
+    void* workspace;          /* device scratch of nb_mcubes_workspace_bytes(nx, ny, nz) bytes, kept from count to emit */
+    size_t workspace_bytes;
+    long long* counts;        /* device int64[2]: n_vertices, n_triangles (written by nb_mcubes_count) */
+    double* vertices;         /* device (n_vertices, 3), index coordinates (nb_mcubes_emit) */
+    long long* triangles;     /* device (n_triangles, 3) (nb_mcubes_emit) */
+} nb_mcubes_args;
+size_t nb_mcubes_workspace_bytes(int nx, int ny, int nz);   /* 0 for dims < 1 */
+int    nb_mcubes_count(const nb_mcubes_args* a, void* stream);
+int    nb_mcubes_emit(const nb_mcubes_args* a, void* stream);   /* after the caller read counts */
+
 /* f-2: ray generation on the device.  Replaces the per-view numpy of get_rays (lib/utils/if_nerf/if_nerf_data_utils.py:8-21)
  * and get_near_far (:54-69) as called from image_rays (lib/utils/render_utils.py:120-137): fp64 arithmetic like upstream, fp32
  * results.  Writes ALL H*W pixels (row-major) plus mask_at_box; the caller compacts with the mask (upstream: ray_o[mask_at_box]).

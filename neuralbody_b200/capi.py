@@ -14,7 +14,8 @@ NB_NUM_LEVELS = 4
 EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_volume_bytes", "nb_packed_volume_level_offset",
            "nb_pack_volume", "nb_packed_weights_bytes", "nb_pack_weights", "nb_render_fwd",
            "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_render_bwd", "nb_render_save_bytes",
-           "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf"]
+           "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf",
+           "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit"]
 
 
 class nb_volume_level(C.Structure):
@@ -59,6 +60,12 @@ class nb_importance_args(C.Structure):
     _fields_ = [("n_rays_total", C.c_int), ("n_samples", C.c_int), ("n_importance", C.c_int),
                 ("near", C.c_void_p), ("far", C.c_void_p), ("t_vals", C.c_void_p), ("t_rand", C.c_void_p),
                 ("weights", C.c_void_p), ("u", C.c_void_p), ("z_out", C.c_void_p), ("z_samples", C.c_void_p)]
+
+
+class nb_mcubes_args(C.Structure):
+    _fields_ = [("grid", C.c_void_p), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int), ("isovalue", C.c_double),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("counts", C.c_void_p),
+                ("vertices", C.c_void_p), ("triangles", C.c_void_p)]
 
 
 class nb_render_bwd_args(C.Structure):
@@ -124,6 +131,12 @@ def load(path=None):
     lib.nb_gen_rays_sharded.argtypes = [C.POINTER(nb_camera)] + [C.c_int] * 4 + [C.c_void_p] * 6
     lib.nb_sample_pdf.restype = C.c_int
     lib.nb_sample_pdf.argtypes = [C.POINTER(nb_importance_args), C.c_void_p]
+    lib.nb_mcubes_workspace_bytes.restype = C.c_size_t
+    lib.nb_mcubes_workspace_bytes.argtypes = [C.c_int] * 3
+    lib.nb_mcubes_count.restype = C.c_int
+    lib.nb_mcubes_count.argtypes = [C.POINTER(nb_mcubes_args), C.c_void_p]
+    lib.nb_mcubes_emit.restype = C.c_int
+    lib.nb_mcubes_emit.argtypes = [C.POINTER(nb_mcubes_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

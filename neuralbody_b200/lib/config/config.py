@@ -102,6 +102,7 @@ def _defaults():
     c.num_train_frame = 60
     c.voxel_size = [0.005, 0.005, 0.005]
     c.big_box = False
+    c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
                                         # (meets the 1e-3 parity gate) | "tc_fp16" wgmma 1-pass (fastest, ~4e-3 on depth)

@@ -1,0 +1,145 @@
+"""Benchmark (GPU) of the mesh renderer (if_mesh_renderer) on the full-size synth-313 frame: density on the 5 mm world grid
+(170x325x146) where it is inside the synthetic mask views, cube, marching cubes at --mesh-th.  One step = one frame, split
+into its steps with CUDA events after warm-up.  Prints one JSON line with the split, the density kernel's FP32 rate, the
+marching-cubes bytes/s, and the card's name and power limit read in the same run.  Writes nothing.
+
+Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10]
+(upstream's default mesh_th = 50 lies above the synthetic body's sigma, p95 ~ 30, and would give an empty mesh)"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+FLOP_PER_POINT_DENSITY = 442880         # fc_0 + fc_1 + fc_2 + alpha_fc: 2 x (352*256 + 2*256*256 + 256) MAC per point
+FP32_TFLOPS_DATASHEET = 67.0             # H100 SXM data sheet, dense FP32 (700 W card)
+HBM_TBS_DATASHEET = 3.35                 # H100 SXM data sheet, HBM3
+PAD = 10
+
+
+def card_info(dev):
+    """Card name and power limit, read in the same run as the measurement."""
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(dev.index or 0)
+        info["power_limit_w"] = pynvml.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
+    except Exception:
+        try:
+            out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i",
+                                  str(dev.index or 0)], capture_output=True, text=True, timeout=30).stdout.strip()
+            info["power_limit_w"] = float(out.splitlines()[0])
+        except Exception:
+            pass
+    return info
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--mesh-th", type=float, default=10.0, help="isovalue (cfg.mesh_th)")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_mesh needs a CUDA device")
+    from oracle import mesh_case
+    from neuralbody_b200 import mcubes
+    from neuralbody_b200.lib.config import cfg
+    from neuralbody_b200.lib.networks.make_network import make_network, load_source
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scene, _, batch = mesh_case.build_case("mesh_full")
+    cfg.num_train_frame = int(scene["weights"]["latent.weight"].shape[0])
+    cfg.voxel_size = list(scene["voxel_size"])
+    cfg.mesh_th = float(args.mesh_th)
+    net = make_network(cfg)
+    net.load_state_dict(scene["weights"], strict=False)
+    net = net.to(dev).eval()
+    net.set_feature_volume([v.to(dev) for v in scene["volumes"]])
+    path = os.path.join(ROOT, "neuralbody_b200", "lib", "networks", "renderer", "if_mesh_renderer.py")
+    ren = load_source("neuralbody_b200.lib.networks.renderer.if_mesh_renderer", path).Renderer(net)
+    bd = {k: v.to(dev) for k, v in batch.items()}
+
+    def frame():
+        """Renderer.render (density_cube + marching cubes + copies) step by step, events between the steps."""
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(7)]
+        with torch.no_grad():
+            ev[0].record()
+            inside = bd["inside"][0].bool()
+            wpts = bd["pts"][0][inside][None]
+            sp = ren.prepare_sp_input(bd)
+            fv = net.encode_sparse_voxels(sp)
+            ev[1].record()
+            alpha = net.calculate_density(wpts, fv, sp)
+            ev[2].record()
+            cube = torch.zeros(tuple(s + 2 * PAD for s in inside.shape), dtype=torch.float32, device=dev)
+            cube[PAD:-PAD, PAD:-PAD, PAD:-PAD][inside] = alpha[0, :, 0]
+            ev[3].record()
+            verts, tris = mcubes.marching_cubes(cube, cfg.mesh_th)
+            ev[4].record()
+            mesh = mcubes.make_mesh(verts.cpu().numpy(), tris.cpu().numpy())
+            ev[5].record()
+            cube_host = cube.cpu().numpy().astype(np.float64)
+            ev[6].record()
+        return ev, int(wpts.shape[1]), mesh, cube_host
+
+    for _ in range(args.warmup):
+        frame()
+    torch.cuda.synchronize(dev)
+    rows = []
+    for _ in range(args.steps):
+        ev, n_in, mesh, cube_host = frame()
+        torch.cuda.synchronize(dev)
+        rows.append([ev[i].elapsed_time(ev[i + 1]) for i in range(6)])
+    # the public call, whole (cube copy included); it must give the same result as the split steps
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    with torch.no_grad():
+        ren.render(bd)
+        torch.cuda.synchronize(dev)
+        t0.record()
+        for _ in range(args.steps):
+            out = ren.render(bd)
+        t1.record()
+        torch.cuda.synchronize(dev)
+    render_ms = t0.elapsed_time(t1) / args.steps
+    assert np.array_equal(np.asarray(out["mesh"].faces), np.asarray(mesh.faces)) and np.array_equal(out["cube"], cube_host)
+    med = [float(np.median([r[i] for r in rows])) for i in range(6)]
+    names = ("prepare_ms", "density_ms", "scatter_ms", "marching_cubes_ms", "mesh_to_host_ms", "cube_to_host_ms")
+    split = dict(zip(names, med))
+    excl_cube = sum(med[:5])
+    nx, ny, nz = cube_host.shape
+    n_pts = nx * ny * nz
+    n_v, n_f = len(mesh.vertices), len(mesh.faces)
+    # bytes the marching-cubes kernels move as written: count (grid 4 B read, code 2 B write per point), two scans
+    # (code 2 B read, offset 4 B write each), emit (code + grid + two offsets read) + 24 B per vertex and per triangle
+    mc_bytes = n_pts * (6 + 2 * 6 + 2 + 4 + 8) + 24 * (n_v + n_f)
+    mc_gbs = mc_bytes / (split["marching_cubes_ms"] * 1e-3) / 1e9
+    dens_tflops = FLOP_PER_POINT_DENSITY * n_in / (split["density_ms"] * 1e-3) / 1e12
+    line = {
+        "metric": "mesh_frame_ms_excl_cube_copy", "value": excl_cube, "unit": "ms", "higher_is_better": False,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "data": "synthetic",
+        "config": {"workload": "mesh renderer (if_mesh_renderer) on the full-size synth-313 frame: 5 mm world grid %s, inside "
+                               "from 4 synthetic 256x256 mask views, cube padded to %s, marching cubes at mesh_th = %g"
+                               % (tuple(batch["inside"].shape[1:]), (nx, ny, nz), cfg.mesh_th),
+                   "grid_points": int(np.prod(batch["inside"].shape)), "padded_points": n_pts},
+        "inside_points": n_in, "vertices": n_v, "triangles": n_f,
+        "split_ms_median": split, "render_ms_excl_cube_copy": excl_cube, "render_call_ms": render_ms,
+        "density": {"flop_per_point": FLOP_PER_POINT_DENSITY, "tflops": dens_tflops,
+                    "fraction_of_fp32_datasheet": dens_tflops / FP32_TFLOPS_DATASHEET,
+                    "datasheet": "67 TFLOP/s dense FP32, H100 SXM at 700 W (not a reached figure)"},
+        "marching_cubes": {"bytes_as_written": mc_bytes, "gbs": mc_gbs, "fraction_of_hbm_datasheet": mc_gbs / (HBM_TBS_DATASHEET * 1e3),
+                           "note": "includes the one host sync between count and emit and the launch gaps"},
+        "card": card_info(dev),
+    }
+    print(json.dumps(line))
+
+
+if __name__ == "__main__":
+    main()
