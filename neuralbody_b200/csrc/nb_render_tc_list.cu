@@ -27,7 +27,6 @@ namespace tcl {
 using tcr::Quad;
 
 constexpr int TP = 128;                                            // list rows per tile
-constexpr int NT = 256;                                            // two warpgroups
 constexpr int NUM_SEGS = 6;
 constexpr int MAXS = 1024;                                         // samples per classification block
 constexpr uint32_t ID_MASK = 0x0FFFFFFFu;                          // list entry .w = frame sample id | level bits << 28
@@ -144,23 +143,42 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 }
 
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
-// One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  Two warpgroups each own 64 rows of a tile and
-// issue the wgmma for them; the B operand (the layer's weights) is streamed through a two-slot shared-memory ring by bulk
-// copies (thread 0 issues, an mbarrier with transaction count signals), one push = two K-steps of both N halves.
+// One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  The CTA is warp-specialised:
+//   producer warpgroup (warps 0-3)   warp 0: one elected lane streams the weights with bulk copies into a 4-slot ring (one
+//                                     K-step of both N halves and both planes per slot).  Warps 1-3: each tile's list rows
+//                                     (double-buffered) and layer 3's per-point tile.
+//   consumer warpgroups 1 and 2      rows [0, 64) and [64, 128) of a tile: gather layer 0's feature segments of their own rows,
+//                                     issue the wgmma and run the epilogues.  Nothing divergent sits between a wgmma and the
+//                                     wait that retires it (the gather runs only while none of the warpgroup's wgmma are in
+//                                     flight; the other warpgroup's MMAs overlap it), and the K-step after a group is issued
+//                                     before that group is waited for (wait_group 1), so the tensor pipe always holds the next
+//                                     group.  A warpgroup's A operand is its own rows: a warpgroup-local named barrier (plus
+//                                     fence.proxy.async) publishes what its epilogue or gather wrote.
 //   activations   the ACT planes hold the current layer's A operand as fp16 (hi plane, and in the 3-pass mode the lo plane):
 //                 during layer 0 a ring of four gathered 64-channel feature segments, then h0 / h1 / h2 (written by the
 //                 epilogue straight from the accumulator registers), and in layer 3 the per-point tile in the lo plane.
-//   gather        every thread gathers: segment s + 1 is gathered while the MMAs of segment s run.
 //   accumulators  fp32 in registers (two m64n128 halves per warpgroup), started from the fp32 bias of the layer.
+// Barriers (mbarrier phases; every wait is bounded by the watchdog):
+//   full[s] / empty[s]   weight slot s: bulk-copy transaction bytes / one arrival per consumer warp
+//   rows_full            the tile's list rows are loaded (every row thread)
+//   l2_done, pe_full     the consumers' layer-2 MMAs are complete, so the lo plane is free (one arrival per consumer warp) /
+//                        the per-point tile is written (every row thread)
+constexpr int NT = 384;                                            // producer warpgroup + two consumer warpgroups
+constexpr int NROWT = 96;                                          // the row threads: producer warps 1..3
+// setmaxnreg moves registers within the CTA's launch allocation (NT x 168: __launch_bounds__(NT, 1) over the 64 K file); a
+// consumer increase the pool cannot cover blocks for ever
+constexpr int LAUNCH_REGS = (65536 / NT) / 8 * 8;
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
 constexpr int CHUNK_STRIDE = TP * 16 + 16;                         // K-chunk stride (LBO) of an ACT plane: 16 bytes of padding
                                                                    // rotate successive chunks by 4 banks for the gather's stores
 constexpr int ACT_CHUNKS = kHidden / 8;
 constexpr int PLANE_BYTES = ACT_CHUNKS * CHUNK_STRIDE;             // 66048
 constexpr int SEG_BUFS = 4;                                        // layer-0 segment ring inside the ACT planes
-constexpr int SLOT_BYTES = 32768, NUM_SLOTS = 2;
+constexpr int SLOT_BYTES = 16384, NUM_SLOTS = 4;
 constexpr int TILE256 = kHalfTile256 * 2;                          // one K-step, one N half (128 rows) of an N = 256 layer: 4 KB
 constexpr int TILE3 = kHalfTile3 * 2;                              // one K-step, one N half (64 rows) of layer 3: 2 KB
-constexpr int L3_PUSH = 8;                                         // layer-3 K-steps per push
+constexpr int L3_PUSH = 4;                                         // layer-3 K-steps per push
+constexpr int L3_PUSHES = (kStepsL3 + L3_PUSH - 1) / L3_PUSH;
 constexpr int HEAD_FLOATS = kHidden + 4 + 3 * kColor + 4 + 3 * kHidden;   // alpha_fc, rgb_fc, then the biases of fc_0..fc_2, fp32
 constexpr int H_ALPHA = 0, H_RGBW = kHidden + 4, H_RGBB = H_RGBW + 3 * kColor, H_B0 = H_RGBB + 4;
 constexpr int OFF_HI = 0, OFF_LO = PLANE_BYTES;
@@ -168,16 +186,16 @@ constexpr int OFF_RING = 2 * PLANE_BYTES;
 constexpr int OFF_HEAD = OFF_RING + NUM_SLOTS * SLOT_BYTES;
 constexpr int OFF_XF = OFF_HEAD + HEAD_FLOATS * 4;
 constexpr int OFF_SCHED = OFF_XF + 128;
-constexpr int OFF_ROWS = OFF_SCHED + 64;                           // the tile's list entries (float4 per row)
-constexpr int OFF_BAR = OFF_ROWS + TP * 16;
-constexpr int SMEM_BYTES = OFF_BAR + NUM_SLOTS * 8;
+constexpr int OFF_ROWS = OFF_SCHED + 64;                           // two tiles' list entries (float4 per row)
+constexpr int OFF_BAR = OFF_ROWS + 2 * TP * 16;
+enum { B_FULL = 0, B_EMPTY = B_FULL + NUM_SLOTS, B_ROWSFULL = B_EMPTY + NUM_SLOTS, B_L2DONE, B_PEFULL, NUM_BARS };
+constexpr int SMEM_BYTES = OFF_BAR + NUM_BARS * 8;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 static_assert(OFF_RING % 128 == 0 && OFF_HEAD % 16 == 0 && OFF_ROWS % 16 == 0 && OFF_BAR % 8 == 0, "alignment");
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NT * LAUNCH_REGS, "register pool of the CTA");
 
-// weight pushes of a tile whose layer 0 runs l0_ksteps K-steps: layer 0 and layers 1 / 2 two K-steps each, layer 3 in groups of L3_PUSH
-__host__ __device__ constexpr int pushes_per_tile(int l0_ksteps) {
-    return l0_ksteps / 2 + 2 * (kKsL12 / 2) + (kStepsL3 + L3_PUSH - 1) / L3_PUSH;
-}
+// weight pushes of a tile whose layer 0 runs l0_ksteps K-steps: one per K-step of layers 0..2, layer 3 in groups of L3_PUSH
+__host__ __device__ constexpr int pushes_per_tile(int l0_ksteps) { return l0_ksteps + 2 * kKsL12 + L3_PUSHES; }
 
 __device__ __forceinline__ uint32_t act_off(int row, int k) {      // byte offset of element (row, k) in an ACT plane
     return (uint32_t)((k >> 3) * CHUNK_STRIDE + (row >> 3) * 128 + (row & 7) * 16 + (k & 7) * 2);
@@ -189,15 +207,21 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
     FrameXf* xf = reinterpret_cast<FrameXf*>(smem + OFF_XF);
     float* head = reinterpret_cast<float*>(smem + OFF_HEAD);
-    float4* rows = reinterpret_cast<float4*>(smem + OFF_ROWS);
+    float4* rows_buf = reinterpret_cast<float4*>(smem + OFF_ROWS);
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    const int wg = warp >> 2;                                       // warpgroup: rows [64 wg, 64 wg + 64) of a tile
+    const int wgid = warp >> 2;                                     // 0: producer, 1 / 2: consumers
     const int S = P.n_samples;
-    const uint32_t s_hi = tc::smem_u32(smem + OFF_HI), s_lo = tc::smem_u32(smem + OFF_LO), s_ring = tc::smem_u32(smem + OFF_RING);
+    const uint32_t s_hi0 = tc::smem_u32(smem + OFF_HI), s_lo0 = tc::smem_u32(smem + OFF_LO), s_ring = tc::smem_u32(smem + OFF_RING);
 
     if (tid == 0) {
-        for (int i = 0; i < NUM_SLOTS; ++i) tc::mbar_init(&bars[i], 1);
+        for (int i = 0; i < NUM_SLOTS; ++i) {
+            tc::mbar_init(&bars[B_FULL + i], 1);
+            tc::mbar_init(&bars[B_EMPTY + i], 8);
+        }
+        tc::mbar_init(&bars[B_ROWSFULL], NROWT);
+        tc::mbar_init(&bars[B_L2DONE], 8);
+        tc::mbar_init(&bars[B_PEFULL], NROWT);
         tc::fence_mbar_init();
     }
     load_frame_xf(P, xf, tid);
@@ -239,181 +263,173 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         return r;
     };
 
-    // ---- the weight stream.  Push j of a tile goes to slot (pc + j) % 2, pc = pushes of the earlier tiles.
-    const unsigned char* seq = reinterpret_cast<const unsigned char*>(P.wf16);
-    auto issue_push = [&](int l0_ksteps, int j, uint32_t gidx) {      // (thread 0)
-        const uint32_t slot = gidx % NUM_SLOTS;
-        unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
-        uint64_t* bar = &bars[slot];
-        const int n0 = l0_ksteps / 2;
-        if (j < n0 + kKsL12) {                                          // layers 0..2: K-steps ks0, ks0 + 1 of both N halves
-            const int layer = j < n0 ? 0 : j < n0 + kKsL12 / 2 ? 1 : 2;
-            const int ks0 = 2 * (layer == 0 ? j : layer == 1 ? j - n0 : j - n0 - kKsL12 / 2);
-            const int nks = layer == 0 ? kKsL0 : kKsL12;
-            const unsigned char* base = seq + 2 * (layer == 0 ? sL0 : layer == 1 ? sL1 : sL2);
-            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * (NP == 3 ? 2 : 1) * 2 * TILE256));
+    if (wgid == 0) {
+        // =============================================================================================== producer warpgroup
+        tc::setmaxnreg_dec<PRODUCER_REGS>();
+        const uint32_t s_hi = s_hi0, s_lo = s_lo0;
+        if (warp == 0) {
+            // ---- warp 0: the weight stream (one elected lane).  Push j of a tile goes to slot g % NUM_SLOTS, g = pushes of the
+            // CTA so far.  A slot is one K-step of both N halves and both planes (layers 0..2), or L3_PUSH K-steps of both
+            // halves of layer 3.  A slot is refilled once every consumer warp has arrived on its empty barrier.
+            if (lane == 0) {
+                tcr::Tracer tl;
+                tl.init(P.trace, 3);
+                const unsigned char* seq = reinterpret_cast<const unsigned char*>(P.wf16);
+                unsigned long long real_tiles = 0, real_ksteps = 0;
+                uint32_t g = 0;
+                for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+                    const TileRef tref = tile_ref(tile);
+                    const int l0_ksteps = class_ksteps(tref.cls);
+                    real_tiles += tref.nrows > 0;
+                    real_ksteps += tref.nrows > 0 ? l0_ksteps : 0;
+                    for (int j = 0; j < pushes_per_tile(l0_ksteps); ++j, ++g) {
+                        const uint32_t slot = g % NUM_SLOTS;
+                        tc::mbar_wait(&bars[B_EMPTY + slot], ((g / NUM_SLOTS) & 1) ^ 1);   // (the first round passes at once)
+                        if (j == 0) tl.ev(1);
+                        unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
+                        uint64_t* bar = &bars[B_FULL + slot];
+                        if (j < l0_ksteps + 2 * kKsL12) {                   // layers 0..2: K-step ks, tile (half h, plane pl) at 2 h + pl
+                            const int layer = j < l0_ksteps ? 0 : j < l0_ksteps + kKsL12 ? 1 : 2;
+                            const int ks = layer == 0 ? j : layer == 1 ? j - l0_ksteps : j - l0_ksteps - kKsL12;
+                            const int nks = layer == 0 ? kKsL0 : kKsL12;
+                            const unsigned char* base = seq + 2 * (layer == 0 ? sL0 : layer == 1 ? sL1 : sL2);
+                            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * (NP == 3 ? 2 : 1) * TILE256));
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
+                            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int pl = 0; pl < (NP == 3 ? 2 : 1); ++pl)
-                    tc::bulk_g2s(dst + (2 * h + pl) * 2 * TILE256, base + 2 * pair_step_offset(ks0, pl, h, nks), 2 * TILE256, bar);
-        } else {                                                        // layer 3: steps [g0, g0 + n) of both N halves
-            const int g0 = (j - n0 - kKsL12) * L3_PUSH;
-            const int n = min(L3_PUSH, kStepsL3 - g0), common = min(n, kStepsL3 - 1 - g0);
-            const bool last = g0 + n == kStepsL3;
-            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * n * TILE3));
+                                for (int pl = 0; pl < (NP == 3 ? 2 : 1); ++pl)
+                                    tc::bulk_g2s(dst + (2 * h + pl) * TILE256, base + 2 * pair_step_offset(ks, pl, h, nks), TILE256, bar);
+                        } else {                                            // layer 3: steps [g0, g0 + n) of both N halves
+                            const int g0 = (j - l0_ksteps - 2 * kKsL12) * L3_PUSH;
+                            const int n = min(L3_PUSH, kStepsL3 - g0), common = min(n, kStepsL3 - 1 - g0);
+                            const bool last = g0 + n == kStepsL3;
+                            tc::mbar_arrive_expect_tx(bar, (uint32_t)(2 * n * TILE3));
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                unsigned char* d = dst + h * (SLOT_BYTES / 2);
-                tc::bulk_g2s(d, seq + 2 * (sL3 + pair_l3_offset(g0, h)), common * TILE3, bar);
-                if (last)                                               // the per-frame step 21 (it carries the frame's bias)
-                    tc::bulk_g2s(d + common * TILE3, reinterpret_cast<const unsigned char*>(P.wframe) + ((size_t)P.frame * 2 + h) * TILE3,
-                                 TILE3, bar);
+                            for (int h = 0; h < 2; ++h) {
+                                unsigned char* d = dst + h * (SLOT_BYTES / 2);
+                                tc::bulk_g2s(d, seq + 2 * (sL3 + pair_l3_offset(g0, h)), common * TILE3, bar);
+                                if (last)                                   // the per-frame step 21 (it carries the frame's bias)
+                                    tc::bulk_g2s(d + common * TILE3, reinterpret_cast<const unsigned char*>(P.wframe) + ((size_t)P.frame * 2 + h) * TILE3,
+                                                 TILE3, bar);
+                            }
+                        }
+                    }
+                    tl.ev(2);
+                }
+                if (P.stats) {
+                    atomicAdd(P.stats + 0, real_tiles);
+                    atomicAdd(P.stats + 4, real_ksteps);
+                    if (blockIdx.x == 0) atomicAdd(P.stats + 1, (unsigned long long)sched->cnt[0] + sched->cnt[1] + sched->cnt[2] + sched->cnt[3]);
+                }
+            }
+            __syncwarp();
+        } else {
+            // ---- warps 1..3: the tiles' list rows (double-buffered) and the per-point tile of layer 3
+            const int pt = tid - 32;                                    // 0 .. NROWT - 1
+            tcr::Tracer tr;
+            tr.init(pt == 0 ? P.trace : nullptr, 0);
+            auto pwait = [&](uint64_t* bar, uint32_t parity) { tc::mbar_wait_backoff(bar, parity, 64); };
+            auto load_rows = [&](float4* dst, int tile) {
+                if (tile < n_tiles) {
+                    const TileRef r = tile_ref(tile);
+                    for (int i = pt; i < TP; i += NROWT)
+                        dst[i] = i < r.nrows ? __ldg(r.ent + i) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
+                }
+                tcr::named_bar_sync(3, NROWT);
+                tc::mbar_arrive(&bars[B_ROWSFULL]);
+            };
+
+            load_rows(rows_buf, blockIdx.x);
+            int it = 0;
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+                const TileRef tref = tile_ref(tile);
+                const int nrows = tref.nrows;
+                const float4* rows = rows_buf + (it & 1) * TP;
+                tr.ev(1);
+
+                // ---- the per-point tile of layer 3 in the lo plane: [PE(xyz) 63 | 0 | PE(view) 27 | 0 | 1 | 1 | 0 | 0]
+                pwait(&bars[B_L2DONE], it & 1);                             // the lo plane's h1 is no longer read
+                tr.ev(31);
+#pragma unroll 1
+                for (int job = pt; job < 2 * TP; job += NROWT) {
+                    const int prow = job % TP;
+                    const float4 e = rows[prow];
+                    auto put = [&](int k, float v) {
+                        const __half hv = __float2half_rn(v);
+                        asm volatile("st.shared.b16 [%0], %1;" ::"r"(s_lo + act_off(prow, k)), "h"(*reinterpret_cast<const unsigned short*>(&hv)) : "memory");
+                    };
+                    if (job < TP) {
+                        positional_embed_anchored<10, 5>(e.x, e.y, e.z, [&](int j, float v) { put(j, v); });
+                        put(63, 0.f);
+                    } else {
+                        const int smp = (int)(__float_as_uint(e.w) & ID_MASK);
+                        const size_t ri = (size_t)P.frame * P.n_rays + (prow < nrows ? smp / S : 0);
+                        const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
+                        const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+                        positional_embed_anchored<4, 4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { put(64 + j, v); });
+                        put(91, 0.f); put(92, 1.f); put(93, 1.f); put(94, 0.f); put(95, 0.f);
+                    }
+                }
+                tc::fence_proxy_async();
+                tc::mbar_arrive(&bars[B_PEFULL]);
+                tr.ev(32);
+                // the other row buffer held the previous tile: its raw records are stored (its layer 2 is long done)
+                load_rows(rows_buf + ((it + 1) & 1) * TP, tile + gridDim.x);
+                tr.ev(30);
             }
         }
-    };
-
-    // this thread's accumulator fragment: rows r0 and r0 + 8 of the tile, columns 8 c + cq + {0, 1} of each 128-column half
-    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
-    float acc0[64], acc1[64];                                      // N halves [0, 128) and [128, 256)
-    auto init_bias = [&](const float* b) {
+    } else {
+        // =============================================================================================== consumer warpgroups
+        tc::setmaxnreg_inc<CONSUMER_REGS>();
+        uint32_t s_hi, s_lo;                                            // the ACT planes (set per tile, below)
+        const int cw = wgid - 1;                                        // rows [64 cw, 64 cw + 64) of a tile
+        const bool arr = lane == 0;                                     // the warp's arrival on the consumer-side barriers
+        tcr::Tracer tr;
+        tr.init((tid & 127) == 0 ? P.trace : nullptr, 1 + cw);
+        // this thread's accumulator fragment: rows r0 and r0 + 8 of the tile, columns 8 c + cq + {0, 1} of each 128-column half
+        const int r0 = 64 * cw + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float acc0[64], acc1[64];                                      // N halves [0, 128) and [128, 256)
+        auto init_bias = [&](const float* b) {
 #pragma unroll
-        for (int c = 0; c < 16; ++c) {
-            const float2 v0 = *reinterpret_cast<const float2*>(b + 8 * c + cq), v1 = *reinterpret_cast<const float2*>(b + 128 + 8 * c + cq);
-            acc0[4 * c] = v0.x; acc0[4 * c + 1] = v0.y; acc0[4 * c + 2] = v0.x; acc0[4 * c + 3] = v0.y;
-            acc1[4 * c] = v1.x; acc1[4 * c + 1] = v1.y; acc1[4 * c + 2] = v1.x; acc1[4 * c + 3] = v1.y;
-        }
-    };
-    const uint32_t wg_rows = (uint32_t)(wg * 8 * 128);              // this warpgroup's first 8-row group in an ACT plane
-    // two K-steps of a 256 -> 256 layer from the slot at `slot`: A K-step ka, ka + 1 (ACT chunk 2 ka)
-    auto mma256 = [&](uint32_t slot, int ka) {
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const uint64_t a_hi = tc::make_smem_desc(s_hi + wg_rows + 2 * (ka + j) * CHUNK_STRIDE, CHUNK_STRIDE, 128);
-            const uint64_t a_lo = tc::make_smem_desc(s_lo + wg_rows + 2 * (ka + j) * CHUNK_STRIDE, CHUNK_STRIDE, 128);
-            const uint64_t b0h = tc::make_smem_desc(slot + 0 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
-            const uint64_t b0l = tc::make_smem_desc(slot + 1 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
-            const uint64_t b1h = tc::make_smem_desc(slot + 2 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
-            const uint64_t b1l = tc::make_smem_desc(slot + 3 * 2 * TILE256 + j * TILE256, 128 * 16, 128);
+            for (int c = 0; c < 16; ++c) {
+                const float2 v0 = *reinterpret_cast<const float2*>(b + 8 * c + cq), v1 = *reinterpret_cast<const float2*>(b + 128 + 8 * c + cq);
+                acc0[4 * c] = v0.x; acc0[4 * c + 1] = v0.y; acc0[4 * c + 2] = v0.x; acc0[4 * c + 3] = v0.y;
+                acc1[4 * c] = v1.x; acc1[4 * c + 1] = v1.y; acc1[4 * c + 2] = v1.x; acc1[4 * c + 3] = v1.y;
+            }
+        };
+        const uint32_t wg_rows = (uint32_t)(cw * 8 * 128);              // this warpgroup's first 8-row group in an ACT plane
+        // one K-step of a 256 -> 256 layer from the slot at `slot`: A K-step ka (ACT chunk 2 ka)
+        auto mma256 = [&](uint32_t slot, int ka) {
+            const uint64_t a_hi = tc::make_smem_desc(s_hi + wg_rows + 2 * ka * CHUNK_STRIDE, CHUNK_STRIDE, 128);
+            const uint64_t a_lo = tc::make_smem_desc(s_lo + wg_rows + 2 * ka * CHUNK_STRIDE, CHUNK_STRIDE, 128);
+            const uint64_t b0h = tc::make_smem_desc(slot + 0 * TILE256, 128 * 16, 128);
+            const uint64_t b0l = tc::make_smem_desc(slot + 1 * TILE256, 128 * 16, 128);
+            const uint64_t b1h = tc::make_smem_desc(slot + 2 * TILE256, 128 * 16, 128);
+            const uint64_t b1l = tc::make_smem_desc(slot + 3 * TILE256, 128 * 16, 128);
             tc::wgmma_m64n128k16_f16(acc0, a_hi, b0h, true);
             tc::wgmma_m64n128k16_f16(acc1, a_hi, b1h, true);
-            if (NP == 3) {                                          // A_lo W_hi + A_hi W_lo
+            if (NP == 3) {                                              // A_lo W_hi + A_hi W_lo
                 tc::wgmma_m64n128k16_f16(acc0, a_lo, b0h, true);
                 tc::wgmma_m64n128k16_f16(acc1, a_lo, b1h, true);
                 tc::wgmma_m64n128k16_f16(acc0, a_hi, b0l, true);
                 tc::wgmma_m64n128k16_f16(acc1, a_hi, b1l, true);
             }
-        }
-    };
-
-    uint32_t pc = 0;                                                // pushes consumed by the earlier tiles
-    unsigned long long real_tiles = 0, real_ksteps = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const TileRef tref = tile_ref(tile);
-        const int nrows = tref.nrows, nseg = class_segments(tref.cls), l0_ksteps = class_ksteps(tref.cls);
-        const int n_push = pushes_per_tile(l0_ksteps);
-        real_tiles += nrows > 0;
-        real_ksteps += nrows > 0 ? l0_ksteps : 0;
-        if (tid == 0) { issue_push(l0_ksteps, 0, pc); issue_push(l0_ksteps, 1, pc + 1); }
-        if (tid < TP) rows[tid] = tid < nrows ? __ldg(tref.ent + tid) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
-        __syncthreads();
-        int jp = 0;                                                 // pushes of this tile consumed
-        // wait for push jp, issue `mma(slot address)`, commit
-        auto consume = [&](auto&& mma) {
-            const uint32_t g = pc + (uint32_t)jp;
-            tc::mbar_wait(&bars[g % NUM_SLOTS], (g / NUM_SLOTS) & 1);
+        };
+        uint32_t g = 0;                                                 // pushes consumed by this CTA
+        uint32_t w_stall = 0, r_stall = 0, pe_stall = 0, g_cycles = 0;  // cycles waited on weights / rows / the per-point tile; gathering
+        // wait for push g, issue `mma(slot address)`, commit
+        auto take = [&](auto&& mma) {
+            const uint32_t s = g % NUM_SLOTS;
+            const uint32_t t0 = (uint32_t)clock();
+            tc::mbar_wait(&bars[B_FULL + s], (g / NUM_SLOTS) & 1);
+            w_stall += (uint32_t)clock() - t0;
             tc::wgmma_fence();
-            mma(s_ring + (g % NUM_SLOTS) * SLOT_BYTES);
+            mma(s_ring + s * SLOT_BYTES);
             tc::wgmma_commit();
-            ++jp;
+            ++g;
         };
-        // the MMAs of the push before the last one are complete in both warpgroups: its slot takes push jp
-        auto retire = [&]() {
-            tc::wgmma_wait<1>();
-            tc::acc_fence(acc0); tc::acc_fence(acc1);
-            tc::fence_proxy_async();
-            __syncthreads();
-            if (tid == 0 && jp >= 2 && jp < n_push) issue_push(l0_ksteps, jp, pc + (uint32_t)jp);
-        };
-        auto drain = [&]() {
-            tc::wgmma_wait<0>();
-            tc::acc_fence(acc0); tc::acc_fence(acc1);
-            __syncthreads();
-        };
-
-        // ---- layer-0 gather: segment seg (64 channels of one level, coarse level first) -> segment buffer seg % SEG_BUFS
-        auto gather = [&](int seg) {
-            const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
-            const int grp = tid >> 3, t = tid & 7;
-            const int lvl = seg < 2 ? 3 : seg < 4 ? 2 : seg < 5 ? 1 : 0;
-            const int cbase0 = seg < 2 ? seg * 64 : seg < 4 ? (seg - 2) * 64 : 0;
-            const int nunits = seg == NUM_SEGS - 1 ? 1 : 2;
-            const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-            const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
-            const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
-            const int kb = 64 * (seg % SEG_BUFS);
-            for (int pp = 0; pp < TP / 32; ++pp) {
-                const int row = 4 * grp + pp;
-                const float4 e = rows[row];
-                const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
-                float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-                if (occ) {
-                    float gx, gy, gz;
-                    world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
-                    Corners cn;
-                    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
-                    // The 8 corners are addressed as (clamped low corner) + constant strides.  A cell that straddles the
-                    // volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted inside by one and
-                    // its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
-                    auto axis = [](int i0, int size, float (&w)[2]) {
-                        if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
-                        if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
-                        if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
-                        return i0;
-                    };
-                    const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
-                    const uint32_t cb = (uint32_t)((zc * H + yc) * W + xc) * dX;
-                    float cw[8];
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
-#pragma unroll
-                    for (int uu = 0; uu < 2; ++uu) {
-                        if (uu >= nunits) continue;
-                        const unsigned char* ub = lvl_ptr + (size_t)(cbase0 + 32 * uu) * sizeof(VT);
-#pragma unroll
-                        for (int h = 0; h < 8; h += 4) {
-                            typename Quad<VT>::raw v[4];
-#pragma unroll
-                            for (int c = 0; c < 4; ++c)
-                                v[c] = Quad<VT>::load_bytes(ub + cb + (((h + c) & 1) ? dX : 0u) + (((h + c) & 2) ? dY : 0u) + (((h + c) & 4) ? dZ : 0u));
-#pragma unroll
-                            for (int c = 0; c < 4; ++c)
-                                if (cw[h + c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw[h + c]);
-                        }
-                    }
-                }
-#pragma unroll
-                for (int uu = 0; uu < 2; ++uu) {
-                    if (uu >= nunits) continue;
-                    const float (&a)[4] = acc[uu];
-                    const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
-                    uint2 hw, lw;
-                    if (NP == 3) {
-                        // (hi, lo) split with a truncated hi: the residual is exact
-                        hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
-                        float q0, q1, q2, q3;
-                        tc::trunc_residual2(a[0], a[1], q0, q1);
-                        tc::trunc_residual2(a[2], a[3], q2, q3);
-                        lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
-                        tcr::sts_v2(s_lo + off, lw);
-                    } else {
-                        hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
-                    }
-                    tcr::sts_v2(s_hi + off, hw);
-                }
-            }
-            tc::fence_proxy_async();
-        };
+        auto release = [&](uint32_t gp, bool pred) { tc::mbar_arrive_if(&bars[B_EMPTY + gp % NUM_SLOTS], pred); };
+        auto release_last = [&]() { release(g - 1, arr); };
 
         // ---- epilogue of a 256-wide layer: relu -> fp16 (hi, lo) operand of the next layer in the ACT planes (own rows only).
         // h2 (`last`) is rounded to nearest, hi only: layer 3 is a 1-pass layer.  Returns this thread's share of alpha_fc . h2.
@@ -451,133 +467,219 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             one(acc1, 1);
             return make_float2(sig0, sig1);
         };
-
-        // ================= layer 0
-        init_bias(head + H_B0);
-        gather(0);
-        __syncthreads();
-        for (int seg = 0; seg < nseg; ++seg) {
-            const int nks = seg == NUM_SEGS - 1 ? 2 : 4;
-            const int ka = 4 * (seg % SEG_BUFS);
-            for (int q = 0; q < nks; q += 2) {
-                consume([&](uint32_t slot) { mma256(slot, ka + q); });
-                if (q + 2 >= nks && seg + 1 < nseg) gather(seg + 1);    // under the MMAs just issued
-                retire();
-            }
-        }
-        drain();
-        convert(false);                                             // h0
-        init_bias(head + H_B0 + kHidden);
-        tc::fence_proxy_async();
-        __syncthreads();
-        // ================= layers 1, 2
-        float2 sig = make_float2(0.f, 0.f);
-        for (int layer = 1; layer <= 2; ++layer) {
-            for (int q = 0; q < kKsL12; q += 2) {
-                consume([&](uint32_t slot) { mma256(slot, q); });
-                retire();
-            }
-            drain();
-            if (layer == 1) {
-                convert(false);                                     // h1
-                init_bias(head + H_B0 + 2 * kHidden);
-            } else {
-                sig = convert(true);                                // h2, and this thread's share of sigma
-            }
-            if (layer == 2) {
-                // the per-point tile of layer 3 in the lo plane: [PE(xyz) 63 | 0 | PE(view) 27 | 0 | 1 | 1 | 0 | 0]
-                const int prow = 64 * wg + (tid & 63);
-                const float4 e = rows[prow];
-                auto put = [&](int k, float v) {
-                    const __half hv = __float2half_rn(v);
-                    asm volatile("st.shared.b16 [%0], %1;" ::"r"(s_lo + act_off(prow, k)), "h"(*reinterpret_cast<const unsigned short*>(&hv)) : "memory");
-                };
-                if ((tid & 127) < 64) {
-                    positional_embed_anchored<10, 5>(e.x, e.y, e.z, [&](int j, float v) { put(j, v); });
-                    put(63, 0.f);
-                } else {
-                    const int smp = (int)(__float_as_uint(e.w) & ID_MASK);
-                    const size_t ri = (size_t)P.frame * P.n_rays + (prow < nrows ? smp / S : 0);
-                    const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
-                    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
-                    positional_embed_anchored<4, 4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { put(64 + j, v); });
-                    put(91, 0.f); put(92, 1.f); put(93, 1.f); put(94, 0.f); put(95, 0.f);
-                }
-            }
+        // the epilogue's stores become the warpgroup's next A operand
+        auto publish = [&]() {
             tc::fence_proxy_async();
-            __syncthreads();
-        }
-        // ================= layer 3 (the folded colour layer, N = 128 as two halves of 64): A = h2 (hi plane) for K-steps
-        // 0..15, the per-point tile (lo plane) for 16..21
-        float c3a[32], c3b[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) { c3a[i] = 0.f; c3b[i] = 0.f; }
-#pragma unroll
-        for (int g0 = 0; g0 < kStepsL3; g0 += L3_PUSH) {
-            consume([&](uint32_t slot) {
-#pragma unroll
-                for (int k = 0; k < L3_PUSH; ++k) {
-                    const int ks = g0 + k;
-                    if (ks >= kStepsL3) break;
-                    const uint32_t a = ks < 16 ? s_hi + 2 * ks * CHUNK_STRIDE : s_lo + 2 * (ks - 16) * CHUNK_STRIDE;
-                    const uint64_t ad = tc::make_smem_desc(a + wg_rows, CHUNK_STRIDE, 128);
-                    tc::wgmma_m64n64k16_f16(c3a, ad, tc::make_smem_desc(slot + k * TILE3, 64 * 16, 128), true);
-                    tc::wgmma_m64n64k16_f16(c3b, ad, tc::make_smem_desc(slot + SLOT_BYTES / 2 + k * TILE3, 64 * 16, 128), true);
-                }
-            });
-            tc::wgmma_wait<1>();
-            tc::acc_fence(c3a); tc::acc_fence(c3b);
-            __syncthreads();
-            if (tid == 0 && jp >= 2 && jp < n_push) issue_push(l0_ksteps, jp, pc + (uint32_t)jp);
-        }
-        tc::wgmma_wait<0>();
-        tc::acc_fence(c3a); tc::acc_fence(c3b);
-        // ---- the colour head: rgb = rgb_fc . relu(layer-3 accumulator) + bias, and sigma = alpha_fc . h2 + bias, fp32
-        float cr[2] = {0.f, 0.f}, cg[2] = {0.f, 0.f}, cbl[2] = {0.f, 0.f};
-        auto color = [&](const float (&a)[32], int nh) {
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const int col = 64 * nh + 8 * c + cq;
-                const float2 w0 = *reinterpret_cast<const float2*>(head + H_RGBW + col);
-                const float2 w1 = *reinterpret_cast<const float2*>(head + H_RGBW + kColor + col);
-                const float2 w2 = *reinterpret_cast<const float2*>(head + H_RGBW + 2 * kColor + col);
-#pragma unroll
-                for (int hr = 0; hr < 2; ++hr) {
-                    const float x0 = fmaxf(a[4 * c + 2 * hr], 0.f), x1 = fmaxf(a[4 * c + 2 * hr + 1], 0.f);
-                    cr[hr] = fmaf(x1, w0.y, fmaf(x0, w0.x, cr[hr]));
-                    cg[hr] = fmaf(x1, w1.y, fmaf(x0, w1.x, cg[hr]));
-                    cbl[hr] = fmaf(x1, w2.y, fmaf(x0, w2.x, cbl[hr]));
-                }
-            }
+            tcr::named_bar_sync(1 + cw, 128);
         };
-        color(c3a, 0);
-        color(c3b, 1);
-        float sg[2] = {sig.x, sig.y};
+
+        int it = 0;
+        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+            const TileRef tref = tile_ref(tile);
+            const int nrows = tref.nrows, nseg = class_segments(tref.cls);
+            const float4* rows = rows_buf + (it & 1) * TP;
+            // the plane bases are re-read per tile: otherwise ptxas hoists every K-step's descriptor out of the tile loop and
+            // spills them
+            asm volatile("mov.u32 %0, %1;" : "=r"(s_hi) : "r"(s_hi0));
+            asm volatile("mov.u32 %0, %1;" : "=r"(s_lo) : "r"(s_lo0));
+            tr.ev(1);
+                // ---- layer-0 gather of this warpgroup's rows: segment seg (64 channels of one level, coarse level first) -> segment
+            // buffer seg % SEG_BUFS.  It runs while none of the warpgroup's wgmma are in flight; the other warpgroup's MMAs overlap it.
+            auto gather = [&](int seg) {
+                const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
+                const int grp = (tid & 127) >> 3, t = tid & 7;
+                const int lvl = seg < 2 ? 3 : seg < 4 ? 2 : seg < 5 ? 1 : 0;
+                const int cbase0 = seg < 2 ? seg * 64 : seg < 4 ? (seg - 2) * 64 : 0;
+                const int nunits = seg == NUM_SEGS - 1 ? 1 : 2;
+                const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+                const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
+                const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
+                const int kb = 64 * (seg % SEG_BUFS);
+                for (int row = 64 * cw + grp; row < 64 * cw + 64; row += 16) {
+                    const float4 e = rows[row];
+                    const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
+                    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+                    if (occ) {
+                        float gx, gy, gz;
+                        world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+                        Corners cn;
+                        corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+                        // The 8 corners are addressed as (clamped low corner) + constant strides.  A cell that straddles the
+                        // volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted inside by one and
+                        // its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
+                        auto axis = [](int i0, int size, float (&w)[2]) {
+                            if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
+                            if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
+                            if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
+                            return i0;
+                        };
+                        const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
+                        const uint32_t cb = (uint32_t)((zc * H + yc) * W + xc) * dX;
+                        float cw[8];
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
+                        for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
 #pragma unroll
-            for (int o = 1; o <= 2; o <<= 1) {
-                cr[hr] += __shfl_xor_sync(0xffffffffu, cr[hr], o);
-                cg[hr] += __shfl_xor_sync(0xffffffffu, cg[hr], o);
-                cbl[hr] += __shfl_xor_sync(0xffffffffu, cbl[hr], o);
-                sg[hr] += __shfl_xor_sync(0xffffffffu, sg[hr], o);
+                        for (int uu = 0; uu < 2; ++uu) {
+                            if (uu >= nunits) continue;
+                            const unsigned char* ub = lvl_ptr + (size_t)(cbase0 + 32 * uu) * sizeof(VT);
+                            typename Quad<VT>::raw v[8];
+#pragma unroll
+                            for (int c = 0; c < 8; ++c)
+                                v[c] = Quad<VT>::load_bytes(ub + cb + ((c & 1) ? dX : 0u) + ((c & 2) ? dY : 0u) + ((c & 4) ? dZ : 0u));
+#pragma unroll
+                            for (int c = 0; c < 8; ++c)
+                                if (cw[c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw[c]);
+                        }
+                    }
+#pragma unroll
+                    for (int uu = 0; uu < 2; ++uu) {
+                        if (uu >= nunits) continue;
+                        const float (&a)[4] = acc[uu];
+                        const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
+                        uint2 hw, lw;
+                        if (NP == 3) {
+                            // (hi, lo) split with a truncated hi: the residual is exact
+                            hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
+                            float q0, q1, q2, q3;
+                            tc::trunc_residual2(a[0], a[1], q0, q1);
+                            tc::trunc_residual2(a[2], a[3], q2, q3);
+                            lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
+                            tcr::sts_v2(s_lo + off, lw);
+                        } else {
+                            hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
+                        }
+                        tcr::sts_v2(s_hi + off, hw);
+                    }
+                }
+            };
+
+            {
+                const uint32_t t0 = (uint32_t)clock();
+                tc::mbar_wait(&bars[B_ROWSFULL], it & 1);
+                r_stall += (uint32_t)clock() - t0;
             }
-            const int row = r0 + 8 * hr;
-            if ((lane & 3) == 0 && row < nrows) {
-                const int smp = (int)(__float_as_uint(rows[row].w) & ID_MASK);
-                P.raw_ws[smp] = make_float4(cr[hr] + head[H_RGBB], cg[hr] + head[H_RGBB + 1], cbl[hr] + head[H_RGBB + 2],
-                                            sg[hr] + head[H_ALPHA + kHidden]);
+            // ================= layer 0: gather a segment, multiply it (its K-steps pipelined), retire them, gather the next
+            init_bias(head + H_B0);
+            for (int seg = 0; seg < nseg; ++seg) {
+                const uint32_t t0 = (uint32_t)clock();
+                gather(seg);
+                publish();
+                g_cycles += (uint32_t)clock() - t0;
+                const int nks = seg == NUM_SEGS - 1 ? 2 : 4, ka = 4 * (seg % SEG_BUFS);
+                for (int q = 0; q < nks; ++q) {
+                    take([&](uint32_t slot) { mma256(slot, ka + q); });
+                    tc::wgmma_wait<1>();
+                    tc::acc_fence(acc0); tc::acc_fence(acc1);
+                    release(g - 2, arr && q > 0);
+                }
+                tc::wgmma_wait<0>();
+                tc::acc_fence(acc0); tc::acc_fence(acc1);
+                release_last();
             }
+            tr.ev(20);
+            convert(false);                                             // h0
+            init_bias(head + H_B0 + kHidden);
+            publish();
+            // ================= layers 1, 2
+            float2 sig = make_float2(0.f, 0.f);
+            for (int layer = 1; layer <= 2; ++layer) {
+                for (int q = 0; q < kKsL12; ++q) {
+                    take([&](uint32_t slot) { mma256(slot, q); });
+                    tc::wgmma_wait<1>();
+                    tc::acc_fence(acc0); tc::acc_fence(acc1);
+                    release(g - 2, arr && q > 0);
+                }
+                tc::wgmma_wait<0>();
+                tc::acc_fence(acc0); tc::acc_fence(acc1);
+                release_last();
+                tr.ev(20 + layer);
+                if (layer == 1) {
+                    convert(false);                                     // h1
+                    init_bias(head + H_B0 + 2 * kHidden);
+                } else {
+                    tc::mbar_arrive_if(&bars[B_L2DONE], arr);           // the lo plane is free for the per-point tile
+                    sig = convert(true);                                // h2, and this thread's share of sigma
+                }
+                publish();
+            }
+            // ================= layer 3 (the folded colour layer, N = 128 as two halves of 64): A = h2 (hi plane) for K-steps
+            // 0..15, the per-point tile (lo plane) for 16..21
+            float c3a[32], c3b[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { c3a[i] = 0.f; c3b[i] = 0.f; }
+#pragma unroll
+            for (int p = 0; p < L3_PUSHES; ++p) {
+                if (p * L3_PUSH == 16) {                              // the first push that reads the per-point tile
+                    const uint32_t t0 = (uint32_t)clock();
+                    tc::mbar_wait(&bars[B_PEFULL], it & 1);
+                    pe_stall += (uint32_t)clock() - t0;
+                }
+                take([&](uint32_t slot) {
+#pragma unroll
+                    for (int k = 0; k < L3_PUSH; ++k) {
+                        const int ks = p * L3_PUSH + k;
+                        if (ks >= kStepsL3) break;
+                        const uint32_t a = ks < 16 ? s_hi + 2 * ks * CHUNK_STRIDE : s_lo + 2 * (ks - 16) * CHUNK_STRIDE;
+                        const uint64_t ad = tc::make_smem_desc(a + wg_rows, CHUNK_STRIDE, 128);
+                        tc::wgmma_m64n64k16_f16(c3a, ad, tc::make_smem_desc(slot + k * TILE3, 64 * 16, 128), true);
+                        tc::wgmma_m64n64k16_f16(c3b, ad, tc::make_smem_desc(slot + SLOT_BYTES / 2 + k * TILE3, 64 * 16, 128), true);
+                    }
+                });
+                tc::wgmma_wait<1>();
+                tc::acc_fence(c3a); tc::acc_fence(c3b);
+                release(g - 2, arr && p > 0);
+            }
+            tc::wgmma_wait<0>();
+            tc::acc_fence(c3a); tc::acc_fence(c3b);
+            release_last();
+            tr.ev(23);
+            // ---- the colour head: rgb = rgb_fc . relu(layer-3 accumulator) + bias, and sigma = alpha_fc . h2 + bias, fp32
+            float cr[2] = {0.f, 0.f}, cg[2] = {0.f, 0.f}, cbl[2] = {0.f, 0.f};
+            auto color = [&](const float (&a)[32], int nh) {
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    const int col = 64 * nh + 8 * c + cq;
+                    const float2 w0 = *reinterpret_cast<const float2*>(head + H_RGBW + col);
+                    const float2 w1 = *reinterpret_cast<const float2*>(head + H_RGBW + kColor + col);
+                    const float2 w2 = *reinterpret_cast<const float2*>(head + H_RGBW + 2 * kColor + col);
+#pragma unroll
+                    for (int hr = 0; hr < 2; ++hr) {
+                        const float x0 = fmaxf(a[4 * c + 2 * hr], 0.f), x1 = fmaxf(a[4 * c + 2 * hr + 1], 0.f);
+                        cr[hr] = fmaf(x1, w0.y, fmaf(x0, w0.x, cr[hr]));
+                        cg[hr] = fmaf(x1, w1.y, fmaf(x0, w1.x, cg[hr]));
+                        cbl[hr] = fmaf(x1, w2.y, fmaf(x0, w2.x, cbl[hr]));
+                    }
+                }
+            };
+            color(c3a, 0);
+            color(c3b, 1);
+            float sg[2] = {sig.x, sig.y};
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+                for (int o = 1; o <= 2; o <<= 1) {
+                    cr[hr] += __shfl_xor_sync(0xffffffffu, cr[hr], o);
+                    cg[hr] += __shfl_xor_sync(0xffffffffu, cg[hr], o);
+                    cbl[hr] += __shfl_xor_sync(0xffffffffu, cbl[hr], o);
+                    sg[hr] += __shfl_xor_sync(0xffffffffu, sg[hr], o);
+                }
+                const int row = r0 + 8 * hr;
+                if ((lane & 3) == 0 && row < nrows) {
+                    const int smp = (int)(__float_as_uint(rows[row].w) & ID_MASK);
+                    P.raw_ws[smp] = make_float4(cr[hr] + head[H_RGBB], cg[hr] + head[H_RGBB + 1], cbl[hr] + head[H_RGBB + 2],
+                                                sg[hr] + head[H_ALPHA + kHidden]);
+                }
+            }
+            tr.ev(24);
+            tr.val(50, w_stall);
+            tr.val(51, r_stall);
+            tr.val(52, pe_stall);
+            tr.val(53, g_cycles);
+            w_stall = r_stall = pe_stall = g_cycles = 0;
         }
-        pc += (uint32_t)n_push;
-        __syncthreads();                                            // rows / ACT planes / slots are free for the next tile
     }
-    if (tid == 0 && P.stats) {
-        atomicAdd(P.stats + 0, real_tiles);
-        atomicAdd(P.stats + 4, real_ksteps);
-        if (blockIdx.x == 0) atomicAdd(P.stats + 1, (unsigned long long)sched->cnt[0] + sched->cnt[1] + sched->cnt[2] + sched->cnt[3]);
-        atomicMax(P.frame_clock + 1, global_ns());
-    }
+    __syncthreads();
+    if (tid == 0 && P.stats) atomicMax(P.frame_clock + 1, global_ns());
 }
 
 // ------------------------------------------------------------------------------------------------ 3. raw2outputs
@@ -616,7 +718,6 @@ template <int NP, typename VT>
 static cudaError_t launch_list(const RenderParams& p, int grid, cudaStream_t stream) {
     cudaError_t e = cudaFuncSetAttribute(render_tc_list_kernel<NP, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
-    // what the 228 KB array does not spend on shared memory is the L1 the producers' gather lives on: ask for the smallest carve-out
     render_tc_list_kernel<NP, VT><<<grid, NT, SMEM_BYTES, stream>>>(p);
     return cudaGetLastError();
 }

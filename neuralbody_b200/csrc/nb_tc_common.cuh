@@ -31,8 +31,10 @@ struct Tracer {
         buf = (base && blockIdx.x == 0) ? base + role * 4096 : nullptr;
         n = 0;
     }
-    __device__ __forceinline__ void ev(int code) {
-        if (buf && n < 4096) buf[n++] = ((unsigned long long)code << 48) | ((unsigned long long)clock64() & 0xFFFFFFFFFFFFull);
+    __device__ __forceinline__ void ev(int code) { val(code, (unsigned long long)clock64()); }
+    // an event that carries a value (e.g. cycles spent waiting) in place of the clock
+    __device__ __forceinline__ void val(int code, unsigned long long v) {
+        if (buf && n < 4096) buf[n++] = ((unsigned long long)code << 48) | (v & 0xFFFFFFFFFFFFull);
     }
 };
 

@@ -18,6 +18,18 @@ __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive only where `pred` holds, as one predicated instruction: no branch between a wgmma and the wait that retires it
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 st;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(
+                     smem_u32(bar)),
+                 "r"((uint32_t)pred)
+                 : "memory");
+}
+// per-warpgroup register budget (warp-specialised kernels): the producers give registers back, the MMA warpgroups take them
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)),
                  "r"(bytes)

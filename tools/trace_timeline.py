@@ -8,14 +8,13 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 
-PROD = {1: "tile begin (list rows loaded)"}
-PROD.update({10 + s: "seg%d buf free" % s for s in range(6)})
-PROD.update({20 + s: "seg%d gathered" % s for s in range(6)})
-MMA = {1: "tile begin", 20: "L0 issued", 21: "L1 issued", 22: "L2 issued", 23: "L3 issued", 31: "h ready L1", 32: "h ready L2",
-       33: "h ready L3", 34: "h ready L4"}
-MMA.update({10 + s: "seg%d available" % s for s in range(6)})
-EPI = {1: "tile begin", 2: "PE written", 10: "acc L0", 11: "acc L1", 12: "acc L2", 13: "acc L3", 14: "acc L4 (rgb)", 20: "epi L0 done",
-       21: "epi L1 done", 22: "epi L2 done", 23: "epi L3 done"}
+# role 0: the row / per-point-tile warps (thread 32), 1 / 2: the two consumer warpgroups (threads 128 / 256), 3: the weight
+# loader (thread 0)
+PROD = {1: "tile begin", 30: "next tile's rows loaded", 31: "L2 done seen", 32: "per-point tile written"}
+MMA = {1: "tile begin", 20: "L0 retired", 21: "L1 retired", 22: "L2 retired", 23: "L3 retired", 24: "raw stored"}
+LOAD = {1: "first push of a tile issued", 2: "last push of a tile issued"}
+VALUES = {50: "weight wait", 51: "row wait", 52: "per-point tile wait", 53: "gather"}     # cycles per tile, not clocks
+LAYERS = [(1, 20, "L0"), (20, 21, "L1"), (21, 22, "L2"), (22, 23, "L3"), (23, 24, "head")]
 
 
 def main():
@@ -40,9 +39,8 @@ def main():
             ren.render_rays(batch["ray_o"], batch["ray_d"], batch["near"], batch["far"], vol, sp, trace=trace)
     torch.cuda.synchronize()
     t = trace.cpu().view(4, 4096)
-    MMA.update({40: "slot wait", 41: "slot: own half landed", 42: "slot: peer half landed", 44: "h wait", 45: "h ready"})
-    LOAD = {1: "tile begin", 2: "push: wait for a free slot", 3: "push: slot free, copy issued"}
-    roles = [("PROD", PROD, 13, 1), ("MMA", MMA, None, 1), ("EPI", EPI, None, 1), ("LOAD", LOAD, None, 1)]
+    roles = [("PROD", PROD, None, 1), ("MMA0", MMA, None, 1), ("MMA1", MMA, None, 1), ("LOAD", LOAD, None, 1)]
+    per_tile = {}                                            # (role, tile) -> {code: clock or value}
     events = []
     for r, (name, names, _, begin_code) in enumerate(roles):
         tile = -1
@@ -52,6 +50,9 @@ def main():
             code, clk = (v >> 48) & 0xFFFF, v & 0xFFFFFFFFFFFF
             if code == begin_code:
                 tile += 1
+            per_tile.setdefault((name, tile), {})[code] = clk
+            if code in VALUES:
+                continue
             events.append((clk, name, tile, names.get(code, str(code))))
     events.sort()
     for first in firsts:
@@ -65,14 +66,17 @@ def main():
             d = clk - last.get(name, clk)
             last[name] = clk
             print("%9d  (+%6d)  %-5s tile %-3d %s" % (clk - t0, d, name, tile, what))
-    # per-tile period of the MMA role
-    begins = [e[0] for e in events if e[1] == "MMA" and e[3] == "tile begin"]
-    if len(begins) > 3:
-        per = [b - a for a, b in zip(begins[:-1], begins[1:])]
-        print("MMA tile period (cycles): mean %.0f  min %d  max %d  over %d tiles" % (sum(per) / len(per), min(per), max(per), len(per)))
-        for lo in range(0, len(per), 40):
-            chunk = per[lo:lo + 40]
-            print("  tiles %3d..%3d: mean period %.0f" % (lo, lo + len(chunk) - 1, sum(chunk) / len(chunk)))
+    # per-tile summary of the consumer warpgroups: cycles per layer, cycles waited on weights / rows / the per-point tile, and
+    # cycles spent gathering layer 0's features
+    for name in ("MMA0", "MMA1"):
+        tiles = [d for (r, _), d in sorted(per_tile.items()) if r == name and all(c in d for c in (1, 20, 21, 22, 23, 24, 50))]
+        if len(tiles) < 2:
+            continue
+        tiles = tiles[1:]                                    # the first tile includes the pipeline fill
+        row = ["%s %.0f" % (lbl, sum(d[b] - d[a] for d in tiles) / len(tiles)) for a, b, lbl in LAYERS]
+        nxt = [b[1] - a[1] for a, b in zip(tiles[:-1], tiles[1:])]
+        print("%s, mean over %d tiles (cycles): %s | tile period %.0f" % (name, len(tiles), "  ".join(row), sum(nxt) / max(1, len(nxt))))
+        print("    per tile: " + "  ".join("%s %.0f" % (lbl, sum(d.get(c, 0) for d in tiles) / len(tiles)) for c, lbl in VALUES.items()))
 
 
 if __name__ == "__main__":
