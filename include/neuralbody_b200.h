@@ -148,8 +148,10 @@ typedef struct nb_render_args {
                               0 = every sample goes through the decoder (same maps bit for bit) */
     unsigned long long* stats; /* device u64[8] or NULL: [0] += 128-sample tiles executed, [1] += listed samples,
                                   [4] += layer-0 K-steps executed by those tiles (8 / 16 / 20 / 22 per tile, see below),
-                                  [2] += ns spent in the decoder kernel (%globaltimer, first CTA start to last CTA end) and
-                                  [3] += decoder launches (tensor-core precisions) */
+                                  [2] += ns spent in the decoder kernel (%globaltimer, first CTA start to last CTA end),
+                                  [3] += decoder launches (tensor-core precisions), [5] / [6] += 64-row half tiles whose
+                                  coarse-level (3 and 2) layer-0 features were gathered from the shared-memory staging /
+                                  directly from global memory (more distinct voxels than the staging holds) */
     float* save;           /* device (B,n,S,1312) activation record for nb_render_bwd, or NULL (NB_PRECISION_FP32 only);
                               size from nb_render_save_bytes() */
     unsigned long long* trace; /* device, 4 x 4096 u64, or NULL: per-role (code<<48 | SM clock) timeline of CTA 0

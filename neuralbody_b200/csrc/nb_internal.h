@@ -42,7 +42,8 @@ struct RenderParams {
     int mask_nv, mask_H, mask_W;
     const float *mask_R0, *mask_Th0;   // single-view _msk variant: SMPL -> snapshot-world transform, or null
     unsigned long long* stats; // u64[8] or null: [4] += layer-0 K-steps executed (x 128 rows); [0] += tiles executed, [1] += listed samples,
-                               // [2] += decoder-kernel ns, [3] += decoder launches
+                               // [2] += decoder-kernel ns, [3] += decoder launches, [5] / [6] += coarse-level half tiles
+                               // gathered from the staging / directly
     float* save;               // (B,n,S,kSaveDim) activation record for nb_render_bwd (exact kernel only) or null
     int rays_per_group;        // rays handled together by one CTA work item
     int tiles_per_group;       // point tiles per group

@@ -145,8 +145,9 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
 // One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  The CTA is warp-specialised:
 //   producer warpgroup (warps 0-3)   warp 0: one elected lane streams the weights with bulk copies into a 4-slot ring (one
-//                                     K-step of both N halves and both planes per slot).  Warps 1-3: each tile's list rows
-//                                     (double-buffered) and layer 3's per-point tile.
+//                                     K-step of both N halves and both planes per slot).  Warps 1-3: each tile's list rows and
+//                                     coarse-level voxel table (double-buffered, built one tile ahead) and layer 3's
+//                                     per-point tile.
 //   consumer warpgroups 1 and 2      rows [0, 64) and [64, 128) of a tile: gather layer 0's feature segments of their own rows,
 //                                     issue the wgmma and run the epilogues.  Nothing divergent sits between a wgmma and the
 //                                     wait that retires it (the gather runs only while none of the warpgroup's wgmma are in
@@ -160,7 +161,8 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 //   accumulators  fp32 in registers (two m64n128 halves per warpgroup), started from the fp32 bias of the layer.
 // Barriers (mbarrier phases; every wait is bounded by the watchdog):
 //   full[s] / empty[s]   weight slot s: bulk-copy transaction bytes / one arrival per consumer warp
-//   rows_full            the tile's list rows are loaded (every row thread)
+//   rows_full            the tile's list rows and voxel table are ready (every row thread)
+//   rows_free            every consumer warp has begun the tile, so the other row buffer is free (one arrival per consumer warp)
 //   l2_done, pe_full     the consumers' layer-2 MMAs are complete, so the lo plane is free (one arrival per consumer warp) /
 //                        the per-point tile is written (every row thread)
 constexpr int NT = 384;                                            // producer warpgroup + two consumer warpgroups
@@ -187,11 +189,32 @@ constexpr int OFF_HEAD = OFF_RING + NUM_SLOTS * SLOT_BYTES;
 constexpr int OFF_XF = OFF_HEAD + HEAD_FLOATS * 4;
 constexpr int OFF_SCHED = OFF_XF + 128;
 constexpr int OFF_ROWS = OFF_SCHED + 64;                           // two tiles' list entries (float4 per row)
-constexpr int OFF_BAR = OFF_ROWS + 2 * TP * 16;
-enum { B_FULL = 0, B_EMPTY = B_FULL + NUM_SLOTS, B_ROWSFULL = B_EMPTY + NUM_SLOTS, B_L2DONE, B_PEFULL, NUM_BARS };
+// Layer-0 voxel tables of the two coarse levels (3 and 2, 128 channels each).  A 64-row half tile of neighbouring samples
+// touches a few dozen distinct voxels of a coarse level but requests 512 corner vectors; the row warps list the distinct ones
+// one tile ahead, and the consumer warpgroup copies each of them once into idle segment buffers of its own ACT-plane rows
+// and blends from there.  Table t = 2 * half + li (li 0: level 3, 1: level 2).
+constexpr int NV = 64;                                             // staged voxels per half tile and level (ACT room: fp32
+                                                                   // 64 x 512 B = 2 segment buffers of both planes)
+constexpr int NTAB = 4;
+constexpr int HBITS = 7, HSIZE = 1 << HBITS;                       // open-addressed hash per table (build scratch)
+constexpr uint32_t HEMPTY = 0xFFFFFFFFu;
+constexpr int kCoarseC = 128;                                      // channels of levels 3 and 2 (two K segments each)
+struct VoxTable {
+    unsigned char slot[TP][2][8];                                  // per row and level: the staged slot of each corner
+    uint32_t ids[NTAB][NV];                                        // the distinct voxels (linear index (z H + y) W + x)
+    uint32_t n[NTAB];                                              // their number; > NV: the level is gathered directly
+};
+constexpr int OFF_VTAB = OFF_ROWS + 2 * TP * 16;                   // two tiles' tables (double-buffered like the rows)
+constexpr int OFF_HKEY = OFF_VTAB + 2 * (int)sizeof(VoxTable);
+constexpr int OFF_HVAL = OFF_HKEY + NTAB * HSIZE * 4;
+constexpr int OFF_HCNT = OFF_HVAL + NTAB * HSIZE;
+constexpr int OFF_BAR = OFF_HCNT + (NTAB + 2) * 4;                 // + the CTA's staged / direct half-tile counts
+enum { B_FULL = 0, B_EMPTY = B_FULL + NUM_SLOTS, B_ROWSFULL = B_EMPTY + NUM_SLOTS, B_L2DONE, B_PEFULL, B_ROWSFREE, NUM_BARS };
 constexpr int SMEM_BYTES = OFF_BAR + NUM_BARS * 8;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-static_assert(OFF_RING % 128 == 0 && OFF_HEAD % 16 == 0 && OFF_ROWS % 16 == 0 && OFF_BAR % 8 == 0, "alignment");
+static_assert(OFF_RING % 128 == 0 && OFF_HEAD % 16 == 0 && OFF_ROWS % 16 == 0 && OFF_VTAB % 16 == 0 && OFF_HKEY % 16 == 0 &&
+              OFF_BAR % 8 == 0, "alignment");
+static_assert(NV * kCoarseC * 4 <= 2 * 2 * 8 * 1024 && NV <= 255 && HSIZE > NV, "voxel staging");
 static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NT * LAUNCH_REGS, "register pool of the CTA");
 
 // weight pushes of a tile whose layer 0 runs l0_ksteps K-steps: one per K-step of layers 0..2, layer 3 in groups of L3_PUSH
@@ -199,6 +222,23 @@ __host__ __device__ constexpr int pushes_per_tile(int l0_ksteps) { return l0_kst
 
 __device__ __forceinline__ uint32_t act_off(int row, int k) {      // byte offset of element (row, k) in an ACT plane
     return (uint32_t)((k >> 3) * CHUNK_STRIDE + (row >> 3) * 128 + (row & 7) * 16 + (k & 7) * 2);
+}
+
+// The trilinear cell of a sample on one level, as the gather addresses it: its 8 corners are (clamped low corner) + {0, 1}
+// per axis.  A cell that straddles the volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted
+// inside by one and its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
+// Returns the low corner's voxel index (z H + y) W + x; cn holds the (moved) weights.  The row warps that list a tile's
+// voxels and the consumers that blend them both call this, so the two cannot disagree.
+__device__ __forceinline__ uint32_t clamped_cell(float gx, float gy, float gz, int W, int H, int D, Corners& cn) {
+    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+    auto axis = [](int i0, int size, float (&w)[2]) {
+        if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
+        if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
+        if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
+        return i0;
+    };
+    const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
+    return (uint32_t)((zc * H + yc) * W + xc);
 }
 
 template <int NP, typename VT>
@@ -222,6 +262,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         tc::mbar_init(&bars[B_ROWSFULL], NROWT);
         tc::mbar_init(&bars[B_L2DONE], 8);
         tc::mbar_init(&bars[B_PEFULL], NROWT);
+        tc::mbar_init(&bars[B_ROWSFREE], 8);
         tc::fence_mbar_init();
     }
     load_frame_xf(P, xf, tid);
@@ -235,6 +276,8 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         }
         head[i] = v;
     }
+    for (int i = tid; i < NTAB * HSIZE; i += NT) reinterpret_cast<uint32_t*>(smem + OFF_HKEY)[i] = HEMPTY;
+    if (tid < NTAB + 2) reinterpret_cast<uint32_t*>(smem + OFF_HCNT)[tid] = 0u;
     struct Sched { unsigned int cnt[4]; int start[4]; int n_tiles; };
     Sched* sched = reinterpret_cast<Sched*>(smem + OFF_SCHED);
     if (tid == 0) {
@@ -324,29 +367,113 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             }
             __syncwarp();
         } else {
-            // ---- warps 1..3: the tiles' list rows (double-buffered) and the per-point tile of layer 3
+            // ---- warps 1..3: the tiles' list rows and voxel tables (double-buffered) and the per-point tile of layer 3
             const int pt = tid - 32;                                    // 0 .. NROWT - 1
+            VoxTable* vtabs = reinterpret_cast<VoxTable*>(smem + OFF_VTAB);
+            uint32_t* hkey = reinterpret_cast<uint32_t*>(smem + OFF_HKEY);
+            unsigned char* hval = smem + OFF_HVAL;
+            uint32_t* hcnt = reinterpret_cast<uint32_t*>(smem + OFF_HCNT);
             tcr::Tracer tr;
             tr.init(pt == 0 ? P.trace : nullptr, 0);
             auto pwait = [&](uint64_t* bar, uint32_t parity) { tc::mbar_wait_backoff(bar, parity, 64); };
-            auto load_rows = [&](float4* dst, int tile) {
+            // insert voxel `id` into table `tab`'s hash: its hash position, or 0xFF once the table holds more than NV voxels
+            // (the consumers then gather that level directly and never read the slots)
+            auto insert = [&](int tab, uint32_t id, VoxTable* vt) -> uint32_t {
+                if (*reinterpret_cast<volatile uint32_t*>(hcnt + tab) > (uint32_t)NV) return 0xFFu;
+                uint32_t* keys = hkey + tab * HSIZE;
+                uint32_t h = (id * 2654435761u) >> (32 - HBITS);
+#pragma unroll 1
+                for (int p = 0; p < HSIZE; ++p, h = (h + 1) & (HSIZE - 1)) {
+                    uint32_t k = *reinterpret_cast<volatile uint32_t*>(keys + h);
+                    if (k == HEMPTY) k = atomicCAS(keys + h, HEMPTY, id);
+                    if (k == HEMPTY) {                                  // claimed: the voxel's slot is the next free one
+                        const uint32_t s = atomicAdd(hcnt + tab, 1u);
+                        if (s < (uint32_t)NV) vt->ids[tab][s] = id;
+                        hval[tab * HSIZE + h] = (unsigned char)min(s, 255u);
+                        return h;
+                    }
+                    if (k == id) return h;
+                }
+                return 0xFFu;                                           // (a full hash already holds HSIZE > NV voxels)
+            };
+            // The voxel table of a tile whose rows are in `rows`: per half tile and coarse level its distinct corner voxels
+            // and, per row, the slot of each of the 8 corners.  Insert (slot bytes = hash positions), then resolve them.
+            auto build_table = [&](VoxTable* vt, const float4* rows, int nrows, int nlev) {
+#pragma unroll 1
+                for (int row = pt; row < TP; row += NROWT) {
+                    const float4 e = rows[row];
+                    float gx, gy, gz;
+                    world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+#pragma unroll 1
+                    for (int li = 0; li < nlev; ++li) {
+                        const int lvl = 3 - li, tab = 2 * (row >> 6) + li;
+                        uint32_t w[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
+                        if (row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u)) {
+                            const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+                            Corners cn;
+                            const uint32_t base = clamped_cell(gx, gy, gz, W, H, D, cn);
+#pragma unroll
+                            for (int c = 0; c < 8; ++c) {
+                                const uint32_t id = base + ((c & 1) ? 1u : 0u) + ((c & 2) ? (uint32_t)W : 0u) + ((c & 4) ? (uint32_t)(W * H) : 0u);
+                                const uint32_t h = insert(tab, id, vt);
+                                w[c >> 2] = (w[c >> 2] & ~(0xFFu << (8 * (c & 3)))) | (h << (8 * (c & 3)));
+                            }
+                        }
+                        *reinterpret_cast<uint2*>(&vt->slot[row][li][0]) = make_uint2(w[0], w[1]);
+                    }
+                }
+                tcr::named_bar_sync(3, NROWT);
+                uint32_t* words = reinterpret_cast<uint32_t*>(&vt->slot[0][0][0]);
+#pragma unroll 1
+                for (int i = pt; i < TP * 2 * 2; i += NROWT) {          // word i: row i / 4, level i / 2 % 2
+                    const int li = (i >> 1) & 1;
+                    if (li >= nlev) continue;
+                    const unsigned char* hv = hval + (2 * ((i >> 2) >> 6) + li) * HSIZE;
+                    uint32_t wd = words[i], out = 0u;
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) {
+                        const uint32_t h = (wd >> (8 * b)) & 0xFFu;
+                        out |= (h == 0xFFu ? 0xFFu : (uint32_t)hv[h]) << (8 * b);
+                    }
+                    words[i] = out;
+                }
+                for (int i = pt; i < NTAB * HSIZE; i += NROWT) hkey[i] = HEMPTY;   // (the keys are not read past the insert)
+                if (pt < NTAB) {
+                    const uint32_t n = hcnt[pt];
+                    vt->n[pt] = n;
+                    hcnt[pt] = 0u;
+                    if ((pt & 1) < nlev && nrows > 64 * (pt >> 1)) atomicAdd(hcnt + NTAB + (n <= (uint32_t)NV ? 0 : 1), 1u);
+                }
+            };
+            // a tile's rows and its voxel table into buffer `buf`, published through rows_full
+            auto load_rows = [&](int buf, int tile) {
                 if (tile < n_tiles) {
                     const TileRef r = tile_ref(tile);
+                    float4* dst = rows_buf + buf * TP;
                     for (int i = pt; i < TP; i += NROWT)
                         dst[i] = i < r.nrows ? __ldg(r.ent + i) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
+                    tcr::named_bar_sync(3, NROWT);
+                    build_table(vtabs + buf, dst, r.nrows, class_segments(r.cls) >= 4 ? 2 : 1);
                 }
                 tcr::named_bar_sync(3, NROWT);
                 tc::mbar_arrive(&bars[B_ROWSFULL]);
             };
 
-            load_rows(rows_buf, blockIdx.x);
-            int it = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+            // Tile it: once every consumer warp has begun it (rows_free), the other row buffer's tile is finished; the next
+            // tile's rows and voxel table are loaded there while this tile's layers 0-2 run, then comes this tile's per-point
+            // tile.  load_rows has one call site: iteration it = -1 only loads the first tile.
+            int it = -1;
+            for (int tile = (int)blockIdx.x - (int)gridDim.x; tile < n_tiles; tile += gridDim.x, ++it) {
+                if (it >= 0) {
+                    pwait(&bars[B_ROWSFREE], it & 1);
+                    tr.ev(1);
+                }
+                load_rows((it + 1) & 1, tile + gridDim.x);
+                if (it < 0) continue;
+                tr.ev(30);
                 const TileRef tref = tile_ref(tile);
                 const int nrows = tref.nrows;
                 const float4* rows = rows_buf + (it & 1) * TP;
-                tr.ev(1);
-
                 // ---- the per-point tile of layer 3 in the lo plane: [PE(xyz) 63 | 0 | PE(view) 27 | 0 | 1 | 1 | 0 | 0]
                 pwait(&bars[B_L2DONE], it & 1);                             // the lo plane's h1 is no longer read
                 tr.ev(31);
@@ -373,9 +500,6 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 tc::fence_proxy_async();
                 tc::mbar_arrive(&bars[B_PEFULL]);
                 tr.ev(32);
-                // the other row buffer held the previous tile: its raw records are stored (its layer 2 is long done)
-                load_rows(rows_buf + ((it + 1) & 1) * TP, tile + gridDim.x);
-                tr.ev(30);
             }
         }
     } else {
@@ -384,8 +508,13 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         uint32_t s_hi, s_lo;                                            // the ACT planes (set per tile, below)
         const int cw = wgid - 1;                                        // rows [64 cw, 64 cw + 64) of a tile
         const bool arr = lane == 0;                                     // the warp's arrival on the consumer-side barriers
-        tcr::Tracer tr;
-        tr.init((tid & 127) == 0 ? P.trace : nullptr, 1 + cw);
+        // trace events of the warpgroup (CTA 0, its first thread): only the entry index lives in a register, the buffer is
+        // read from the kernel parameters at each event (same records as tcr::Tracer)
+        int tn = ((tid & 127) == 0 && blockIdx.x == 0 && P.trace) ? (1 + cw) * 4096 : -1;
+        auto tval = [&](int code, unsigned long long v) {
+            if (tn >= 0 && tn < (2 + cw) * 4096) P.trace[tn++] = ((unsigned long long)code << 48) | (v & 0xFFFFFFFFFFFFull);
+        };
+        auto tev = [&](int code) { tval(code, (unsigned long long)clock64()); };
         // this thread's accumulator fragment: rows r0 and r0 + 8 of the tile, columns 8 c + cq + {0, 1} of each 128-column half
         const int r0 = 64 * cw + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
         float acc0[64], acc1[64];                                      // N halves [0, 128) and [128, 256)
@@ -482,42 +611,104 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             // spills them
             asm volatile("mov.u32 %0, %1;" : "=r"(s_hi) : "r"(s_hi0));
             asm volatile("mov.u32 %0, %1;" : "=r"(s_lo) : "r"(s_lo0));
-            tr.ev(1);
-                // ---- layer-0 gather of this warpgroup's rows: segment seg (64 channels of one level, coarse level first) -> segment
+            tev(1);
+            // ---- layer-0 gather of this warpgroup's rows: segment seg (64 channels of one level, coarse level first) -> segment
             // buffer seg % SEG_BUFS.  It runs while none of the warpgroup's wgmma are in flight; the other warpgroup's MMAs overlap it.
+            // Levels 3 and 2 (segments 0-3) are staged: at a level's first segment the warpgroup copies its half tile's distinct
+            // voxels (all 128 channels) with cp.async into the level's two idle segment buffers of its own rows (level 3: buffers
+            // 2, 3; level 2: buffers 0, 1; the warpgroup's MMAs on them are retired), and both segments blend from there.  A half
+            // tile with more than NV distinct voxels on a level reads them from global memory, as levels 1 and 0 always do.  The
+            // blend (weights, corner order, FMA order) is the same on both paths, so the results are bit-identical.
             auto gather = [&](int seg) {
                 const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
+                const VoxTable* vt = reinterpret_cast<const VoxTable*>(smem + OFF_VTAB) + (it & 1);
                 const int grp = (tid & 127) >> 3, t = tid & 7;
                 const int lvl = seg < 2 ? 3 : seg < 4 ? 2 : seg < 5 ? 1 : 0;
                 const int cbase0 = seg < 2 ? seg * 64 : seg < 4 ? (seg - 2) * 64 : 0;
                 const int nunits = seg == NUM_SEGS - 1 ? 1 : 2;
                 const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-                const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
-                const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
                 const int kb = 64 * (seg % SEG_BUFS);
-                for (int row = 64 * cw + grp; row < 64 * cw + 64; row += 16) {
-                    const float4 e = rows[row];
-                    const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
-                    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-                    if (occ) {
-                        float gx, gy, gz;
-                        world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
-                        Corners cn;
-                        corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
-                        // The 8 corners are addressed as (clamped low corner) + constant strides.  A cell that straddles the
-                        // volume boundary (index -1 or size-1 on an axis; zeros padding upstream) is shifted inside by one and
-                        // its in-range voxel's weight moves to the slot that now addresses it; the out-of-range slot gets 0.
-                        auto axis = [](int i0, int size, float (&w)[2]) {
-                            if (i0 < 0) { w[0] = w[1]; w[1] = 0.f; return 0; }                        // i0 == -1: only voxel 0
-                            if (i0 >= size) { w[0] = w[1] = 0.f; return size - 2; }                   // both neighbours outside
-                            if (i0 == size - 1) { w[1] = w[0]; w[0] = 0.f; return size - 2; }         // only voxel size-1
-                            return i0;
-                        };
-                        const int xc = axis(cn.x0, W, cn.wx), yc = axis(cn.y0, H, cn.wy), zc = axis(cn.z0, D, cn.wz);
-                        const uint32_t cb = (uint32_t)((zc * H + yc) * W + xc) * dX;
-                        float cw[8];
+                // staging: voxel v at 1 KB piece v / VPP (the warpgroup's 64 rows of one K chunk), pieces 0-15 in the hi plane and
+                // 16-31 in the lo plane, from chunk 16 (level 3) or 0 (level 2) on
+                constexpr uint32_t VB = kCoarseC * sizeof(VT), VPP = 1024 / VB, PPV = VB / 16;
+                const int tab = 2 * cw + (seg >> 1);
+                const bool staged = seg < 4 && C == kCoarseC && vt->n[tab] <= (uint32_t)NV;
+                const uint32_t st_base = s_hi + (seg < 2 ? 16 : 0) * CHUNK_STRIDE + cw * 1024;
+                auto stage_addr = [&](uint32_t v) {
+                    const uint32_t p = v / VPP;
+                    return st_base + (p >> 4) * PLANE_BYTES + (p & 15) * CHUNK_STRIDE + (v % VPP) * VB;
+                };
+                if (staged && (seg & 1) == 0) {
+                    const unsigned char* src = volbase + P.lvl_off[lvl] + (size_t)P.frame * P.lvl_bstride[lvl] * sizeof(VT);
+                    const uint32_t nq = vt->n[tab] * PPV;
+#pragma unroll 4
+                    for (uint32_t i = tid & 127; i < nq; i += 128) {
+                        const uint32_t v = i / PPV, q = i % PPV;
+                        tc::cp_async_16(stage_addr(v) + 16 * q, src + (size_t)vt->ids[tab][v] * VB + 16 * q);
+                    }
+                    tc::cp_async_wait_all();
+                    tcr::named_bar_sync(1 + cw, 128);
+                }
+                // the warpgroup's 64 rows; blend(row, cb, cw, acc) accumulates the row's 8 corners of both 32-channel units.  The
+                // two paths get a loop each, so neither keeps the other's addressing state live beside the accumulators.
+                auto rows_loop = [&](auto&& blend) {
+                    for (int row = 64 * cw + grp; row < 64 * cw + 64; row += 16) {
+                        const float4 e = rows[row];
+                        const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
+                        float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+                        if (occ) {
+                            float gx, gy, gz;
+                            world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+                            Corners cn;
+                            const uint32_t cb = clamped_cell(gx, gy, gz, W, H, D, cn);
+                            float cw[8];
 #pragma unroll
-                        for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
+                            for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
+                            blend(row, cb, cw, acc);
+                        }
+#pragma unroll
+                        for (int uu = 0; uu < 2; ++uu) {
+                            if (uu >= nunits) continue;
+                            const float (&a)[4] = acc[uu];
+                            const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
+                            uint2 hw, lw;
+                            if (NP == 3) {
+                                // (hi, lo) split with a truncated hi: the residual is exact
+                                hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
+                                float q0, q1, q2, q3;
+                                tc::trunc_residual2(a[0], a[1], q0, q1);
+                                tc::trunc_residual2(a[2], a[3], q2, q3);
+                                lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
+                                tcr::sts_v2(s_lo + off, lw);
+                            } else {
+                                hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
+                            }
+                            tcr::sts_v2(s_hi + off, hw);
+                        }
+                    }
+                };
+                if (staged) {
+                    // shared-memory latency is short: one corner (both units) at a time keeps the registers low.  Each unit
+                    // still accumulates its corners in order 0..7.
+                    const uint32_t st_off = ((seg & 1) * 64 + 4 * t) * sizeof(VT);   // this lane's channels inside a voxel
+                    const int li = seg >> 1;
+                    rows_loop([&](int row, uint32_t, const float (&cw)[8], float (&acc)[2][4]) {
+                        const uint2 sl = *reinterpret_cast<const uint2*>(&vt->slot[row][li][0]);
+#pragma unroll
+                        for (int c = 0; c < 8; ++c) {
+                            const uint32_t a = stage_addr((((c < 4) ? sl.x : sl.y) >> (8 * (c & 3))) & 0xFFu) + st_off;
+                            const typename Quad<VT>::raw v0 = Quad<VT>::load_shared(a), v1 = Quad<VT>::load_shared(a + 32 * sizeof(VT));
+                            if (cw[c] != 0.f) {
+                                Quad<VT>::fma(acc[0], v0, cw[c]);
+                                Quad<VT>::fma(acc[1], v1, cw[c]);
+                            }
+                        }
+                    });
+                } else {
+                    const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
+                    const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
+                    rows_loop([&](int, uint32_t cell, const float (&cw)[8], float (&acc)[2][4]) {
+                        const uint32_t cb = cell * dX;
 #pragma unroll
                         for (int uu = 0; uu < 2; ++uu) {
                             if (uu >= nunits) continue;
@@ -530,26 +721,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                             for (int c = 0; c < 8; ++c)
                                 if (cw[c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw[c]);
                         }
-                    }
-#pragma unroll
-                    for (int uu = 0; uu < 2; ++uu) {
-                        if (uu >= nunits) continue;
-                        const float (&a)[4] = acc[uu];
-                        const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
-                        uint2 hw, lw;
-                        if (NP == 3) {
-                            // (hi, lo) split with a truncated hi: the residual is exact
-                            hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
-                            float q0, q1, q2, q3;
-                            tc::trunc_residual2(a[0], a[1], q0, q1);
-                            tc::trunc_residual2(a[2], a[3], q2, q3);
-                            lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
-                            tcr::sts_v2(s_lo + off, lw);
-                        } else {
-                            hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
-                        }
-                        tcr::sts_v2(s_hi + off, hw);
-                    }
+                    });
                 }
             };
 
@@ -558,6 +730,8 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 tc::mbar_wait(&bars[B_ROWSFULL], it & 1);
                 r_stall += (uint32_t)clock() - t0;
             }
+            __syncwarp();                                               // (every lane is past the previous tile)
+            tc::mbar_arrive_if(&bars[B_ROWSFREE], arr);                 // done with the previous tile's row buffer
             // ================= layer 0: gather a segment, multiply it (its K-steps pipelined), retire them, gather the next
             init_bias(head + H_B0);
             for (int seg = 0; seg < nseg; ++seg) {
@@ -576,7 +750,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 tc::acc_fence(acc0); tc::acc_fence(acc1);
                 release_last();
             }
-            tr.ev(20);
+            tev(20);
             convert(false);                                             // h0
             init_bias(head + H_B0 + kHidden);
             publish();
@@ -592,7 +766,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 tc::wgmma_wait<0>();
                 tc::acc_fence(acc0); tc::acc_fence(acc1);
                 release_last();
-                tr.ev(20 + layer);
+                tev(20 + layer);
                 if (layer == 1) {
                     convert(false);                                     // h1
                     init_bias(head + H_B0 + 2 * kHidden);
@@ -632,7 +806,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             tc::wgmma_wait<0>();
             tc::acc_fence(c3a); tc::acc_fence(c3b);
             release_last();
-            tr.ev(23);
+            tev(23);
             // ---- the colour head: rgb = rgb_fc . relu(layer-3 accumulator) + bias, and sigma = alpha_fc . h2 + bias, fp32
             float cr[2] = {0.f, 0.f}, cg[2] = {0.f, 0.f}, cbl[2] = {0.f, 0.f};
             auto color = [&](const float (&a)[32], int nh) {
@@ -670,16 +844,21 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                                                 sg[hr] + head[H_ALPHA + kHidden]);
                 }
             }
-            tr.ev(24);
-            tr.val(50, w_stall);
-            tr.val(51, r_stall);
-            tr.val(52, pe_stall);
-            tr.val(53, g_cycles);
+            tev(24);
+            tval(50, w_stall);
+            tval(51, r_stall);
+            tval(52, pe_stall);
+            tval(53, g_cycles);
             w_stall = r_stall = pe_stall = g_cycles = 0;
         }
     }
     __syncthreads();
-    if (tid == 0 && P.stats) atomicMax(P.frame_clock + 1, global_ns());
+    if (tid == 0 && P.stats) {
+        atomicMax(P.frame_clock + 1, global_ns());
+        const uint32_t* paths = reinterpret_cast<const uint32_t*>(smem + OFF_HCNT) + NTAB;
+        atomicAdd(P.stats + 5, (unsigned long long)paths[0]);             // coarse-level half tiles gathered from the staging
+        atomicAdd(P.stats + 6, (unsigned long long)paths[1]);             // ... and directly (more than NV distinct voxels)
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ 3. raw2outputs

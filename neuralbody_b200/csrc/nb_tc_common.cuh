@@ -47,6 +47,11 @@ template <> struct Quad<float> {
     static __device__ __forceinline__ raw zero() { return make_uint4(0u, 0u, 0u, 0u); }
     static __device__ __forceinline__ raw load(const float* p) { return ldg_nc_v4(p); }
     static __device__ __forceinline__ raw load_bytes(const unsigned char* p) { return ldg_nc_v4(p); }
+    static __device__ __forceinline__ raw load_shared(uint32_t addr) {
+        uint4 r;
+        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr) : "memory");
+        return r;
+    }
     static __device__ __forceinline__ void fma(float (&a)[4], const raw& v, float w) {
         a[0] = fmaf(__uint_as_float(v.x), w, a[0]); a[1] = fmaf(__uint_as_float(v.y), w, a[1]);
         a[2] = fmaf(__uint_as_float(v.z), w, a[2]); a[3] = fmaf(__uint_as_float(v.w), w, a[3]);
@@ -61,6 +66,11 @@ template <> struct Quad<__half> {
         return r;
     }
     static __device__ __forceinline__ raw load_bytes(const unsigned char* p) { return load(reinterpret_cast<const __half*>(p)); }
+    static __device__ __forceinline__ raw load_shared(uint32_t addr) {
+        uint2 r;
+        asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(addr) : "memory");
+        return r;
+    }
     static __device__ __forceinline__ void fma(float (&a)[4], const raw& v, float w) {
         const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
         const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&v.y));

@@ -100,6 +100,13 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
+// ---------------------------------------------------------------- 16-byte async copy global -> shared (L2 only, no registers)
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+// every cp.async this thread issued has landed (visible to the thread; a barrier then publishes them)
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 // ---------------------------------------------------------------- warpgroup MMA (wgmma, sm_90a)
 // Shared-memory matrix descriptor, K-major, no swizzle ("interleave"):
 //   bits [0,14)  start address >> 4          bits [16,30) leading-dimension byte offset >> 4

@@ -33,11 +33,16 @@ def main():
     sp = ren.prepare_sp_input(batch)
     vol = net.encode_sparse_voxels(sp)
     trace = torch.zeros(4 * 4096, dtype=torch.int64, device="cuda")
+    ren.stats = torch.zeros(8, dtype=torch.int64, device="cuda")
     for _ in range(2):
         trace.zero_()
+        ren.stats.zero_()
         with torch.no_grad():
             ren.render_rays(batch["ray_o"], batch["ray_d"], batch["near"], batch["far"], vol, sp, trace=trace)
     torch.cuda.synchronize()
+    staged, direct = int(ren.stats[5]), int(ren.stats[6])
+    print("coarse-level half tiles (levels 3 and 2, all CTAs): %d staged, %d direct (%.2f%% direct)"
+          % (staged, direct, 100.0 * direct / max(1, staged + direct)))
     t = trace.cpu().view(4, 4096)
     roles = [("PROD", PROD, None, 1), ("MMA0", MMA, None, 1), ("MMA1", MMA, None, 1), ("LOAD", LOAD, None, 1)]
     per_tile = {}                                            # (role, tile) -> {code: clock or value}
