@@ -151,7 +151,8 @@ typedef struct nb_render_args {
                                   [2] += ns spent in the decoder kernel (%globaltimer, first CTA start to last CTA end),
                                   [3] += decoder launches (tensor-core precisions), [5] / [6] += 64-row half tiles whose
                                   coarse-level (3 and 2) layer-0 features were gathered from the shared-memory staging /
-                                  directly from global memory (more distinct voxels than the staging holds) */
+                                  directly from global memory (more distinct voxels than the staging holds), [7] += 64-row
+                                  half tiles whose fine-level (1 or 0) features were gathered directly, one per level */
     float* save;           /* device (B,n,S,1312) activation record for nb_render_bwd, or NULL (NB_PRECISION_FP32 only);
                               size from nb_render_save_bytes() */
     unsigned long long* trace; /* device, 4 x 4096 u64, or NULL: per-role (code<<48 | SM clock) timeline of CTA 0

@@ -145,9 +145,9 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
 // One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  The CTA is warp-specialised:
 //   producer warpgroup (warps 0-3)   warp 0: one elected lane streams the weights with bulk copies into a 4-slot ring (one
-//                                     K-step of both N halves and both planes per slot).  Warps 1-3: each tile's list rows and
-//                                     coarse-level voxel table (double-buffered, built one tile ahead) and layer 3's
-//                                     per-point tile.
+//                                     K-step of both N halves and both planes per slot).  Warps 1-3: each tile's list rows,
+//                                     their grid coordinates and voxel table (double-buffered, built one tile ahead) and
+//                                     layer 3's per-point tile.
 //   consumer warpgroups 1 and 2      rows [0, 64) and [64, 128) of a tile: gather layer 0's feature segments of their own rows,
 //                                     issue the wgmma and run the epilogues.  Nothing divergent sits between a wgmma and the
 //                                     wait that retires it (the gather runs only while none of the warpgroup's wgmma are in
@@ -189,32 +189,45 @@ constexpr int OFF_HEAD = OFF_RING + NUM_SLOTS * SLOT_BYTES;
 constexpr int OFF_XF = OFF_HEAD + HEAD_FLOATS * 4;
 constexpr int OFF_SCHED = OFF_XF + 128;
 constexpr int OFF_ROWS = OFF_SCHED + 64;                           // two tiles' list entries (float4 per row)
-// Layer-0 voxel tables of the two coarse levels (3 and 2, 128 channels each).  A 64-row half tile of neighbouring samples
-// touches a few dozen distinct voxels of a coarse level but requests 512 corner vectors; the row warps list the distinct ones
+// Layer-0 voxel tables of the four levels, li = 3 - level (li 0, 1: the coarse levels 3 and 2, 128 channels each; li 2:
+// level 1, 64 channels; li 3: level 0, 32 channels).  A 64-row half tile of neighbouring samples touches a few dozen (coarse)
+// to about a hundred (fine) distinct voxels of a level but requests 512 corner vectors; the row warps list the distinct ones
 // one tile ahead, and the consumer warpgroup copies each of them once into idle segment buffers of its own ACT-plane rows
-// and blends from there.  Table t = 2 * half + li (li 0: level 3, 1: level 2).
-constexpr int NV = 64;                                             // staged voxels per half tile and level (ACT room: fp32
-                                                                   // 64 x 512 B = 2 segment buffers of both planes)
-constexpr int NTAB = 4;
-constexpr int HBITS = 7, HSIZE = 1 << HBITS;                       // open-addressed hash per table (build scratch)
+// and blends from there.  The row warps also publish each row's grid coordinates, so the consumers do not redo world_to_grid
+// (six divisions) in every segment.
+constexpr int NV_COARSE = 64, NV_FINE = 128;                       // staged voxels per half tile and level (ACT room, fp32:
+                                                                   // 64 x 512 B, 128 x 256 B = 2 segment buffers of both planes)
+__host__ __device__ constexpr int level_nv(int li) { return li < 2 ? NV_COARSE : NV_FINE; }
+__host__ __device__ constexpr int level_channels(int li) { return li < 2 ? 128 : li == 2 ? 64 : 32; }
+// the distinct voxels of level li and half tile `half` start at ids[ids_at(li, half)]
+__host__ __device__ constexpr int ids_at(int li, int half) {
+    return li < 2 ? (2 * li + half) * NV_COARSE : 4 * NV_COARSE + (2 * (li - 2) + half) * NV_FINE;
+}
+constexpr int HBITS = 8, HSIZE = 1 << HBITS;                       // open-addressed hash per half tile, reused level by level
 constexpr uint32_t HEMPTY = 0xFFFFFFFFu;
-constexpr int kCoarseC = 128;                                      // channels of levels 3 and 2 (two K segments each)
 struct VoxTable {
-    unsigned char slot[TP][2][8];                                  // per row and level: the staged slot of each corner
-    uint32_t ids[NTAB][NV];                                        // the distinct voxels (linear index (z H + y) W + x)
-    uint32_t n[NTAB];                                              // their number; > NV: the level is gathered directly
+    float4 grid[TP];                                               // per row: world_to_grid of the sample (x, y, z, -)
+    unsigned char slot[TP][4][8];                                  // per row and level: the staged slot of each corner
+    uint32_t ids[ids_at(4, 0)];                                    // the distinct voxels (linear index (z H + y) W + x)
+    uint32_t n[8];                                                 // their number, [2 li + half]; > level_nv(li): direct
 };
 constexpr int OFF_VTAB = OFF_ROWS + 2 * TP * 16;                   // two tiles' tables (double-buffered like the rows)
 constexpr int OFF_HKEY = OFF_VTAB + 2 * (int)sizeof(VoxTable);
-constexpr int OFF_HVAL = OFF_HKEY + NTAB * HSIZE * 4;
-constexpr int OFF_HCNT = OFF_HVAL + NTAB * HSIZE;
-constexpr int OFF_BAR = OFF_HCNT + (NTAB + 2) * 4;                 // + the CTA's staged / direct half-tile counts
+constexpr int OFF_HVAL = OFF_HKEY + 2 * HSIZE * 4;
+constexpr int OFF_HCNT = OFF_HVAL + 2 * HSIZE;
+// hcnt: [0, 1] the voxels of the level being built per half tile, then the CTA's half-tile counts: [2] / [3] coarse levels
+// staged / direct, [4] fine levels direct
+constexpr int NCNT = 5;
+constexpr int OFF_BAR = OFF_HCNT + 8 * 4;
 enum { B_FULL = 0, B_EMPTY = B_FULL + NUM_SLOTS, B_ROWSFULL = B_EMPTY + NUM_SLOTS, B_L2DONE, B_PEFULL, B_ROWSFREE, NUM_BARS };
 constexpr int SMEM_BYTES = OFF_BAR + NUM_BARS * 8;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 static_assert(OFF_RING % 128 == 0 && OFF_HEAD % 16 == 0 && OFF_ROWS % 16 == 0 && OFF_VTAB % 16 == 0 && OFF_HKEY % 16 == 0 &&
               OFF_BAR % 8 == 0, "alignment");
-static_assert(NV * kCoarseC * 4 <= 2 * 2 * 8 * 1024 && NV <= 255 && HSIZE > NV, "voxel staging");
+// a level's staging fits two segment buffers of the warpgroup's rows in both planes; a slot fits a byte with 0xFF = none, and
+// the hash never fills (at most NV_FINE + 1 + NROWT keys: an insert stops once the count is past the capacity)
+static_assert(NV_COARSE * level_channels(0) * 4 <= 2 * 2 * 8 * 1024 && NV_FINE * level_channels(2) * 4 <= 2 * 2 * 8 * 1024 &&
+              NV_FINE < 255 && HSIZE > NV_FINE + 1 + NROWT && NCNT <= 8, "voxel staging");
 static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NT * LAUNCH_REGS, "register pool of the CTA");
 
 // weight pushes of a tile whose layer 0 runs l0_ksteps K-steps: one per K-step of layers 0..2, layer 3 in groups of L3_PUSH
@@ -276,8 +289,8 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         }
         head[i] = v;
     }
-    for (int i = tid; i < NTAB * HSIZE; i += NT) reinterpret_cast<uint32_t*>(smem + OFF_HKEY)[i] = HEMPTY;
-    if (tid < NTAB + 2) reinterpret_cast<uint32_t*>(smem + OFF_HCNT)[tid] = 0u;
+    for (int i = tid; i < 2 * HSIZE; i += NT) reinterpret_cast<uint32_t*>(smem + OFF_HKEY)[i] = HEMPTY;
+    if (tid < NCNT) reinterpret_cast<uint32_t*>(smem + OFF_HCNT)[tid] = 0u;
     struct Sched { unsigned int cnt[4]; int start[4]; int n_tiles; };
     Sched* sched = reinterpret_cast<Sched*>(smem + OFF_SCHED);
     if (tid == 0) {
@@ -376,84 +389,88 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             tcr::Tracer tr;
             tr.init(pt == 0 ? P.trace : nullptr, 0);
             auto pwait = [&](uint64_t* bar, uint32_t parity) { tc::mbar_wait_backoff(bar, parity, 64); };
-            // insert voxel `id` into table `tab`'s hash: its hash position, or 0xFF once the table holds more than NV voxels
-            // (the consumers then gather that level directly and never read the slots)
-            auto insert = [&](int tab, uint32_t id, VoxTable* vt) -> uint32_t {
-                if (*reinterpret_cast<volatile uint32_t*>(hcnt + tab) > (uint32_t)NV) return 0xFFu;
-                uint32_t* keys = hkey + tab * HSIZE;
+            // insert voxel `id` into half tile `half`'s hash: its hash position, or 0xFF once the level holds more than nv
+            // voxels (the consumers then gather that level directly and never read the slots)
+            auto insert = [&](int half, uint32_t id, uint32_t* ids, uint32_t nv) -> uint32_t {
+                if (*reinterpret_cast<volatile uint32_t*>(hcnt + half) > nv) return 0xFFu;
+                uint32_t* keys = hkey + half * HSIZE;
                 uint32_t h = (id * 2654435761u) >> (32 - HBITS);
 #pragma unroll 1
                 for (int p = 0; p < HSIZE; ++p, h = (h + 1) & (HSIZE - 1)) {
                     uint32_t k = *reinterpret_cast<volatile uint32_t*>(keys + h);
                     if (k == HEMPTY) k = atomicCAS(keys + h, HEMPTY, id);
                     if (k == HEMPTY) {                                  // claimed: the voxel's slot is the next free one
-                        const uint32_t s = atomicAdd(hcnt + tab, 1u);
-                        if (s < (uint32_t)NV) vt->ids[tab][s] = id;
-                        hval[tab * HSIZE + h] = (unsigned char)min(s, 255u);
+                        const uint32_t s = atomicAdd(hcnt + half, 1u);
+                        if (s < nv) ids[s] = id;
+                        hval[half * HSIZE + h] = (unsigned char)min(s, 255u);
                         return h;
                     }
                     if (k == id) return h;
                 }
-                return 0xFFu;                                           // (a full hash already holds HSIZE > NV voxels)
+                return 0xFFu;                                           // (the hash never fills, see the static_assert)
             };
-            // The voxel table of a tile whose rows are in `rows`: per half tile and coarse level its distinct corner voxels
-            // and, per row, the slot of each of the 8 corners.  Insert (slot bytes = hash positions), then resolve them.
+            // The voxel table of a tile whose rows and grid coordinates are in `rows` / `vt`, level by level in one hash per
+            // half tile: the level's distinct corner voxels per half tile and, per row, the slot of each of the 8 corners.
+            // Insert (slot bytes = hash positions), then resolve them and clear the hash for the next level.
             auto build_table = [&](VoxTable* vt, const float4* rows, int nrows, int nlev) {
+                auto occupied = [&](int row, int lvl) { return row < nrows && ((__float_as_uint(rows[row].w) >> (28 + lvl)) & 1u); };
 #pragma unroll 1
-                for (int row = pt; row < TP; row += NROWT) {
-                    const float4 e = rows[row];
-                    float gx, gy, gz;
-                    world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+                for (int li = 0; li < nlev; ++li) {
+                    const int lvl = 3 - li, D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+                    const uint32_t nv = (uint32_t)level_nv(li);
 #pragma unroll 1
-                    for (int li = 0; li < nlev; ++li) {
-                        const int lvl = 3 - li, tab = 2 * (row >> 6) + li;
-                        uint32_t w[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
-                        if (row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u)) {
-                            const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+                    for (int j = pt; j < TP * 8; j += NROWT) {              // corner j % 8 of row j / 8
+                        const int row = j >> 3, c = j & 7;
+                        uint32_t h = 0xFFu;
+                        if (occupied(row, lvl)) {
+                            const float4 gq = vt->grid[row];
                             Corners cn;
-                            const uint32_t base = clamped_cell(gx, gy, gz, W, H, D, cn);
-#pragma unroll
-                            for (int c = 0; c < 8; ++c) {
-                                const uint32_t id = base + ((c & 1) ? 1u : 0u) + ((c & 2) ? (uint32_t)W : 0u) + ((c & 4) ? (uint32_t)(W * H) : 0u);
-                                const uint32_t h = insert(tab, id, vt);
-                                w[c >> 2] = (w[c >> 2] & ~(0xFFu << (8 * (c & 3)))) | (h << (8 * (c & 3)));
-                            }
+                            const uint32_t id = clamped_cell(gq.x, gq.y, gq.z, W, H, D, cn) + ((c & 1) ? 1u : 0u) +
+                                                ((c & 2) ? (uint32_t)W : 0u) + ((c & 4) ? (uint32_t)(W * H) : 0u);
+                            h = insert(row >> 6, id, vt->ids + ids_at(li, row >> 6), nv);
                         }
-                        *reinterpret_cast<uint2*>(&vt->slot[row][li][0]) = make_uint2(w[0], w[1]);
+                        vt->slot[row][li][c] = (unsigned char)h;
                     }
-                }
-                tcr::named_bar_sync(3, NROWT);
-                uint32_t* words = reinterpret_cast<uint32_t*>(&vt->slot[0][0][0]);
+                    tcr::named_bar_sync(3, NROWT);
 #pragma unroll 1
-                for (int i = pt; i < TP * 2 * 2; i += NROWT) {          // word i: row i / 4, level i / 2 % 2
-                    const int li = (i >> 1) & 1;
-                    if (li >= nlev) continue;
-                    const unsigned char* hv = hval + (2 * ((i >> 2) >> 6) + li) * HSIZE;
-                    uint32_t wd = words[i], out = 0u;
+                    for (int i = pt; i < TP * 2; i += NROWT) {              // corners 4 (i & 1) .. 4 (i & 1) + 3 of row i / 2
+                        const int row = i >> 1;
+                        uint32_t* wp = reinterpret_cast<uint32_t*>(&vt->slot[row][li][4 * (i & 1)]);
+                        const unsigned char* hv = hval + (row >> 6) * HSIZE;
+                        uint32_t out = 0xFFFFFFFFu;
+                        if (occupied(row, lvl)) {
+                            const uint32_t wd = *wp;
+                            out = 0u;
 #pragma unroll
-                    for (int b = 0; b < 4; ++b) {
-                        const uint32_t h = (wd >> (8 * b)) & 0xFFu;
-                        out |= (h == 0xFFu ? 0xFFu : (uint32_t)hv[h]) << (8 * b);
+                            for (int b = 0; b < 4; ++b) out |= (uint32_t)hv[(wd >> (8 * b)) & 0xFFu] << (8 * b);
+                        }
+                        *wp = out;
                     }
-                    words[i] = out;
-                }
-                for (int i = pt; i < NTAB * HSIZE; i += NROWT) hkey[i] = HEMPTY;   // (the keys are not read past the insert)
-                if (pt < NTAB) {
-                    const uint32_t n = hcnt[pt];
-                    vt->n[pt] = n;
-                    hcnt[pt] = 0u;
-                    if ((pt & 1) < nlev && nrows > 64 * (pt >> 1)) atomicAdd(hcnt + NTAB + (n <= (uint32_t)NV ? 0 : 1), 1u);
+                    for (int i = pt; i < 2 * HSIZE; i += NROWT) hkey[i] = HEMPTY;   // (the keys are not read past the insert)
+                    if (pt < 2) {
+                        const uint32_t n = hcnt[pt];
+                        vt->n[2 * li + pt] = n;
+                        hcnt[pt] = 0u;
+                        if (nrows > 64 * pt && (li < 2 || n > nv)) atomicAdd(hcnt + (li < 2 ? (n <= nv ? 2 : 3) : 4), 1u);
+                    }
+                    tcr::named_bar_sync(3, NROWT);
                 }
             };
-            // a tile's rows and its voxel table into buffer `buf`, published through rows_full
+            // a tile's rows, their grid coordinates and its voxel table into buffer `buf`, published through rows_full
             auto load_rows = [&](int buf, int tile) {
                 if (tile < n_tiles) {
                     const TileRef r = tile_ref(tile);
                     float4* dst = rows_buf + buf * TP;
-                    for (int i = pt; i < TP; i += NROWT)
-                        dst[i] = i < r.nrows ? __ldg(r.ent + i) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
+                    VoxTable* vt = vtabs + buf;
+                    for (int i = pt; i < TP; i += NROWT) {
+                        const float4 e = i < r.nrows ? __ldg(r.ent + i) : make_float4(0.f, 0.f, 0.f, __uint_as_float(0xFFFFFFFFu));
+                        dst[i] = e;
+                        float gx, gy, gz;
+                        world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
+                        vt->grid[i] = make_float4(gx, gy, gz, 0.f);
+                    }
                     tcr::named_bar_sync(3, NROWT);
-                    build_table(vtabs + buf, dst, r.nrows, class_segments(r.cls) >= 4 ? 2 : 1);
+                    build_table(vt, dst, r.nrows, 4 - r.cls);               // a class-c tile gathers levels 3 .. c
                 }
                 tcr::named_bar_sync(3, NROWT);
                 tc::mbar_arrive(&bars[B_ROWSFULL]);
@@ -545,7 +562,8 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             }
         };
         uint32_t g = 0;                                                 // pushes consumed by this CTA
-        uint32_t w_stall = 0, r_stall = 0, pe_stall = 0, g_cycles = 0;  // cycles waited on weights / rows / the per-point tile; gathering
+        // cycles waited on weights / rows / the per-point tile; gathering the coarse (segments 0-3) and fine (4, 5) levels
+        uint32_t w_stall = 0, r_stall = 0, pe_stall = 0, g_coarse = 0, g_fine = 0;
         // wait for push g, issue `mma(slot address)`, commit
         auto take = [&](auto&& mma) {
             const uint32_t s = g % NUM_SLOTS;
@@ -614,11 +632,12 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             tev(1);
             // ---- layer-0 gather of this warpgroup's rows: segment seg (64 channels of one level, coarse level first) -> segment
             // buffer seg % SEG_BUFS.  It runs while none of the warpgroup's wgmma are in flight; the other warpgroup's MMAs overlap it.
-            // Levels 3 and 2 (segments 0-3) are staged: at a level's first segment the warpgroup copies its half tile's distinct
-            // voxels (all 128 channels) with cp.async into the level's two idle segment buffers of its own rows (level 3: buffers
-            // 2, 3; level 2: buffers 0, 1; the warpgroup's MMAs on them are retired), and both segments blend from there.  A half
-            // tile with more than NV distinct voxels on a level reads them from global memory, as levels 1 and 0 always do.  The
-            // blend (weights, corner order, FMA order) is the same on both paths, so the results are bit-identical.
+            // Every level is staged: at a level's first segment the warpgroup copies its half tile's distinct voxels (all of the
+            // level's channels) with cp.async into idle segment buffers of its own rows (level 2: buffers 0, 1; levels 3, 1 and 0:
+            // buffers 2, 3; the warpgroup's MMAs on them are retired, and no segment of the level writes there), and the level's
+            // segments blend from there.  A half tile with more distinct voxels on a level than level_nv holds reads them from
+            // global memory and redoes world_to_grid (the direct path).  The blend (weights, corner order, FMA order) is the same
+            // on both paths, so the results are bit-identical.
             auto gather = [&](int seg) {
                 const unsigned char* volbase = reinterpret_cast<const unsigned char*>(P.volume);
                 const VoxTable* vt = reinterpret_cast<const VoxTable*>(smem + OFF_VTAB) + (it & 1);
@@ -628,30 +647,107 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 const int nunits = seg == NUM_SEGS - 1 ? 1 : 2;
                 const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
                 const int kb = 64 * (seg % SEG_BUFS);
-                // staging: voxel v at 1 KB piece v / VPP (the warpgroup's 64 rows of one K chunk), pieces 0-15 in the hi plane and
-                // 16-31 in the lo plane, from chunk 16 (level 3) or 0 (level 2) on
-                constexpr uint32_t VB = kCoarseC * sizeof(VT), VPP = 1024 / VB, PPV = VB / 16;
-                const int tab = 2 * cw + (seg >> 1);
-                const bool staged = seg < 4 && C == kCoarseC && vt->n[tab] <= (uint32_t)NV;
-                const uint32_t st_base = s_hi + (seg < 2 ? 16 : 0) * CHUNK_STRIDE + cw * 1024;
+                // staging: voxel v (VB = 2^lg_vb bytes, all channels of the level) at 1 KB piece v / VPP (the warpgroup's 64 rows of
+                // one K chunk), pieces 0-15 in the hi plane and 16-31 in the lo plane, from chunk 0 (level 2) or 16 (the others) on
+                const int li = seg < 4 ? seg >> 1 : seg - 2;
+                const int lg_vb = (li < 2 ? 7 : li == 2 ? 6 : 5) + (sizeof(VT) == 4 ? 2 : 1), lg_vpp = 10 - lg_vb;
+                const bool staged = C == level_channels(li) && vt->n[2 * li + cw] <= (uint32_t)level_nv(li);
+                const uint32_t st_base = s_hi + (li == 1 ? 0 : 16) * CHUNK_STRIDE + cw * 1024;
                 auto stage_addr = [&](uint32_t v) {
-                    const uint32_t p = v / VPP;
-                    return st_base + (p >> 4) * PLANE_BYTES + (p & 15) * CHUNK_STRIDE + (v % VPP) * VB;
+                    const uint32_t p = v >> lg_vpp;
+                    return st_base + (p >> 4) * PLANE_BYTES + (p & 15) * CHUNK_STRIDE + ((v & ((1u << lg_vpp) - 1)) << lg_vb);
                 };
-                if (staged && (seg & 1) == 0) {
+                if (staged && (seg >= 4 || (seg & 1) == 0)) {                 // the level's first segment
                     const unsigned char* src = volbase + P.lvl_off[lvl] + (size_t)P.frame * P.lvl_bstride[lvl] * sizeof(VT);
-                    const uint32_t nq = vt->n[tab] * PPV;
+                    const uint32_t* ids = vt->ids + ids_at(li, cw);
+                    const int lg_ppv = lg_vb - 4;
+                    const uint32_t nq = vt->n[2 * li + cw] << lg_ppv;
 #pragma unroll 4
                     for (uint32_t i = tid & 127; i < nq; i += 128) {
-                        const uint32_t v = i / PPV, q = i % PPV;
-                        tc::cp_async_16(stage_addr(v) + 16 * q, src + (size_t)vt->ids[tab][v] * VB + 16 * q);
+                        const uint32_t v = i >> lg_ppv, q = i & ((1u << lg_ppv) - 1);
+                        tc::cp_async_16(stage_addr(v) + 16 * q, src + ((size_t)ids[v] << lg_vb) + 16 * q);
                     }
                     tc::cp_async_wait_all();
                     tcr::named_bar_sync(1 + cw, 128);
                 }
-                // the warpgroup's 64 rows; blend(row, cb, cw, acc) accumulates the row's 8 corners of both 32-channel units.  The
-                // two paths get a loop each, so neither keeps the other's addressing state live beside the accumulators.
-                auto rows_loop = [&](auto&& blend) {
+                // a row's trilinear set-up at grid coordinates (gx, gy, gz): the clamped cell's low corner and the 8 corner weights
+                auto setup = [&](float gx, float gy, float gz, float (&cw)[8]) {
+                    Corners cn;
+                    const uint32_t cb = clamped_cell(gx, gy, gz, W, H, D, cn);
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
+                    return cb;
+                };
+                // a row's blended units -> its fp16 operand(s) in the segment buffer
+                auto store_row = [&](int row, const float (&acc)[2][4]) {
+#pragma unroll
+                    for (int uu = 0; uu < 2; ++uu) {
+                        if (uu >= nunits) continue;
+                        const float (&a)[4] = acc[uu];
+                        const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
+                        uint2 hw, lw;
+                        if (NP == 3) {
+                            // (hi, lo) split with a truncated hi: the residual is exact
+                            hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
+                            float q0, q1, q2, q3;
+                            tc::trunc_residual2(a[0], a[1], q0, q1);
+                            tc::trunc_residual2(a[2], a[3], q2, q3);
+                            lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
+                            tcr::sts_v2(s_lo + off, lw);
+                        } else {
+                            hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
+                        }
+                        tcr::sts_v2(s_hi + off, hw);
+                    }
+                };
+                // The warpgroup's 64 rows, 4 per lane group.  Each unit accumulates its corners in order 0..7 and skips zero
+                // weights on both paths.  The two paths get a loop each, so neither keeps the other's addressing state live
+                // beside the accumulators.
+                if (staged) {
+                    // Two rows in flight: their set-up (from the grid coordinates the row warps published) and their corner
+                    // loads are independent, so each hides the other's shared-memory latency.  An unoccupied row blends voxel 0
+                    // with weight 0, which leaves its accumulators at 0.
+                    const uint32_t st_off = (cbase0 + 4 * t) * sizeof(VT);       // this lane's channels inside a voxel
+#pragma unroll 1
+                    for (int row = 64 * cw + grp; row < 64 * cw + 64; row += 32) {
+                        float acc[2][2][4] = {};
+                        float cw8[2][8];
+                        uint2 sl[2];
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const int rw = row + 16 * r;
+                            const bool occ = rw < nrows && ((__float_as_uint(rows[rw].w) >> (28 + lvl)) & 1u);
+                            const float4 g = vt->grid[rw];
+                            setup(g.x, g.y, g.z, cw8[r]);
+                            sl[r] = *reinterpret_cast<const uint2*>(&vt->slot[rw][li][0]);
+                            if (!occ) {
+                                sl[r] = make_uint2(0u, 0u);
+#pragma unroll
+                                for (int c = 0; c < 8; ++c) cw8[r][c] = 0.f;
+                            }
+                        }
+#pragma unroll
+                        for (int c = 0; c < 8; ++c) {
+                            typename Quad<VT>::raw v0[2], v1[2];
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) {
+                                const uint32_t a = stage_addr((((c < 4) ? sl[r].x : sl[r].y) >> (8 * (c & 3))) & 0xFFu) + st_off;
+                                v0[r] = Quad<VT>::load_shared(a);
+                                v1[r] = nunits > 1 ? Quad<VT>::load_shared(a + 32 * sizeof(VT)) : Quad<VT>::zero();
+                            }
+#pragma unroll
+                            for (int r = 0; r < 2; ++r)
+                                if (cw8[r][c] != 0.f) {
+                                    Quad<VT>::fma(acc[r][0], v0[r], cw8[r][c]);
+                                    Quad<VT>::fma(acc[r][1], v1[r], cw8[r][c]);
+                                }
+                        }
+                        store_row(row, acc[0]);
+                        store_row(row + 16, acc[1]);
+                    }
+                } else {
+                    const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
+                    const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
                     for (int row = 64 * cw + grp; row < 64 * cw + 64; row += 16) {
                         const float4 e = rows[row];
                         const bool occ = row < nrows && ((__float_as_uint(e.w) >> (28 + lvl)) & 1u);
@@ -659,69 +755,23 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                         if (occ) {
                             float gx, gy, gz;
                             world_to_grid(*xf, e.x, e.y, e.z, gx, gy, gz);
-                            Corners cn;
-                            const uint32_t cb = clamped_cell(gx, gy, gz, W, H, D, cn);
-                            float cw[8];
+                            float cw8[8];
+                            const uint32_t cb = setup(gx, gy, gz, cw8) * dX;
 #pragma unroll
-                            for (int c = 0; c < 8; ++c) cw[c] = __fmul_rn(__fmul_rn(cn.wx[c & 1], cn.wy[(c >> 1) & 1]), cn.wz[c >> 2]);
-                            blend(row, cb, cw, acc);
-                        }
+                            for (int uu = 0; uu < 2; ++uu) {
+                                if (uu >= nunits) continue;
+                                const unsigned char* ub = lvl_ptr + (size_t)(cbase0 + 32 * uu) * sizeof(VT);
+                                typename Quad<VT>::raw v[8];
 #pragma unroll
-                        for (int uu = 0; uu < 2; ++uu) {
-                            if (uu >= nunits) continue;
-                            const float (&a)[4] = acc[uu];
-                            const uint32_t off = act_off(row, kb + 32 * uu + 4 * t);
-                            uint2 hw, lw;
-                            if (NP == 3) {
-                                // (hi, lo) split with a truncated hi: the residual is exact
-                                hw.x = tc::cvt_rz_f16x2(a[0], a[1]); hw.y = tc::cvt_rz_f16x2(a[2], a[3]);
-                                float q0, q1, q2, q3;
-                                tc::trunc_residual2(a[0], a[1], q0, q1);
-                                tc::trunc_residual2(a[2], a[3], q2, q3);
-                                lw.x = tc::cvt_f16x2(q0, q1); lw.y = tc::cvt_f16x2(q2, q3);
-                                tcr::sts_v2(s_lo + off, lw);
-                            } else {
-                                hw.x = tc::cvt_f16x2(a[0], a[1]); hw.y = tc::cvt_f16x2(a[2], a[3]);
+                                for (int c = 0; c < 8; ++c)
+                                    v[c] = Quad<VT>::load_bytes(ub + cb + ((c & 1) ? dX : 0u) + ((c & 2) ? dY : 0u) + ((c & 4) ? dZ : 0u));
+#pragma unroll
+                                for (int c = 0; c < 8; ++c)
+                                    if (cw8[c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw8[c]);
                             }
-                            tcr::sts_v2(s_hi + off, hw);
                         }
+                        store_row(row, acc);
                     }
-                };
-                if (staged) {
-                    // shared-memory latency is short: one corner (both units) at a time keeps the registers low.  Each unit
-                    // still accumulates its corners in order 0..7.
-                    const uint32_t st_off = ((seg & 1) * 64 + 4 * t) * sizeof(VT);   // this lane's channels inside a voxel
-                    const int li = seg >> 1;
-                    rows_loop([&](int row, uint32_t, const float (&cw)[8], float (&acc)[2][4]) {
-                        const uint2 sl = *reinterpret_cast<const uint2*>(&vt->slot[row][li][0]);
-#pragma unroll
-                        for (int c = 0; c < 8; ++c) {
-                            const uint32_t a = stage_addr((((c < 4) ? sl.x : sl.y) >> (8 * (c & 3))) & 0xFFu) + st_off;
-                            const typename Quad<VT>::raw v0 = Quad<VT>::load_shared(a), v1 = Quad<VT>::load_shared(a + 32 * sizeof(VT));
-                            if (cw[c] != 0.f) {
-                                Quad<VT>::fma(acc[0], v0, cw[c]);
-                                Quad<VT>::fma(acc[1], v1, cw[c]);
-                            }
-                        }
-                    });
-                } else {
-                    const unsigned char* lvl_ptr = volbase + P.lvl_off[lvl] + ((size_t)P.frame * P.lvl_bstride[lvl] + 4 * t) * sizeof(VT);
-                    const uint32_t dX = (uint32_t)(C * sizeof(VT)), dY = dX * W, dZ = dY * H;
-                    rows_loop([&](int, uint32_t cell, const float (&cw)[8], float (&acc)[2][4]) {
-                        const uint32_t cb = cell * dX;
-#pragma unroll
-                        for (int uu = 0; uu < 2; ++uu) {
-                            if (uu >= nunits) continue;
-                            const unsigned char* ub = lvl_ptr + (size_t)(cbase0 + 32 * uu) * sizeof(VT);
-                            typename Quad<VT>::raw v[8];
-#pragma unroll
-                            for (int c = 0; c < 8; ++c)
-                                v[c] = Quad<VT>::load_bytes(ub + cb + ((c & 1) ? dX : 0u) + ((c & 2) ? dY : 0u) + ((c & 4) ? dZ : 0u));
-#pragma unroll
-                            for (int c = 0; c < 8; ++c)
-                                if (cw[c] != 0.f) Quad<VT>::fma(acc[uu], v[c], cw[c]);
-                        }
-                    });
                 }
             };
 
@@ -738,7 +788,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                 const uint32_t t0 = (uint32_t)clock();
                 gather(seg);
                 publish();
-                g_cycles += (uint32_t)clock() - t0;
+                (seg < 4 ? g_coarse : g_fine) += (uint32_t)clock() - t0;
                 const int nks = seg == NUM_SEGS - 1 ? 2 : 4, ka = 4 * (seg % SEG_BUFS);
                 for (int q = 0; q < nks; ++q) {
                     take([&](uint32_t slot) { mma256(slot, ka + q); });
@@ -848,16 +898,18 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
             tval(50, w_stall);
             tval(51, r_stall);
             tval(52, pe_stall);
-            tval(53, g_cycles);
-            w_stall = r_stall = pe_stall = g_cycles = 0;
+            tval(53, g_coarse);
+            tval(54, g_fine);
+            w_stall = r_stall = pe_stall = g_coarse = g_fine = 0;
         }
     }
     __syncthreads();
     if (tid == 0 && P.stats) {
         atomicMax(P.frame_clock + 1, global_ns());
-        const uint32_t* paths = reinterpret_cast<const uint32_t*>(smem + OFF_HCNT) + NTAB;
+        const uint32_t* paths = reinterpret_cast<const uint32_t*>(smem + OFF_HCNT) + 2;
         atomicAdd(P.stats + 5, (unsigned long long)paths[0]);             // coarse-level half tiles gathered from the staging
-        atomicAdd(P.stats + 6, (unsigned long long)paths[1]);             // ... and directly (more than NV distinct voxels)
+        atomicAdd(P.stats + 6, (unsigned long long)paths[1]);             // ... and directly (more than NV_COARSE distinct voxels)
+        atomicAdd(P.stats + 7, (unsigned long long)paths[2]);             // fine-level half tiles gathered directly
     }
 }
 

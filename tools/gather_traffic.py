@@ -4,10 +4,11 @@ Replays what the list pipeline does with one view of a synthetic scene (oracle/s
 four cell-occupancy bits and class (finest occupied level), the class lists in the classifier's order (blocks of
 1024 / S rays, sample-major, one class after the other), and 128-row tiles of two 64-row halves.  For every level it
 prints the corner-vector bytes the gather requests (8 per occupied row), the bytes of the distinct voxels per tile, and
-the distribution of distinct voxels per half tile; for the coarse levels 3 and 2 also the share of half tiles that do not
-fit a staging buffer of --nv voxels (the decoder gathers those directly from global memory).
+the distribution of distinct voxels per half tile, and the share of half tiles that do not fit the decoder's staging of
+--nv voxels (coarse levels 3 and 2) or --nv-fine voxels (fine levels 1 and 0); the decoder gathers those directly from
+global memory.
 
-    python tools/gather_traffic.py [--size 512] [--samples 64] [--nv 64]
+    python tools/gather_traffic.py [--size 512] [--samples 64] [--nv 64] [--nv-fine 128]
 
 The feature volumes are the scene's dense synthetic ones: a voxel is occupied when any of its channels is non-zero."""
 import argparse
@@ -100,6 +101,7 @@ def main():
     ap.add_argument("--size", type=int, default=512, help="image side (c2: 512)")
     ap.add_argument("--samples", type=int, default=64)
     ap.add_argument("--nv", type=int, default=64, help="staged voxels per half tile and coarse level")
+    ap.add_argument("--nv-fine", type=int, default=128, help="staged voxels per half tile and fine level")
     ap.add_argument("--sms", type=int, default=132)
     args = ap.parse_args()
     levels, lm, cls, order = replay(args.size, args.samples)
@@ -108,7 +110,8 @@ def main():
     print("synth-313, %dx%d, %d samples: %d listed samples, %d tiles (%.0f per CTA on %d SMs)"
           % (args.size, args.size, args.samples, int((cls >= 0).sum()), n_tiles, n_tiles / args.sms, args.sms))
     print("| level (channels, fp32 B/voxel) | corner bytes requested | distinct voxel bytes per tile | ratio | "
-          "distinct voxels per half tile p50 / p99 / max | half tiles over %d voxels |" % args.nv)
+          "distinct voxels per half tile p50 / p99 / max | half tiles over the staging (%d coarse / %d fine voxels) |"
+          % (args.nv, args.nv_fine))
     print("|---|---|---|---|---|---|")
     tot_req = tot_uniq = 0
     for lvl in (3, 2, 1, 0):
@@ -132,7 +135,7 @@ def main():
             has_rows = valid.reshape(len(t) * 2, HALF).any(1)
             halves.append(hv[has_rows])
         h = np.concatenate(halves) if halves else np.zeros(1, np.int64)
-        over = "%.2f %%" % (100.0 * (h > args.nv).mean()) if lvl >= 2 else "(direct)"
+        over = "%.2f %%" % (100.0 * (h > (args.nv if lvl >= 2 else args.nv_fine)).mean())
         print("| %d (%d ch, %d B; %.1f MB) | %.1f GB | %.2f GB | %.1fx | %d / %d / %d | %s |"
               % (lvl, L["C"], vb, np.prod(L["dims"]) * vb / 1e6, req / 1e9, uniq / 1e9, req / max(1, uniq),
                  np.percentile(h, 50), np.percentile(h, 99), h.max(), over))

@@ -13,7 +13,7 @@ import torch  # noqa: E402
 PROD = {1: "tile begin", 30: "next tile's rows loaded", 31: "L2 done seen", 32: "per-point tile written"}
 MMA = {1: "tile begin", 20: "L0 retired", 21: "L1 retired", 22: "L2 retired", 23: "L3 retired", 24: "raw stored"}
 LOAD = {1: "first push of a tile issued", 2: "last push of a tile issued"}
-VALUES = {50: "weight wait", 51: "row wait", 52: "per-point tile wait", 53: "gather"}     # cycles per tile, not clocks
+VALUES = {50: "weight wait", 51: "row wait", 52: "per-point tile wait", 53: "gather coarse", 54: "gather fine"}   # cycles per tile
 LAYERS = [(1, 20, "L0"), (20, 21, "L1"), (21, 22, "L2"), (22, 23, "L3"), (23, 24, "head")]
 
 
@@ -43,6 +43,7 @@ def main():
     staged, direct = int(ren.stats[5]), int(ren.stats[6])
     print("coarse-level half tiles (levels 3 and 2, all CTAs): %d staged, %d direct (%.2f%% direct)"
           % (staged, direct, 100.0 * direct / max(1, staged + direct)))
+    print("fine-level half tiles (levels 1 and 0, all CTAs): %d direct" % int(ren.stats[7]))
     t = trace.cpu().view(4, 4096)
     roles = [("PROD", PROD, None, 1), ("MMA0", MMA, None, 1), ("MMA1", MMA, None, 1), ("LOAD", LOAD, None, 1)]
     per_tile = {}                                            # (role, tile) -> {code: clock or value}
