@@ -205,6 +205,19 @@ int nb_sample_pdf(const nb_importance_args* args, void* stream);
  * points: device (B, n_points, 3) world coordinates; sigma: device (B, n_points). */
 int nb_decode_density(const nb_render_args* frame, const float* points, int n_points, float* sigma, void* stream);
 
+/* The same density on the tensor cores (opt-in; nb_decode_density stays the exact reference).  Reads the frame fields of
+ * nb_decode_density plus precision (NB_PRECISION_TC_FP16X3 or NB_PRECISION_TC_FP16; anything else is NB_ERR_BAD_ARG),
+ * skip_empty, workspace / workspace_bytes (required, nb_decode_density_workspace_bytes), stats ([0]-[7] as for
+ * nb_render_fwd, [1] = listed points) and trace.  sigma (B, n_points) is raw sigma, no relu.  With skip_empty = 1 a point
+ * whose trilinear cells are unoccupied on all four levels (its features are all exactly 0, also outside the volume) gets
+ * sigma_empty of the weight blob, whatever its sign; every other point goes through the decoder, and its sigma does not
+ * depend on which points share its tile: it is the same bit for bit with skipping on or off and under any permutation of
+ * the points.  n_points >= 2^28 returns NB_ERR_UNSUPPORTED before anything is enqueued; n_points = 0 is a no-op.  Per
+ * frame: a classification launch and the decoder (plus a 1-thread launch that accounts stats[2] / [3] when stats is set),
+ * after one memset of the control blocks per call. */
+size_t nb_decode_density_workspace_bytes(int batch, int n_points);   /* control blocks + two list buffers of n_points entries */
+int    nb_decode_density_list(const nb_render_args* frame, const float* points, int n_points, float* sigma, void* stream);
+
 /* Marching cubes over a dense fp32 grid: the mesh step of the mesh renderer (lib/networks/renderer/if_mesh_renderer.py:42-48,
  * mcubes.marching_cubes(cube, cfg.mesh_th)).  A grid value is inside when it is > isovalue (equal counts as outside).
  * Vertices are the crossed grid edges p -> p + e_a, at p + t e_a with t = (iso - v(p)) / (v(p + e_a) - v(p)) in fp64, in

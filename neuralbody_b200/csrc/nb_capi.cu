@@ -481,6 +481,7 @@ int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out) {
     }
     p.rays_per_group = p.tiles_per_group = p.n_groups = p.groups_per_frame = 0;
     p.frame = 0; p.train_list = 0; p.list_a = p.list_b = nullptr; p.list_cap = 0; p.list_count = nullptr; p.frame_clock = nullptr; p.raw_ws = nullptr;
+    p.points = nullptr; p.sigma = nullptr; p.n_points = 0;
 
     return NB_OK;
 }
@@ -512,20 +513,45 @@ int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, in
     return NB_OK;
 }
 
-int nb_decode_density(const nb_render_args* a, const float* points, int n_points, float* sigma, void* stream) {
-    if (!a || !points || !sigma || n_points < 0) { set_error("nb_decode_density: null argument"); return NB_ERR_BAD_ARG; }
-    // reuse the forward call's validation: only the frame / volume / weight fields matter here
+// the density calls reuse the forward call's validation: only the frame / volume / weight fields (and the tensor-core
+// options) matter there
+static int fill_density_params(const nb_render_args* a, RenderParams* p) {
     nb_render_args tmp = *a;
-    static float dummy;   // never dereferenced: the density kernel touches no ray or output-map pointer
+    static float dummy;   // never dereferenced: the density kernels touch no ray or output-map pointer
     float* d = &dummy;
     tmp.n_rays = 1; tmp.n_samples = 1;
     tmp.ray_o = tmp.ray_d = tmp.near = tmp.far = d;
     tmp.rgb_map = tmp.disp_map = tmp.acc_map = tmp.depth_map = d;
     tmp.mask_msks = nullptr; tmp.save = nullptr;
+    return nbi_fill_render_params(&tmp, p);
+}
+
+int nb_decode_density(const nb_render_args* a, const float* points, int n_points, float* sigma, void* stream) {
+    if (!a || !points || !sigma || n_points < 0) { set_error("nb_decode_density: null argument"); return NB_ERR_BAD_ARG; }
     RenderParams p;
-    const int stp = nbi_fill_render_params(&tmp, &p);
+    const int stp = fill_density_params(a, &p);
     if (stp != NB_OK) return stp;
     return launch_density_f32(p, a->volume_dtype, points, n_points, sigma, (cudaStream_t)stream);
+}
+
+size_t nb_decode_density_workspace_bytes(int batch, int n_points) {
+    if (batch <= 0 || n_points <= 0) return 0;
+    return density_tc_list_workspace_bytes(batch, n_points);
+}
+
+int nb_decode_density_list(const nb_render_args* a, const float* points, int n_points, float* sigma, void* stream) {
+    if (!a || !points || !sigma || n_points < 0) { set_error("nb_decode_density_list: null argument or n_points < 0"); return NB_ERR_BAD_ARG; }
+    if (a->precision != NB_PRECISION_TC_FP16X3 && a->precision != NB_PRECISION_TC_FP16) {
+        set_error("nb_decode_density_list: precision %d; it runs NB_PRECISION_TC_FP16X3 or NB_PRECISION_TC_FP16 (exact fp32: "
+                  "nb_decode_density)", a->precision);
+        return NB_ERR_BAD_ARG;
+    }
+    RenderParams p;
+    const int stp = fill_density_params(a, &p);
+    if (stp != NB_OK) return stp;
+    p.points = points; p.sigma = sigma; p.n_points = n_points;
+    return launch_density_tc_list(p, a->volume_dtype, a->precision == NB_PRECISION_TC_FP16X3 ? 3 : 1, a->workspace,
+                                  a->workspace_bytes, (cudaStream_t)stream);
 }
 
 int nb_render_fwd(const nb_render_args* a, void* stream) {

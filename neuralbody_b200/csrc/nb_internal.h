@@ -61,6 +61,10 @@ struct RenderParams {
     unsigned int* list_count;  // [4] entries per class, appended by classify_compact_kernel
     unsigned long long* frame_clock;   // [0] max(~start), [1] max(end) of the decoder launch (%globaltimer ns)
     float4* raw_ws;            // (n, S) raw records of this frame: (rgb logits, sigma)
+    // density queries (nb_decode_density_list): world points in, raw sigma out; the list entry ids are point ids
+    const float* points;       // (n_points, 3) of this frame (the launch) / of frame 0 (the caller)
+    float* sigma;              // (n_points) likewise
+    int n_points;
 };
 
 int launch_render_f32(const RenderParams& p, int volume_dtype, cudaStream_t stream);
@@ -68,6 +72,8 @@ int launch_render_tc_list(const RenderParams& p, int volume_dtype, int passes, v
 size_t render_tc_list_workspace_bytes(int batch, int n_rays, int n_samples);
 bool render_tc_list_supported(const RenderParams& p);
 int launch_density_f32(const RenderParams& p, int volume_dtype, const float* pts, int n_points, float* sigma, cudaStream_t stream);
+int launch_density_tc_list(const RenderParams& p, int volume_dtype, int passes, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t density_tc_list_workspace_bytes(int batch, int n_points);
 bool tc_available();
 
 }  // namespace nb

@@ -18,6 +18,11 @@
 //
 // Results do not depend on the (non-deterministic) order of the blocks in the list: a tile row is evaluated
 // independently of its neighbours.  The list and the raw (rgb logits, sigma) records cross HBM once each way.
+//
+// Density queries (nb_decode_density_list, the mesh renderer) run the same pipeline on world points instead of ray
+// samples: classify_points_kernel lists the points (a point whose cells are unoccupied on every level gets sigma_empty at
+// once with skip_empty = 1), and density_tc_list_kernel, the decoder with layer 3 and the rgb head left out, writes raw
+// sigma (layers 0-2 and alpha_fc) for the listed ones.  There is no composite.
 #include "nb_tc_common.cuh"
 #include <type_traits>
 
@@ -142,6 +147,76 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
     }
 }
 
+// bit l = the level-l trilinear cell at grid coordinates (gx, gy, gz) holds a non-zero voxel of frame b.  A cell with no
+// corner inside the volume (outside the box, where grid_sample pads with zeros) holds none.
+__device__ __forceinline__ uint32_t occupied_levels(const RenderParams& P, int b, float gx, float gy, float gz) {
+    const uint32_t* occ_base = reinterpret_cast<const uint32_t*>(P.volume);
+    uint32_t lm = 0;
+#pragma unroll
+    for (int lvl = 0; lvl < 4; ++lvl) {
+        const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+        Corners cn;
+        corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+        if (cn.x0 != -2 && cn.x0 < W && cn.y0 < H && cn.z0 < D) {
+            const uint32_t* cellbits = occ_base + P.occ_off[lvl] / 4 + (size_t)b * P.occ_bstride[lvl];
+            const uint32_t cell = ((uint32_t)(cn.z0 + 1) * (H + 1) + (cn.y0 + 1)) * (W + 1) + (cn.x0 + 1);
+            lm |= ((__ldg(cellbits + (cell >> 5)) >> (cell & 31)) & 1u) << lvl;
+        }
+    }
+    return lm;
+}
+
+// ------------------------------------------------------------------------------------------------ 1'. classify points
+// Density queries: one thread per world point of frame P.frame.  A point whose cells are unoccupied on all four levels has
+// all-zero features, so its raw sigma is sigma_empty whatever the sign: with skip_empty it is written at once.  Every other
+// point (all of them with skip_empty = 0) is appended to the list of its class as classify_compact_kernel does, in point
+// order inside the block (neighbouring grid points share their corner voxels).  Entry: (world xyz, point id | level bits << 28).
+__global__ void __launch_bounds__(CLS_THREADS) classify_points_kernel(const __grid_constant__ RenderParams P) {
+    __shared__ FrameXf xf;
+    __shared__ int wcnt[4][CLS_THREADS / 32];
+    __shared__ unsigned int sbase[4];
+    __shared__ int stotal[4];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int b = P.frame, n = P.n_points;
+    const int i = blockIdx.x * CLS_THREADS + tid;
+    load_frame_xf(P, &xf, tid);
+    __syncthreads();
+    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
+    int cls = -1;                                     // 0..3 = finest occupied level (list class), -1 = not listed
+    if (i < n) {
+        const float* q = P.points + (size_t)i * 3;
+        e.x = __ldg(q); e.y = __ldg(q + 1); e.z = __ldg(q + 2);
+        float gx, gy, gz;
+        world_to_grid(xf, e.x, e.y, e.z, gx, gy, gz);
+        const uint32_t lm = occupied_levels(P, b, gx, gy, gz);
+        if (lm != 0u || !P.skip_empty) cls = lm ? __ffs((int)lm) - 1 : 3;
+        e.w = __uint_as_float((uint32_t)i | (lm << 28));
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const uint32_t bal = __ballot_sync(0xffffffffu, cls == c);
+        if (lane == 0) wcnt[c][warp] = __popc(bal);
+    }
+    __syncthreads();
+    if (tid < 4) {                                    // one reservation per class and block
+        int total = 0;
+        for (int w = 0; w < CLS_THREADS / 32; ++w) total += wcnt[tid][w];
+        stotal[tid] = total;
+        sbase[tid] = total ? atomicAdd(P.list_count + tid, (unsigned int)total) : 0u;
+    }
+    __syncthreads();
+    const uint32_t same = __match_any_sync(0xffffffffu, cls);
+    if (cls >= 0) {
+        int local = __popc(same & ((1u << lane) - 1));
+        for (int w = 0; w < warp; ++w) local += wcnt[cls][w];
+        float4* buf = cls >= 2 ? P.list_a : P.list_b;          // the buffers and growth directions of classify_compact_kernel
+        const size_t at = (cls & 1) ? (size_t)sbase[cls] + local : P.list_cap - (size_t)sbase[cls] - stotal[cls] + local;
+        buf[at] = e;
+    } else if (i < n) {
+        P.sigma[i] = __ldg(P.wf32 + oSigmaEmpty);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
 // One persistent CTA per SM walks the frame's tiles of TP = 128 list rows.  The CTA is warp-specialised:
 //   producer warpgroup (warps 0-3)   warp 0: one elected lane streams the weights with bulk copies into a 4-slot ring (one
@@ -254,8 +329,11 @@ __device__ __forceinline__ uint32_t clamped_cell(float gx, float gy, float gz, i
     return (uint32_t)((zc * H + yc) * W + xc);
 }
 
-template <int NP, typename VT>
-__global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_constant__ RenderParams P) {
+// The decoder over the list: the body of render_tc_list_kernel and, with DENSITY, of density_tc_list_kernel.  DENSITY runs
+// layers 0-2 and alpha_fc only: the weight stream stops after layer 2, the row warps write no per-point tile (l2_done and
+// pe_full are not used), and the consumers store raw sigma to P.sigma[id] in place of the raw record.
+template <int NP, typename VT, bool DENSITY>
+__device__ __forceinline__ void decode_list(const RenderParams& P) {
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
     FrameXf* xf = reinterpret_cast<FrameXf*>(smem + OFF_XF);
@@ -338,7 +416,8 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                     const int l0_ksteps = class_ksteps(tref.cls);
                     real_tiles += tref.nrows > 0;
                     real_ksteps += tref.nrows > 0 ? l0_ksteps : 0;
-                    for (int j = 0; j < pushes_per_tile(l0_ksteps); ++j, ++g) {
+                    const int npush = pushes_per_tile(l0_ksteps) - (DENSITY ? L3_PUSHES : 0);
+                    for (int j = 0; j < npush; ++j, ++g) {
                         const uint32_t slot = g % NUM_SLOTS;
                         tc::mbar_wait(&bars[B_EMPTY + slot], ((g / NUM_SLOTS) & 1) ^ 1);   // (the first round passes at once)
                         if (j == 0) tl.ev(1);
@@ -486,7 +565,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                     tr.ev(1);
                 }
                 load_rows((it + 1) & 1, tile + gridDim.x);
-                if (it < 0) continue;
+                if (DENSITY || it < 0) continue;
                 tr.ev(30);
                 const TileRef tref = tile_ref(tile);
                 const int nrows = tref.nrows;
@@ -526,8 +605,9 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
         const int cw = wgid - 1;                                        // rows [64 cw, 64 cw + 64) of a tile
         const bool arr = lane == 0;                                     // the warp's arrival on the consumer-side barriers
         // trace events of the warpgroup (CTA 0, its first thread): only the entry index lives in a register, the buffer is
-        // read from the kernel parameters at each event (same records as tcr::Tracer)
-        int tn = ((tid & 127) == 0 && blockIdx.x == 0 && P.trace) ? (1 + cw) * 4096 : -1;
+        // read from the kernel parameters at each event (same records as tcr::Tracer).  DENSITY records none: without them
+        // its consumers stay spill-free
+        int tn = (!DENSITY && (tid & 127) == 0 && blockIdx.x == 0 && P.trace) ? (1 + cw) * 4096 : -1;
         auto tval = [&](int code, unsigned long long v) {
             if (tn >= 0 && tn < (2 + cw) * 4096) P.trace[tn++] = ((unsigned long long)code << 48) | (v & 0xFFFFFFFFFFFFull);
         };
@@ -596,6 +676,7 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                             float& sg = hr ? sig1 : sig0;
                             sg = fmaf(fmaxf(x0, 0.f), aw.x, sg);
                             sg = fmaf(fmaxf(x1, 0.f), aw.y, sg);
+                            if (DENSITY) continue;                      // no layer 3 reads h2
                             hv = tc::cvt_relu_f16x2(x0, x1);
                         } else if (NP == 3) {
                             hv = tc::cvt_rz_relu_f16x2(x0, x1);
@@ -821,10 +902,24 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
                     convert(false);                                     // h1
                     init_bias(head + H_B0 + 2 * kHidden);
                 } else {
-                    tc::mbar_arrive_if(&bars[B_L2DONE], arr);           // the lo plane is free for the per-point tile
-                    sig = convert(true);                                // h2, and this thread's share of sigma
+                    if (!DENSITY) tc::mbar_arrive_if(&bars[B_L2DONE], arr);   // the lo plane is free for the per-point tile
+                    sig = convert(true);                                // h2 (not stored by DENSITY), and this thread's share of sigma
                 }
                 publish();
+            }
+            if constexpr (DENSITY) {
+                float sg[2] = {sig.x, sig.y};
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+                    for (int o = 1; o <= 2; o <<= 1) sg[hr] += __shfl_xor_sync(0xffffffffu, sg[hr], o);
+                    const int row = r0 + 8 * hr;
+                    if ((lane & 3) == 0 && row < nrows) {
+                        const uint32_t id = __float_as_uint(rows[row].w) & ID_MASK;
+                        P.sigma[id] = sg[hr] + head[H_ALPHA + kHidden];
+                    }
+                }
+                continue;
             }
             // ================= layer 3 (the folded colour layer, N = 128 as two halves of 64): A = h2 (hi plane) for K-steps
             // 0..15, the per-point tile (lo plane) for 16..21
@@ -913,17 +1008,30 @@ __global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_cons
     }
 }
 
+template <int NP, typename VT>
+__global__ void __launch_bounds__(NT, 1) render_tc_list_kernel(const __grid_constant__ RenderParams P) {
+    decode_list<NP, VT, false>(P);
+}
+template <int NP, typename VT>
+__global__ void __launch_bounds__(NT, 1) density_tc_list_kernel(const __grid_constant__ RenderParams P) {
+    decode_list<NP, VT, true>(P);
+}
+
+// stats[2] / [3]: the device-timed duration of the decoder launch that fed this frame, once the launch is complete
+__device__ __forceinline__ void add_decoder_time(const RenderParams& P) {
+    const unsigned long long t0 = ~P.frame_clock[0], t1 = P.frame_clock[1];
+    atomicAdd(P.stats + 2, t1 > t0 ? t1 - t0 : 0ull);
+    atomicAdd(P.stats + 3, 1ull);
+}
+__global__ void decoder_time_kernel(const __grid_constant__ RenderParams P) { add_decoder_time(P); }
+
 // ------------------------------------------------------------------------------------------------ 3. raw2outputs
 constexpr int COMP_WARPS = 8;
 __global__ void __launch_bounds__(COMP_WARPS * 32) composite_kernel(const __grid_constant__ RenderParams P) {
     __shared__ float zs[COMP_WARPS][MAXS];          // rays of up to MAXS samples (the decoder itself does not care about S)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ray = blockIdx.x * COMP_WARPS + warp;
-    if (blockIdx.x == 0 && threadIdx.x == 0 && P.stats) {      // device-timed duration of the decoder launch that fed this frame
-        const unsigned long long t0 = ~P.frame_clock[0], t1 = P.frame_clock[1];
-        atomicAdd(P.stats + 2, t1 > t0 ? t1 - t0 : 0ull);
-        atomicAdd(P.stats + 3, 1ull);
-    }
+    if (blockIdx.x == 0 && threadIdx.x == 0 && P.stats) add_decoder_time(P);
     if (ray >= P.n_rays) return;
     const int S = P.n_samples;
     const size_t rg = (size_t)P.frame * P.n_rays + ray;
@@ -945,12 +1053,27 @@ __global__ void __launch_bounds__(COMP_WARPS * 32) composite_kernel(const __grid
     }
 }
 
-template <int NP, typename VT>
+template <int NP, typename VT, bool DENSITY>
 static cudaError_t launch_list(const RenderParams& p, int grid, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(render_tc_list_kernel<NP, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    void (*kernel)(RenderParams) = DENSITY ? density_tc_list_kernel<NP, VT> : render_tc_list_kernel<NP, VT>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
-    render_tc_list_kernel<NP, VT><<<grid, NT, SMEM_BYTES, stream>>>(p);
+    kernel<<<grid, NT, SMEM_BYTES, stream>>>(p);
     return cudaGetLastError();
+}
+template <bool DENSITY>
+static cudaError_t launch_decoder(const RenderParams& p, int volume_dtype, int passes, int grid, cudaStream_t stream) {
+    if (passes == 3) return volume_dtype == NB_DTYPE_F32 ? launch_list<3, float, DENSITY>(p, grid, stream) : launch_list<3, __half, DENSITY>(p, grid, stream);
+    return volume_dtype == NB_DTYPE_F32 ? launch_list<1, float, DENSITY>(p, grid, stream) : launch_list<1, __half, DENSITY>(p, grid, stream);
+}
+// one persistent CTA per SM; the tile count of a frame is only known on the device, so the grid is sized for the worst case
+// (every entry listed) and tiles past the end are no-ops
+static int decoder_grid(size_t max_entries) {
+    int dev = 0, sms = kGridSMs;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const long long max_tiles = ((long long)max_entries + TP - 1) / TP + 4;
+    return (int)(max_tiles < sms ? max_tiles : sms);
 }
 
 static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -1000,18 +1123,13 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
     p.groups_per_frame = (p.n_rays + p.rays_per_group - 1) / p.rays_per_group;
     p.n_groups = p.groups_per_frame * p.batch;
     if (p.n_rays == 0) return NB_OK;
-    int dev = 0, sms = kGridSMs;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t per_frame = tcl::align256((size_t)p.n_rays * S * sizeof(float4));
     unsigned char* ws = static_cast<unsigned char*>(workspace);
     float4* list = reinterpret_cast<float4*>(ws + tcl::align256((size_t)p.batch * tcl::CTL_BYTES));
     float4* raw_ws = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(list) + 2 * per_frame);
     cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
     if (e != cudaSuccess) { set_error("render_tc_list: memset failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    // the tile count of a frame is only known on the device: size the grid for the worst case (every sample occupied)
-    const long long max_tiles = ((long long)p.n_rays * S + tcl::TP - 1) / tcl::TP + 4;
-    const int grid = (int)(max_tiles < sms ? max_tiles : sms);         // one persistent CTA per SM; tiles past the end are no-ops
+    const int grid = tcl::decoder_grid((size_t)p.n_rays * S);
     for (int b = 0; b < p.batch; ++b) {
         p.frame = b;
         p.list_a = list;
@@ -1022,15 +1140,59 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
         p.raw_ws = p_in.raw ? reinterpret_cast<float4*>(p_in.raw) + (size_t)b * p.n_rays * S : raw_ws;
         tcl::classify_compact_kernel<<<p.groups_per_frame, tcl::CLS_THREADS, 0, stream>>>(p);
         e = cudaGetLastError();
-        if (e == cudaSuccess) {
-            if (passes == 3) e = (volume_dtype == NB_DTYPE_F32) ? tcl::launch_list<3, float>(p, grid, stream) : tcl::launch_list<3, __half>(p, grid, stream);
-            else e = (volume_dtype == NB_DTYPE_F32) ? tcl::launch_list<1, float>(p, grid, stream) : tcl::launch_list<1, __half>(p, grid, stream);
-        }
+        if (e == cudaSuccess) e = tcl::launch_decoder<false>(p, volume_dtype, passes, grid, stream);
         if (e == cudaSuccess) {
             tcl::composite_kernel<<<(p.n_rays + tcl::COMP_WARPS - 1) / tcl::COMP_WARPS, tcl::COMP_WARPS * 32, 0, stream>>>(p);
             e = cudaGetLastError();
         }
         if (e != cudaSuccess) { set_error("render_tc_list launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
+    }
+    return NB_OK;
+}
+
+size_t density_tc_list_workspace_bytes(int batch, int n_points) {
+    return tcl::align256((size_t)batch * tcl::CTL_BYTES) + 2 * tcl::align256((size_t)n_points * sizeof(float4));   // control + 2 list buffers
+}
+
+// p.points / p.sigma / p.n_points set by the caller for the whole batch
+int launch_density_tc_list(const RenderParams& p_in, int volume_dtype, int passes, void* workspace, size_t workspace_bytes,
+                           cudaStream_t stream) {
+    RenderParams p = p_in;
+    const int n = p.n_points;
+    if ((size_t)n > (size_t)tcl::ID_MASK) {
+        set_error("nb_decode_density_list: n_points = %d; the tensor-core list holds < 2^28 points per frame", n);
+        return NB_ERR_UNSUPPORTED;
+    }
+    if (n == 0) return NB_OK;
+    if (!workspace || workspace_bytes < density_tc_list_workspace_bytes(p.batch, n)) {
+        set_error("nb_decode_density_list: needs nb_render_args.workspace (%zu bytes given, %zu needed; see "
+                  "nb_decode_density_workspace_bytes)", workspace ? workspace_bytes : (size_t)0,
+                  density_tc_list_workspace_bytes(p.batch, n));
+        return NB_ERR_BAD_ARG;
+    }
+    const size_t per_frame = tcl::align256((size_t)n * sizeof(float4));
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    float4* list = reinterpret_cast<float4*>(ws + tcl::align256((size_t)p.batch * tcl::CTL_BYTES));
+    cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
+    if (e != cudaSuccess) { set_error("density_tc_list: memset failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
+    const int grid = tcl::decoder_grid((size_t)n);
+    for (int b = 0; b < p.batch; ++b) {
+        p.frame = b;
+        p.list_a = list;
+        p.list_b = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(list) + per_frame);
+        p.list_cap = (size_t)n;
+        p.list_count = reinterpret_cast<unsigned int*>(ws + (size_t)b * tcl::CTL_BYTES);
+        p.frame_clock = reinterpret_cast<unsigned long long*>(ws + (size_t)b * tcl::CTL_BYTES + 16);
+        p.points = p_in.points + (size_t)b * n * 3;
+        p.sigma = p_in.sigma + (size_t)b * n;
+        tcl::classify_points_kernel<<<(n + tcl::CLS_THREADS - 1) / tcl::CLS_THREADS, tcl::CLS_THREADS, 0, stream>>>(p);
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = tcl::launch_decoder<true>(p, volume_dtype, passes, grid, stream);
+        if (e == cudaSuccess && p.stats) {
+            tcl::decoder_time_kernel<<<1, 1, 0, stream>>>(p);
+            e = cudaGetLastError();
+        }
+        if (e != cudaSuccess) { set_error("density_tc_list launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     }
     return NB_OK;
 }

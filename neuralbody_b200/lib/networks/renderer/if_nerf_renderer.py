@@ -475,15 +475,22 @@ class Renderer:
         return w, keep
 
     def calculate_density(self, wpts, feature_volume, sp_input):
-        """Network.calculate_density (latent_xyzc.py:74-89) on arbitrary world points: (B,P,3) -> (B,P,1).
-        f-3: the alpha decoder of the mesh renderer (if_mesh_renderer.py:36-41); exact fp32 kernel."""
+        """Network.calculate_density (latent_xyzc.py:74-89) on arbitrary world points: (B,P,3) -> (B,P,1), raw sigma.
+        f-3: the alpha decoder of the mesh renderer (if_mesh_renderer.py:36-41).  `cfg.density_precision`: 'fp32' (default,
+        the exact kernel nb_decode_density), or 'tc_fp16x3' / 'tc_fp16' (nb_decode_density_list on the tensor cores; with
+        `cfg.render_skip_empty` a point with all-zero features gets sigma(empty) without running the decoder)."""
         cfg = get_active_cfg()
         dev = wpts.device
         if dev.type != "cuda":
             raise RuntimeError("calculate_density needs CUDA tensors: there is no CPU implementation")
+        name = str(self._opt("density_precision", "fp32"))
+        if name not in _PRECISIONS:
+            raise ValueError("cfg.density_precision must be one of %s" % sorted(_PRECISIONS))
+        precision = _PRECISIONS[name]
+        vdtype = capi.NB_DTYPE_F32 if precision == capi.NB_PRECISION_FP32 else self._volume_dtype(precision)
         B, Pn = int(wpts.shape[0]), int(wpts.shape[1])
         with torch.cuda.device(dev), torch.no_grad():
-            vol_blob, dims = self.pack_volume(feature_volume, capi.NB_DTYPE_F32)
+            vol_blob, dims = self.pack_volume(feature_volume, vdtype)
             w_blob = self.pack_weights(sp_input['latent_index'], dev)
             pts = _f32c(wpts, dev)
             R, Th = _f32c(sp_input['R'], dev), _f32c(sp_input['Th'], dev).reshape(B, 3)
@@ -498,11 +505,22 @@ class Renderer:
             for l in range(capi.NB_NUM_LEVELS):
                 for j in range(4):
                     a.level_dims[l][j] = dims[l][j]
-            a.volume_blob, a.volume_dtype, a.weights_blob = vol_blob.data_ptr(), capi.NB_DTYPE_F32, w_blob.data_ptr()
-            a.precision = capi.NB_PRECISION_FP32
+            a.volume_blob, a.volume_dtype, a.weights_blob = vol_blob.data_ptr(), vdtype, w_blob.data_ptr()
+            a.precision = precision
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_decode_density(C.byref(a), pts.data_ptr(), Pn, sigma.data_ptr(), C.c_void_p(stream)),
-                       "nb_decode_density")
+            if precision == capi.NB_PRECISION_FP32:
+                capi.check(self.lib.nb_decode_density(C.byref(a), pts.data_ptr(), Pn, sigma.data_ptr(), C.c_void_p(stream)),
+                           "nb_decode_density")
+                self.launches += 1
+            else:   # per frame: classify the points -> decoder over the listed ones
+                stats = getattr(self, "stats", None)
+                a.skip_empty = 1 if bool(self._opt("render_skip_empty", True)) else 0
+                a.stats = stats.data_ptr() if stats is not None else None
+                ws = self._workspace(self.lib.nb_decode_density_workspace_bytes(B, Pn), dev)
+                a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+                capi.check(self.lib.nb_decode_density_list(C.byref(a), pts.data_ptr(), Pn, sigma.data_ptr(),
+                                                           C.c_void_p(stream)), "nb_decode_density_list")
+                self.launches += B * (2 + (stats is not None))
         return sigma
 
     def get_pixel_value(self, ray_o, ray_d, near, far, feature_volume, sp_input, batch):

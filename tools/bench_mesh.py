@@ -3,7 +3,12 @@
 into its steps with CUDA events after warm-up.  Prints one JSON line with the split, the density kernel's FP32 rate, the
 marching-cubes bytes/s, and the card's name and power limit read in the same run.  Writes nothing.
 
-Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10]
+--density-precision picks cfg.density_precision (fp32, the default, or the tensor-core tc_fp16x3 / tc_fp16); --ab alternates
+fp32 and tc_fp16x3 step by step in one process and reports the density ms of both arms.  For a tensor-core arm it also
+reports the points listed for the decoder and skipped (stats[1]) and the algorithmic rate on the evaluated points only:
+fc_0 (minus the layer-0 K-steps the tile's class skipped, as bench.py counts them for rays) + fc_1 + fc_2 + alpha_fc.
+
+Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab]
 (upstream's default mesh_th = 50 lies above the synthetic body's sigma, p95 ~ 30, and would give an empty mesh)"""
 import argparse
 import json
@@ -18,6 +23,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 FLOP_PER_POINT_DENSITY = 442880         # fc_0 + fc_1 + fc_2 + alpha_fc: 2 x (352*256 + 2*256*256 + 256) MAC per point
+FLOP_L0_PER_KSTEP = 2 * 16 * 256        # one layer-0 K-step (16 of fc_0's 352 inputs), per point
 FP32_TFLOPS_DATASHEET = 67.0             # H100 SXM data sheet, dense FP32 (700 W card)
 HBM_TBS_DATASHEET = 3.35                 # H100 SXM data sheet, HBM3
 PAD = 10
@@ -46,7 +52,10 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--mesh-th", type=float, default=10.0, help="isovalue (cfg.mesh_th)")
+    ap.add_argument("--density-precision", choices=("fp32", "tc_fp16x3", "tc_fp16"), default="fp32")
+    ap.add_argument("--ab", action="store_true", help="alternate fp32 and tc_fp16x3 density steps in one process")
     args = ap.parse_args()
+    arms = ("fp32", "tc_fp16x3") if args.ab else (args.density_precision,)
     if not torch.cuda.is_available():
         raise SystemExit("bench_mesh needs a CUDA device")
     from oracle import mesh_case
@@ -67,8 +76,13 @@ def main():
     ren = load_source("neuralbody_b200.lib.networks.renderer.if_mesh_renderer", path).Renderer(net)
     bd = {k: v.to(dev) for k, v in batch.items()}
 
-    def frame():
+    stats = torch.zeros(8, dtype=torch.int64, device=dev)
+
+    def frame(arm):
         """Renderer.render (density_cube + marching cubes + copies) step by step, events between the steps."""
+        cfg.density_precision = arm
+        if getattr(net, "_density_renderer", None) is not None:
+            net._density_renderer.stats = stats
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(7)]
         with torch.no_grad():
             ev[0].record()
@@ -91,13 +105,41 @@ def main():
         return ev, int(wpts.shape[1]), mesh, cube_host
 
     for _ in range(args.warmup):
-        frame()
+        for arm in arms:
+            frame(arm)
     torch.cuda.synchronize(dev)
-    rows = []
+    rows = {arm: [] for arm in arms}
+    arm_stats = {arm: [] for arm in arms}
+    cubes = {}
     for _ in range(args.steps):
-        ev, n_in, mesh, cube_host = frame()
-        torch.cuda.synchronize(dev)
-        rows.append([ev[i].elapsed_time(ev[i + 1]) for i in range(6)])
+        for arm in arms:
+            stats.zero_()
+            ev, n_in, mesh, cube_host = frame(arm)
+            torch.cuda.synchronize(dev)
+            rows[arm].append([ev[i].elapsed_time(ev[i + 1]) for i in range(6)])
+            arm_stats[arm].append([int(v) for v in stats.tolist()])
+            cubes[arm] = cube_host
+    density = {}
+    for arm in arms:
+        ms = float(np.median([r[1] for r in rows[arm]]))
+        d = {"density_ms_median": ms, "density_ms_all": [r[1] for r in rows[arm]]}
+        st = arm_stats[arm][-1]
+        if arm == "fp32":
+            d["tflops_fp32_kernel"] = FLOP_PER_POINT_DENSITY * n_in / (ms * 1e-3) / 1e12
+        else:
+            listed = st[1]
+            l0 = st[4] / max(1, st[0])                       # layer-0 K-steps per executed tile (22 = all of fc_0)
+            flop_pt = FLOP_PER_POINT_DENSITY - (22.0 - l0) * FLOP_L0_PER_KSTEP
+            d.update({"points": n_in, "listed": listed, "skipped": n_in - listed, "evaluated_fraction": listed / max(1, n_in),
+                      "layer0_ksteps_per_tile": l0, "flop_per_evaluated_point": flop_pt,
+                      "decoder_kernel_ms": st[2] * 1e-6 / max(1, st[3]),
+                      "tflops_evaluated_points": listed * flop_pt / (ms * 1e-3) / 1e12})
+        density[arm] = d
+    if args.ab:
+        density["max_abs_cube_diff_vs_fp32"] = float(np.abs(cubes["tc_fp16x3"] - cubes["fp32"]).max())
+    arm = arms[-1]                                         # the split, the public call and the mesh below: the last arm
+    cfg.density_precision = arm
+    rows = rows[arm]
     # the public call, whole (cube copy included); it must give the same result as the split steps
     t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
@@ -133,9 +175,11 @@ def main():
         "split_ms_median": split, "render_ms_excl_cube_copy": excl_cube, "render_call_ms": render_ms,
         "density": {"flop_per_point": FLOP_PER_POINT_DENSITY, "tflops": dens_tflops,
                     "fraction_of_fp32_datasheet": dens_tflops / FP32_TFLOPS_DATASHEET,
-                    "datasheet": "67 TFLOP/s dense FP32, H100 SXM at 700 W (not a reached figure)"},
+                    "datasheet": "67 TFLOP/s dense FP32, H100 SXM at 700 W (not a reached figure)"} if arm == "fp32" else
+                   {"see": "density_arms"},
         "marching_cubes": {"bytes_as_written": mc_bytes, "gbs": mc_gbs, "fraction_of_hbm_datasheet": mc_gbs / (HBM_TBS_DATASHEET * 1e3),
                            "note": "includes the one host sync between count and emit and the launch gaps"},
+        "density_precision": arm, "density_arms": density,
         "card": card_info(dev),
     }
     print(json.dumps(line))
