@@ -2,7 +2,7 @@
 // once-per-frame pack kernels (volume re-layout, decoder-weight fold + re-layout).
 #include <stdarg.h>
 #include <stdio.h>
-#include "nb_internal.h"
+#include "nb_device.cuh"
 #include "nb_train.h"
 
 namespace nb {
@@ -113,9 +113,7 @@ __global__ void fold_T_kernel(nb_decoder_weights w, double* __restrict__ T, doub
     } else if (idx < kColor * kHidden + w.batch * kHidden) {
         const int r = idx - kColor * kHidden;
         const int b = r / kHidden, j = r % kHidden;
-        long long li = w.latent_index[b];
-        if (li < 0) li = 0;
-        if (li >= w.num_train_frame) li = w.num_train_frame - 1;
+        const long long li = clamp_latent(w.latent_index[b], w.num_train_frame);
         double acc = (double)w.latent_b[j];
         for (int i = 0; i < 128; ++i) acc += (double)w.latent_w[j * 384 + 256 + i] * (double)w.latent[li * 128 + i];
         u[r] = acc;
@@ -210,7 +208,7 @@ __device__ __forceinline__ bool gen_ray(const nb_camera& cam, int pix, float (&o
     for (int a = 0; a < 3; ++a) d[a] = pw[a] - o[a];
     // the dataset casts to float32 BEFORE get_near_far (multi_view_demo_dataset.py / image_rays: ray_o.astype(np.float32))
     for (int a = 0; a < 3; ++a) { of[a] = (float)o[a]; df[a] = (float)d[a]; }
-    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(df[0], df[0]), __fmul_rn(df[1], df[1])), __fmul_rn(df[2], df[2])));
+    const float nrm = ray_norm(df[0], df[1], df[2]);
     float tnear = -INFINITY, tfar = INFINITY;
     for (int a = 0; a < 3; ++a) {
         float v = __fdiv_rn(df[a], nrm);
@@ -451,7 +449,7 @@ int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out) {
     p.batch = a->batch; p.n_rays = a->n_rays; p.n_samples = a->n_samples;
     p.ray_o = a->ray_o; p.ray_d = a->ray_d; p.near = a->near; p.far = a->far; p.t_vals = a->t_vals; p.t_rand = a->t_rand; p.z_user = a->z_vals;
     p.R = a->R; p.Th = a->Th; p.bounds = a->bounds;
-    for (int i = 0; i < 3; ++i) { p.voxel_size[i] = a->voxel_size[i]; p.inv_voxel[i] = 1.f / a->voxel_size[i]; p.out_sh[i] = (float)a->out_sh[i]; }
+    for (int i = 0; i < 3; ++i) { p.voxel_size[i] = a->voxel_size[i]; p.out_sh[i] = (float)a->out_sh[i]; }
     for (int l = 0; l < NB_NUM_LEVELS; ++l) {
         p.lvl_C[l] = a->level_dims[l][0]; p.lvl_D[l] = a->level_dims[l][1]; p.lvl_H[l] = a->level_dims[l][2]; p.lvl_W[l] = a->level_dims[l][3];
         p.lvl_off[l] = nb_packed_volume_level_offset(a->level_dims, a->batch, a->volume_dtype, l);

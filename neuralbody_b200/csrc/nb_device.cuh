@@ -1,6 +1,6 @@
-// Device helpers shared by the exact-fp32 and the tensor-core render kernels:
-// sample generation, world->SMPL->grid transform, trilinear corner set-up,
-// positional encoding and the alpha-compositing warp scan.
+// Device helpers shared by the exact-fp32, the tensor-core and the training kernels:
+// sample generation, the ray norm, world->SMPL->grid transform, trilinear corner set-up and gather,
+// positional encoding, the alpha-compositing warp scan and the per-ray map stores.
 //
 // Parity-critical arithmetic follows the reference's op sequence in fp32 with
 // explicit round-to-nearest intrinsics (no FMA contraction) where upstream issues
@@ -48,6 +48,11 @@ __device__ __forceinline__ float z_sample(float near, float far, const float* __
     return z;
 }
 
+// torch.norm(ray_d, dim=-1): sqrt(x^2 + y^2 + z^2), summed left to right without contraction
+__device__ __forceinline__ float ray_norm(float x, float y, float z) {
+    return sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
+}
+
 // Per-frame constants of the world -> grid transform, staged once per CTA work item.
 struct FrameXf {
     float R[9];        // sp_input['R'][b]   row-major
@@ -56,6 +61,18 @@ struct FrameXf {
     float voxel[3];    // cfg.voxel_size (dhw)
     float out_sh[3];   // dhw
 };
+
+// Element i of each FrameXf array of frame b: threads 0..8 of a CTA fill a shared FrameXf with i = tid; a thread that needs
+// its own copy calls it for i = 0..8.
+__device__ __forceinline__ void load_frame_xf(const RenderParams& P, int b, FrameXf& xf, int i) {
+    if (i < 9) xf.R[i] = __ldg(P.R + b * 9 + i);
+    if (i < 3) {
+        xf.Th[i] = __ldg(P.Th + b * 3 + i);
+        xf.min_dhw[i] = __ldg(P.bounds + b * 6 + (2 - i));
+        xf.voxel[i] = P.voxel_size[i];
+        xf.out_sh[i] = P.out_sh[i];
+    }
+}
 
 // a5 + a6: latent_xyzc.py:41-60.  Input world point, output grid coords (x,y,z) in [-1,1].
 __device__ __forceinline__ void world_to_grid(const FrameXf& f, float wx, float wy, float wz, float& gx, float& gy,
@@ -93,12 +110,60 @@ __device__ __forceinline__ void corner_setup(float ix, float iy, float iz, int W
     c.wy[0] = __fsub_rn(__fadd_rn(fy, 1.f), iy); c.wy[1] = __fsub_rn(iy, fy);
     c.wz[0] = __fsub_rn(__fadd_rn(fz, 1.f), iz); c.wz[1] = __fsub_rn(iz, fz);
 }
-__device__ __forceinline__ bool corner_valid(const Corners& c, int dx, int dy, int dz, int W, int H, int D) {
-    int x = c.x0 + dx, y = c.y0 + dy, z = c.z0 + dz;
-    return (c.x0 != -2) && x >= 0 && x < W && y >= 0 && y < H && z >= 0 && z < D;
+// f(voxel index, weight) for the corners of the cell that lie inside the W x H x D volume, in ATen's accumulation order:
+// tnw, tne, tsw, tse, bnw, bne, bsw, bse (x fastest)
+template <typename F>
+__device__ __forceinline__ void for_each_corner(const Corners& c, int W, int H, int D, F&& f) {
+#pragma unroll
+    for (int dz = 0; dz < 2; ++dz)
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 2; ++dx) {
+                const int x = c.x0 + dx, y = c.y0 + dy, z = c.z0 + dz;
+                if ((c.x0 != -2) && x >= 0 && x < W && y >= 0 && y < H && z >= 0 && z < D)
+                    f(((size_t)z * H + y) * W + x, __fmul_rn(__fmul_rn(c.wx[dx], c.wy[dy]), c.wz[dz]));
+            }
 }
-__device__ __forceinline__ float corner_weight(const Corners& c, int dx, int dy, int dz) {
-    return __fmul_rn(__fmul_rn(c.wx[dx], c.wy[dy]), c.wz[dz]);
+
+// Channel quad q (0..87) of the 352-wide feature, level 0 first (latent_xyzc.py:66-71): its level and first channel there
+__device__ __forceinline__ int level_feature_base(int lvl) { return lvl == 0 ? 0 : lvl == 1 ? 32 : lvl == 2 ? 96 : 224; }
+__device__ __forceinline__ void feature_quad(int q, int& lvl, int& c0) {
+    lvl = q < 8 ? 0 : q < 24 ? 1 : q < 56 ? 2 : 3;
+    c0 = 4 * q - level_feature_base(lvl);
+}
+
+template <typename VT>
+__device__ __forceinline__ float4 load4(const VT* p);
+template <>
+__device__ __forceinline__ float4 load4<float>(const float* p) {
+    return __ldg(reinterpret_cast<const float4*>(p));
+}
+template <>
+__device__ __forceinline__ float4 load4<__half>(const __half* p) {
+    uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+    float2 a = __half22float2(*reinterpret_cast<__half2*>(&u.x));
+    float2 b = __half22float2(*reinterpret_cast<__half2*>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+
+// a7 (latent_xyzc.py:62-72): channel quad q of the trilinear sample (F.grid_sample, align_corners=True, zeros padding) of
+// frame b's volumes at grid coordinates (gx, gy, gz) in [-1, 1]
+template <typename VT>
+__device__ __forceinline__ float4 gather_quad(const RenderParams& P, int b, float gx, float gy, float gz, int q) {
+    int lvl, c0;
+    feature_quad(q, lvl, c0);
+    const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+    Corners cn;
+    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+    const VT* vol = reinterpret_cast<const VT*>(reinterpret_cast<const char*>(P.volume) + P.lvl_off[lvl]) + (size_t)b * P.lvl_bstride[lvl];
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for_each_corner(cn, W, H, D, [&](size_t vox, float wgt) {
+        const float4 v = load4<VT>(vol + vox * C + c0);
+        acc.x = fmaf(v.x, wgt, acc.x); acc.y = fmaf(v.y, wgt, acc.y);
+        acc.z = fmaf(v.z, wgt, acc.z); acc.w = fmaf(v.w, wgt, acc.w);
+    });
+    return acc;
 }
 
 // ---------------------------------------------------------------- f-1: if_clight_renderer_mmsk.py:12-45
@@ -237,6 +302,17 @@ __device__ __forceinline__ float disparity(float depth, float acc) {
     float q = __fdiv_rn(depth, acc);
     float m = (q != q) ? q : fmaxf(1e-10f, q);
     return __fdiv_rn(1.f, m);
+}
+
+// the maps of ray ri (frame-major ray index); white_bkgd adds 1 - acc to rgb (nerf_net_utils.py:47-48)
+__device__ __forceinline__ void store_ray_outputs(const RenderParams& P, size_t ri, const RayOut& o) {
+    const float add = P.white_bkgd ? __fsub_rn(1.f, o.acc) : 0.f;
+    P.rgb_map[ri * P.rgb_stride + 0] = o.r + add;
+    P.rgb_map[ri * P.rgb_stride + 1] = o.g + add;
+    P.rgb_map[ri * P.rgb_stride + 2] = o.b + add;
+    P.depth_map[ri * P.map_stride] = o.depth;
+    P.acc_map[ri * P.map_stride] = o.acc;
+    P.disp_map[ri * P.map_stride] = disparity(o.depth, o.acc);
 }
 
 }  // namespace nb

@@ -11,8 +11,14 @@ namespace nb {
 void set_error(const char* fmt, ...);
 
 // Grid-size unit of the persistent / grid-stride kernels: the SM count of the H100 SXM.  (Launches that must match the
-// device's SM count exactly query cudaDevAttrMultiProcessorCount instead.)
+// device's SM count exactly use sm_count() instead.)
 constexpr int kGridSMs = 132;
+inline int sm_count() {
+    int dev = 0, sms = kGridSMs;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+}
 
 // Kernel-side view of one nb_render_fwd call (passed by value as a __grid_constant__).
 struct RenderParams {
@@ -20,7 +26,6 @@ struct RenderParams {
     const float *ray_o, *ray_d, *near, *far, *t_vals, *t_rand;
     const float* z_user;       // (B,n,S) caller-supplied sample depths (nb_render_args.z_vals) or null
     const float *R, *Th, *bounds;
-    float inv_voxel[3];        // not used for parity-critical math (we divide, as upstream does)
     float voxel_size[3];       // dhw
     float out_sh[3];           // dhw, as float (upstream: torch.tensor(out_sh).to(dhw))
     int   lvl_C[4], lvl_D[4], lvl_H[4], lvl_W[4];

@@ -47,6 +47,11 @@ constexpr size_t oWc = oRgbB + 4;                           // [128][256] folded
 constexpr size_t oSigmaEmpty = oWc + (size_t)kColor * kHidden;   // [1] (+3 pad): sigma of an all-zero feature vector
 constexpr size_t kF32Floats = oSigmaEmpty + 4;
 
+// row of the latent table frame b uses: latent_index[b] clamped into [0, num_train_frame)
+__host__ __device__ inline long long clamp_latent(long long li, int num_train_frame) {
+    return li < 0 ? 0 : li >= num_train_frame ? num_train_frame - 1 : li;
+}
+
 // ---- fp16 section: the tensor-core kernel's weight STREAM, in consumption order.
 // One "step" = the B operand of one K=16 MMA: an N x 16 tile in the canonical K-major
 // no-swizzle layout: element (n, kk) at half-offset ((kk/8) * (N/8) + n/8) * 64 + (n%8) * 8 + (kk%8),

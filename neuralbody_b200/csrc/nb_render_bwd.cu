@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdP
     if (ri >= (size_t)P.batch * P.n_rays) return;
     const float near = P.near[ri], far = P.far[ri];
     const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
-    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+    const float nrm = ray_norm(dx, dy, dz);
     const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
     const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
     const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
@@ -193,11 +193,8 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                 const int s = (int)(g % S), b = (int)(ri / P.n_rays);
                 // frame transform (threads of the same frame recompute it; cheap)
                 FrameXf fx;
-                for (int j = 0; j < 9; ++j) fx.R[j] = P.R[b * 9 + j];
-                for (int j = 0; j < 3; ++j) {
-                    fx.Th[j] = P.Th[b * 3 + j]; fx.min_dhw[j] = P.bounds[b * 6 + (2 - j)];
-                    fx.voxel[j] = P.voxel_size[j]; fx.out_sh[j] = P.out_sh[j];
-                }
+#pragma unroll
+                for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
                 const float z = z_sample(P.near[ri], P.far[ri], P.t_vals, s, S, P.t_rand ? P.t_rand + ri * S : nullptr, P.z_user ? P.z_user + ri * S : nullptr);
                 const float wx = __fadd_rn(P.ray_o[ri * 3], __fmul_rn(P.ray_d[ri * 3], z));
                 const float wy = __fadd_rn(P.ray_o[ri * 3 + 1], __fmul_rn(P.ray_d[ri * 3 + 1], z));
@@ -205,21 +202,17 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                 float gx, gy, gz;
                 world_to_grid(fx, wx, wy, wz, gx, gy, gz);
                 const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-                const int cbase = lvl == 0 ? 0 : lvl == 1 ? 32 : lvl == 2 ? 96 : 224;
+                const int cbase = level_feature_base(lvl);
                 Corners cn;
                 corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
                 float* dv = Q.d_vol[lvl] + (size_t)b * C * D * H * W;
                 const size_t cs = (size_t)D * H * W;
-                for (int c8 = 0; c8 < 8; ++c8) {
-                    const int ddx = c8 & 1, ddy = (c8 >> 1) & 1, ddz = c8 >> 2;
-                    if (!corner_valid(cn, ddx, ddy, ddz, W, H, D)) continue;
-                    const float wgt = corner_weight(cn, ddx, ddy, ddz);
-                    const size_t vox = ((size_t)(cn.z0 + ddz) * H + (cn.y0 + ddy)) * W + (cn.x0 + ddx);
+                for_each_corner(cn, W, H, D, [&](size_t vox, float wgt) {
                     for (int c = 0; c < C; ++c) {
                         const float dfv = X[p * LDX + cbase + c];
                         if (dfv != 0.f) atomicAdd(dv + (size_t)c * cs + vox, wgt * dfv);
                     }
-                }
+                });
             }
         }
         __syncthreads();
@@ -289,7 +282,7 @@ __global__ void view_wgrad_kernel(const BwdParams Q, float* __restrict__ d_view_
     __shared__ float pe[kViewPE];
     if (n == 0) {
         const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
-        const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+        const float nrm = ray_norm(dx, dy, dz);
         positional_embed<4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { pe[j] = v; });
     }
     __syncthreads();
@@ -325,8 +318,7 @@ __global__ void unfold_stage1(const Unfold U) {     // T, u, d b_v, d view_fc[:,
         U.T[idx] = acc;
     } else if (idx < kColor * kHidden + B * kHidden) {
         const int r = idx - kColor * kHidden, b = r / kHidden, j = r % kHidden;
-        long long li = U.w.latent_index[b];
-        li = li < 0 ? 0 : (li >= U.w.num_train_frame ? U.w.num_train_frame - 1 : li);
+        const long long li = clamp_latent(U.w.latent_index[b], U.w.num_train_frame);
         float acc = U.w.latent_b[j];
         for (int i = 0; i < 128; ++i) acc = fmaf(U.w.latent_w[j * 384 + 256 + i], U.w.latent[li * 128 + i], acc);
         U.u[r] = acc;
@@ -381,8 +373,7 @@ __global__ void unfold_stage3(const Unfold U) {     // d view_fc[:, :256], d lat
             for (int n = 0; n < kColor; ++n) acc = fmaf(U.w.view_w[n * 346 + j], U.dT[n * kHidden + k], acc);
         } else {                                     // dLl[j][i] = sum_b du[b][j] latent[idx_b][i]
             for (int b = 0; b < B; ++b) {
-                long long li = U.w.latent_index[b];
-                li = li < 0 ? 0 : (li >= U.w.num_train_frame ? U.w.num_train_frame - 1 : li);
+                const long long li = clamp_latent(U.w.latent_index[b], U.w.num_train_frame);
                 acc = fmaf(U.du[b * kHidden + j], U.w.latent[li * 128 + (k - kHidden)], acc);
             }
         }
@@ -394,8 +385,7 @@ __global__ void unfold_stage3(const Unfold U) {     // d view_fc[:, :256], d lat
         NB_G(U.g.latent_b)[j] += acc;
     } else if (idx < kColor * kHidden + kHidden * 384 + kHidden + B * 128) {   // d latent[idx_b][i] += sum_j Ll[j][i] du[b][j]
         const int r = idx - kColor * kHidden - kHidden * 384 - kHidden, b = r / 128, i = r % 128;
-        long long li = U.w.latent_index[b];
-        li = li < 0 ? 0 : (li >= U.w.num_train_frame ? U.w.num_train_frame - 1 : li);
+        const long long li = clamp_latent(U.w.latent_index[b], U.w.num_train_frame);
         float acc = 0.f;
         for (int j = 0; j < kHidden; ++j) acc = fmaf(U.w.latent_w[j * 384 + 256 + i], U.du[b * kHidden + j], acc);
         atomicAdd(NB_G(U.g.latent) + li * 128 + i, acc);

@@ -118,57 +118,26 @@ __device__ __forceinline__ void mlp_layer(const float* __restrict__ Xs, float* _
     __syncthreads();
 }
 
-template <typename VT>
-__device__ __forceinline__ float4 load4(const VT* p);
-template <>
-__device__ __forceinline__ float4 load4<float>(const float* p) {
-    return __ldg(reinterpret_cast<const float4*>(p));
-}
-template <>
-__device__ __forceinline__ float4 load4<__half>(const __half* p) {
-    uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-    float2 a = __half22float2(*reinterpret_cast<__half2*>(&u.x));
-    float2 b = __half22float2(*reinterpret_cast<__half2*>(&u.y));
-    return make_float4(a.x, a.y, b.x, b.y);
-}
-
-// Trilinear gather of one 64-point tile (a7, latent_xyzc.py:62-72): work item = (point, level, channel quad);
-// lanes run over the quads of one corner => contiguous 16-byte loads.  gcoord = [64][3] grid coords, X = [64][LDX].
+// Trilinear gather of one 64-point tile: work item = (point, channel quad); lanes run over the quads of one corner => contiguous
+// 16-byte loads.  gcoord = [64][3] grid coords, X = [64][LDX].
 template <typename VT>
 __device__ __forceinline__ void gather_tile(const RenderParams& P, int b, const float* __restrict__ gcoord, float* __restrict__ X) {
-    const int tid = threadIdx.x;
     constexpr int QUADS = kFeat / 4;   // 88 per point
-    for (int item = tid; item < TP * QUADS; item += NT) {
+    for (int item = threadIdx.x; item < TP * QUADS; item += NT) {
         const int p = item / QUADS, q = item % QUADS;
-        int lvl, c0;   // channel offset inside the level
-        if (q < 8) { lvl = 0; c0 = q * 4; }
-        else if (q < 24) { lvl = 1; c0 = (q - 8) * 4; }
-        else if (q < 56) { lvl = 2; c0 = (q - 24) * 4; }
-        else { lvl = 3; c0 = (q - 56) * 4; }
-        const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-        Corners cn;
-        corner_setup(unnormalize(gcoord[p * 3 + 0], W), unnormalize(gcoord[p * 3 + 1], H),
-                     unnormalize(gcoord[p * 3 + 2], D), W, H, D, cn);
-        const VT* vol = reinterpret_cast<const VT*>(reinterpret_cast<const char*>(P.volume) + P.lvl_off[lvl]) +
-                        (size_t)b * P.lvl_bstride[lvl];
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-        // ATen accumulation order: tnw, tne, tsw, tse, bnw, bne, bsw, bse  (x fastest)
-#pragma unroll
-        for (int dz = 0; dz < 2; ++dz)
-#pragma unroll
-            for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-                for (int dx = 0; dx < 2; ++dx) {
-                    if (corner_valid(cn, dx, dy, dz, W, H, D)) {
-                        const float wgt = corner_weight(cn, dx, dy, dz);
-                        const size_t vox = ((size_t)(cn.z0 + dz) * H + (cn.y0 + dy)) * W + (cn.x0 + dx);
-                        const float4 v = load4<VT>(vol + vox * C + c0);
-                        acc.x = fmaf(v.x, wgt, acc.x); acc.y = fmaf(v.y, wgt, acc.y);
-                        acc.z = fmaf(v.z, wgt, acc.z); acc.w = fmaf(v.w, wgt, acc.w);
-                    }
-                }
-        *reinterpret_cast<float4*>(X + p * LDX + q * 4) = acc;
+        *reinterpret_cast<float4*>(X + p * LDX + q * 4) = gather_quad<VT>(P, b, gcoord[p * 3 + 0], gcoord[p * 3 + 1], gcoord[p * 3 + 2], q);
     }
+}
+
+// sigma = alpha_fc h2 of tile point tid / 4, h2 = its row of Y: four threads per point, each over every fourth channel
+__device__ __forceinline__ float alpha_head(const float* __restrict__ Y, const float* __restrict__ wf, int tid) {
+    const int p = tid >> 2, q = tid & 3;
+    float acc = 0.f;
+#pragma unroll 8
+    for (int k = q; k < kHidden; k += 4) acc = fmaf(Y[p * LDY + k], __ldg(wf + oAlphaW + k), acc);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+    return acc + __ldg(wf + oAlphaB);
 }
 
 struct RayInfo {
@@ -201,21 +170,14 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
         const int nr = min(G, P.n_rays - r0);
 
         // ---- per-frame transform + per-ray set-up
-        if (tid < 9) xf.R[tid] = __ldg(P.R + b * 9 + tid);
-        if (tid < 3) {
-            xf.Th[tid] = __ldg(P.Th + b * 3 + tid);
-            xf.min_dhw[tid] = __ldg(P.bounds + b * 6 + (2 - tid));
-            xf.voxel[tid] = P.voxel_size[tid];
-            xf.out_sh[tid] = P.out_sh[tid];
-        }
+        load_frame_xf(P, b, xf, tid);
         if (tid < nr) {
             const size_t ri = (size_t)b * P.n_rays + r0 + tid;
             RayInfo& r = rays[tid];
 #pragma unroll
             for (int j = 0; j < 3; ++j) { r.o[j] = __ldg(P.ray_o + ri * 3 + j); r.d[j] = __ldg(P.ray_d + ri * 3 + j); }
             r.near = __ldg(P.near + ri); r.far = __ldg(P.far + ri);
-            // torch.norm(ray_d, dim=2): sqrt(x^2 + y^2 + z^2)
-            r.norm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(r.d[0], r.d[0]), __fmul_rn(r.d[1], r.d[1])), __fmul_rn(r.d[2], r.d[2])));
+            r.norm = ray_norm(r.d[0], r.d[1], r.d[2]);
 #pragma unroll
             for (int j = 0; j < 3; ++j) r.vd[j] = __fdiv_rn(r.d[j], r.norm);   // if_clight_renderer.py:68
         }
@@ -289,17 +251,10 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
             save_rows(X, LDX, kHidden, kSaveH1);
             mlp_layer<kHidden, kHidden, LDX, LDY, true, false>(X, Y, wf + oW2t, wf + oB2, Ws, nullptr, nullptr);
             save_rows(Y, LDY, kColorK, kSaveH2);
-            {   // sigma = alpha_fc h2: 4 threads per point
-                const int p = tid >> 2, q = tid & 3;
-                float acc = 0.f;
-#pragma unroll 8
-                for (int k = q; k < kHidden; k += 4) acc = fmaf(Y[p * LDY + k], __ldg(wf + oAlphaW + k), acc);
-                acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-                acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-                if (q == 0 && pray[p] >= 0) {
-                    const int pgidx = tile * TP + p;
-                    reinterpret_cast<float*>(rawbuf + pgidx)[3] = acc + __ldg(wf + oAlphaB);
-                }
+            {
+                const int p = tid >> 2;
+                const float sigma = alpha_head(Y, wf, tid);
+                if ((tid & 3) == 0 && pray[p] >= 0) reinterpret_cast<float*>(rawbuf + tile * TP + p)[3] = sigma;
             }
             // w = relu(Wc h2 + Wx PE(xyz) + bc + vt[ray]); padding rows borrow ray 0's view term (discarded)
             __syncthreads();
@@ -340,15 +295,7 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
                 float4* rdst = reinterpret_cast<float4*>(P.raw) + ri * S;
                 for (int s = lane; s < S; s += 32) rdst[s] = rawbuf[ry * S + s];
             }
-            if (lane == 0) {
-                float add = P.white_bkgd ? __fsub_rn(1.f, o.acc) : 0.f;
-                P.rgb_map[ri * P.rgb_stride + 0] = o.r + add;
-                P.rgb_map[ri * P.rgb_stride + 1] = o.g + add;
-                P.rgb_map[ri * P.rgb_stride + 2] = o.b + add;
-                P.depth_map[ri * P.map_stride] = o.depth;
-                P.acc_map[ri * P.map_stride] = o.acc;
-                P.disp_map[ri * P.map_stride] = disparity(o.depth, o.acc);
-            }
+            if (lane == 0) store_ray_outputs(P, ri, o);
         }
         __syncthreads();
     }
@@ -370,13 +317,7 @@ __global__ void __launch_bounds__(NT, 1) density_f32_kernel(const __grid_constan
     const int tiles_per_frame = (n_points + TP - 1) / TP;
     for (int t = blockIdx.x; t < tiles_per_frame * P.batch; t += gridDim.x) {
         const int b = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TP;
-        if (tid < 9) xf.R[tid] = __ldg(P.R + b * 9 + tid);
-        if (tid < 3) {
-            xf.Th[tid] = __ldg(P.Th + b * 3 + tid);
-            xf.min_dhw[tid] = __ldg(P.bounds + b * 6 + (2 - tid));
-            xf.voxel[tid] = P.voxel_size[tid];
-            xf.out_sh[tid] = P.out_sh[tid];
-        }
+        load_frame_xf(P, b, xf, tid);
         __syncthreads();
         if (tid < TP) {
             float gx = -4.f, gy = -4.f, gz = -4.f;
@@ -393,13 +334,9 @@ __global__ void __launch_bounds__(NT, 1) density_f32_kernel(const __grid_constan
         mlp_layer<kHidden, kHidden, LDY, LDX, true, false>(Y, X, wf + oW1t, wf + oB1, Ws, nullptr, nullptr);
         mlp_layer<kHidden, kHidden, LDX, LDY, true, false>(X, Y, wf + oW2t, wf + oB2, Ws, nullptr, nullptr);
         {
-            const int p = tid >> 2, q = tid & 3;
-            float acc = 0.f;
-#pragma unroll 8
-            for (int k = q; k < kHidden; k += 4) acc = fmaf(Y[p * LDY + k], __ldg(wf + oAlphaW + k), acc);
-            acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-            acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-            if (q == 0 && p0 + p < n_points) sigma[(size_t)b * n_points + p0 + p] = acc + __ldg(wf + oAlphaB);
+            const int p = tid >> 2;
+            const float sg = alpha_head(Y, wf, tid);
+            if ((tid & 3) == 0 && p0 + p < n_points) sigma[(size_t)b * n_points + p0 + p] = sg;
         }
         __syncthreads();
     }
@@ -413,6 +350,23 @@ size_t smem_bytes(int G, int S) {
 
 }  // namespace f32
 
+// kernel<float> or kernel<__half> by the volume dtype: a persistent grid of min(work items, SMs) CTAs of NT threads with smem
+// bytes of dynamic shared memory
+template <typename Kernel, typename... Args>
+static int launch_by_dtype(const char* name, Kernel k32, Kernel k16, int volume_dtype, int work, size_t smem, cudaStream_t stream,
+                           Args... args) {
+    if (work == 0) return NB_OK;
+    const int sms = sm_count(), grid = work < sms ? work : sms;
+    const Kernel kernel = volume_dtype == NB_DTYPE_F32 ? k32 : k16;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) {
+        kernel<<<grid, f32::NT, smem, stream>>>(args...);
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) { set_error("%s launch failed: %s", name, cudaGetErrorString(e)); return NB_ERR_CUDA; }
+    return NB_OK;
+}
+
 int launch_render_f32(const RenderParams& p_in, int volume_dtype, cudaStream_t stream) {
     RenderParams p = p_in;
     const int S = p.n_samples;
@@ -422,43 +376,15 @@ int launch_render_f32(const RenderParams& p_in, int volume_dtype, cudaStream_t s
     p.n_groups = p.groups_per_frame * p.batch;
     const size_t smem = f32::smem_bytes(p.rays_per_group, S);
     if (smem > 227 * 1024) { set_error("n_samples=%d needs %zu B of shared memory (> 227 KB)", S, smem); return NB_ERR_UNSUPPORTED; }
-    int dev = 0, sms = kGridSMs;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int grid = p.n_groups < sms ? p.n_groups : sms;
-    if (grid == 0) return NB_OK;
-    cudaError_t e;
-    if (volume_dtype == NB_DTYPE_F32) {
-        e = cudaFuncSetAttribute(f32::render_f32_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) f32::render_f32_kernel<float><<<grid, f32::NT, smem, stream>>>(p);
-    } else {
-        e = cudaFuncSetAttribute(f32::render_f32_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) f32::render_f32_kernel<__half><<<grid, f32::NT, smem, stream>>>(p);
-    }
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("render_f32 launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    return NB_OK;
+    return launch_by_dtype("render_f32", f32::render_f32_kernel<float>, f32::render_f32_kernel<__half>, volume_dtype,
+                           p.n_groups, smem, stream, p);
 }
 
 int launch_density_f32(const RenderParams& p, int volume_dtype, const float* pts, int n_points, float* sigma, cudaStream_t stream) {
     const size_t smem = ((size_t)f32::TP * f32::LDX + (size_t)f32::TP * f32::LDY + 2 * f32::KC * 256 + f32::TP * 3) * 4;
-    int dev = 0, sms = kGridSMs;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int tiles = ((n_points + f32::TP - 1) / f32::TP) * p.batch;
-    if (tiles == 0) return NB_OK;
-    const int grid = tiles < sms ? tiles : sms;
-    cudaError_t e;
-    if (volume_dtype == NB_DTYPE_F32) {
-        e = cudaFuncSetAttribute(f32::density_f32_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) f32::density_f32_kernel<float><<<grid, f32::NT, smem, stream>>>(p, pts, n_points, sigma);
-    } else {
-        e = cudaFuncSetAttribute(f32::density_f32_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) f32::density_f32_kernel<__half><<<grid, f32::NT, smem, stream>>>(p, pts, n_points, sigma);
-    }
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("density_f32 launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    return NB_OK;
+    return launch_by_dtype("density_f32", f32::density_f32_kernel<float>, f32::density_f32_kernel<__half>, volume_dtype,
+                           tiles, smem, stream, p, pts, n_points, sigma);
 }
 
 }  // namespace nb

@@ -42,37 +42,82 @@ __device__ __forceinline__ unsigned long long global_ns() {
     return t;
 }
 
-__device__ __forceinline__ void load_frame_xf(const RenderParams& P, FrameXf* xf, int i) {
-    const int b = P.frame;
-    if (i < 9) xf->R[i] = __ldg(P.R + b * 9 + i);
-    if (i < 3) {
-        xf->Th[i] = __ldg(P.Th + b * 3 + i);
-        xf->min_dhw[i] = __ldg(P.bounds + b * 6 + (2 - i));
-        xf->voxel[i] = P.voxel_size[i];
-        xf->out_sh[i] = P.out_sh[i];
+// ------------------------------------------------------------------------------------------------ 1. classify + compact
+constexpr int CLS_THREADS = 256;
+
+// bit l = the level-l trilinear cell at grid coordinates (gx, gy, gz) holds a non-zero voxel of frame b.  A cell with no
+// corner inside the volume (outside the box, where grid_sample pads with zeros) holds none.
+__device__ __forceinline__ uint32_t occupied_levels(const RenderParams& P, int b, float gx, float gy, float gz) {
+    const uint32_t* occ_base = reinterpret_cast<const uint32_t*>(P.volume);
+    uint32_t lm = 0;
+#pragma unroll
+    for (int lvl = 0; lvl < 4; ++lvl) {
+        const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+        Corners cn;
+        corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+        if (cn.x0 != -2 && cn.x0 < W && cn.y0 < H && cn.z0 < D) {
+            const uint32_t* cellbits = occ_base + P.occ_off[lvl] / 4 + (size_t)b * P.occ_bstride[lvl];
+            const uint32_t cell = ((uint32_t)(cn.z0 + 1) * (H + 1) + (cn.y0 + 1)) * (W + 1) + (cn.x0 + 1);
+            lm |= ((__ldg(cellbits + (cell >> 5)) >> (cell & 31)) & 1u) << lvl;
+        }
     }
+    return lm;
 }
 
-// ------------------------------------------------------------------------------------------------ 1. classify + compact
-// One CTA per block of rays_per_group rays (<= 1024 samples), CLS_PER_THREAD samples per thread, SAMPLE-major inside the
-// block so that consecutive list entries are the same depth sample of neighbouring rays (they share their corner lines).
-// 256-thread CTAs: eight of them are resident per SM, which hides the one atomicAdd round trip each block waits for.
-constexpr int CLS_THREADS = 256, CLS_PER_THREAD = MAXS / CLS_THREADS;
-__global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __grid_constant__ RenderParams P) {
-    __shared__ FrameXf xf;
-    __shared__ int wcnt[4][MAXS / 32];
+// Appends a CLS_THREADS block's entries to the lists of their class.  Thread tid holds N entries e[k] of class cls[k] (0..3,
+// -1 = not listed); entry k of thread tid is entry k * CLS_THREADS + tid of the block, and each class keeps that order.
+// The classes are counted with ballots and reserved with one atomicAdd per class and block, so a block's entries of a class
+// stay contiguous.  Classes 3 / 1 grow upwards from the start of list_a / list_b, classes 2 / 0 downwards from their end.
+template <int N>
+__device__ __forceinline__ void append_to_lists(const RenderParams& P, const float4 (&e)[N], const int (&cls)[N]) {
+    constexpr int WARPS = CLS_THREADS / 32;
+    __shared__ int wcnt[4][N * WARPS];
     __shared__ unsigned int sbase[4];
     __shared__ int stotal[4];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const uint32_t bal = __ballot_sync(0xffffffffu, cls[k] == c);
+            if (lane == 0) wcnt[c][k * WARPS + warp] = __popc(bal);
+        }
+    __syncthreads();
+    if (tid < 4) {
+        int total = 0;
+        for (int w = 0; w < N * WARPS; ++w) total += wcnt[tid][w];
+        stotal[tid] = total;
+        sbase[tid] = total ? atomicAdd(P.list_count + tid, (unsigned int)total) : 0u;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        const int slot = k * WARPS + warp, c = cls[k];
+        const uint32_t same = __match_any_sync(0xffffffffu, c);
+        if (c >= 0) {
+            int local = __popc(same & ((1u << lane) - 1));
+            for (int w = 0; w < slot; ++w) local += wcnt[c][w];
+            float4* buf = c >= 2 ? P.list_a : P.list_b;
+            const size_t at = (c & 1) ? (size_t)sbase[c] + local : P.list_cap - (size_t)sbase[c] - stotal[c] + local;
+            buf[at] = e[k];
+        }
+    }
+}
+
+// One CTA per block of rays_per_group rays (<= 1024 samples), CLS_PER_THREAD samples per thread, SAMPLE-major inside the
+// block so that consecutive list entries are the same depth sample of neighbouring rays (they share their corner lines).
+// 256-thread CTAs: eight of them are resident per SM, which hides the one atomicAdd round trip each block waits for.
+constexpr int CLS_PER_THREAD = MAXS / CLS_THREADS;
+__global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __grid_constant__ RenderParams P) {
+    __shared__ FrameXf xf;
+    const int tid = threadIdx.x;
     const int S = P.n_samples, b = P.frame;
     const int r0 = blockIdx.x * P.rays_per_group;
     const int nr = min(P.rays_per_group, P.n_rays - r0);
-    load_frame_xf(P, &xf, tid);
+    load_frame_xf(P, b, xf, tid);
     __syncthreads();
-    const float sigma_empty = __ldg(P.wf32 + oSigmaEmpty);
     // robustly negative sigma on all-zero features => such a sample has compositing weight exactly 0 and is not evaluated
-    const bool can_skip = P.skip_empty && sigma_empty < -1e-3f;
-    const uint32_t* occ_base = reinterpret_cast<const uint32_t*>(P.volume);
+    const bool can_skip = P.skip_empty && __ldg(P.wf32 + oSigmaEmpty) < -1e-3f;
     const uint32_t id0 = P.train_list ? (uint32_t)b * (uint32_t)P.n_rays * (uint32_t)S : 0u;   // training lists span the batch
 
     float4 gm[CLS_PER_THREAD];
@@ -95,75 +140,17 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
             gm[k].z = __fadd_rn(oz, __fmul_rn(dz, z));
             float gx, gy, gz;
             world_to_grid(xf, gm[k].x, gm[k].y, gm[k].z, gx, gy, gz);
-            uint32_t lm = 0;                           // bit l = the sample's level-l cell holds a non-zero voxel
             const bool inside = P.mask_nv == 0 || inside_masks(P, xf, gm[k].x, gm[k].y, gm[k].z);   // f-1 mask views
-            if (inside) {
-#pragma unroll
-                for (int lvl = 0; lvl < 4; ++lvl) {
-                    const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-                    Corners cn;
-                    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
-                    if (cn.x0 != -2) {
-                        const uint32_t* cellbits = occ_base + P.occ_off[lvl] / 4 + (size_t)b * P.occ_bstride[lvl];
-                        const uint32_t cell = ((uint32_t)(cn.z0 + 1) * (H + 1) + (cn.y0 + 1)) * (W + 1) + (cn.x0 + 1);
-                        lm |= ((__ldg(cellbits + (cell >> 5)) >> (cell & 31)) & 1u) << lvl;
-                    }
-                }
-            }
+            const uint32_t lm = inside ? occupied_levels(P, b, gx, gy, gz) : 0u;
             if (inside && (lm != 0u || !can_skip)) cls[k] = (lm && !P.train_list) ? __ffs((int)lm) - 1 : 3;
             gm[k].w = __uint_as_float(((uint32_t)((r0 + ry) * S + s) + id0) | (lm << 28));
         }
-        const int slot = k * (CLS_THREADS / 32) + warp;
+    }
+    append_to_lists(P, gm, cls);
+    const float4 empty = make_float4(0.f, 0.f, 0.f, fminf(__ldg(P.wf32 + oSigmaEmpty), 0.f));   // skipped sample: weight exactly 0
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const uint32_t bal = __ballot_sync(0xffffffffu, cls[k] == c);
-            if (lane == 0) wcnt[c][slot] = __popc(bal);
-        }
-    }
-    __syncthreads();
-    if (tid < 4) {                                    // one reservation per class: the block's entries of a class stay contiguous
-        int total = 0;
-        for (int w = 0; w < MAXS / 32; ++w) total += wcnt[tid][w];
-        stotal[tid] = total;
-        sbase[tid] = total ? atomicAdd(P.list_count + tid, (unsigned int)total) : 0u;
-    }
-    __syncthreads();
-    const float4 empty = make_float4(0.f, 0.f, 0.f, fminf(sigma_empty, 0.f));   // skipped sample: weight exactly 0
-#pragma unroll
-    for (int k = 0; k < CLS_PER_THREAD; ++k) {
-        const int slot = k * (CLS_THREADS / 32) + warp;     // list order = sample-major order of the block, per class
-        const int c = cls[k];
-        const uint32_t same = __match_any_sync(0xffffffffu, c);
-        if (c >= 0) {
-            int local = __popc(same & ((1u << lane) - 1));
-            for (int w = 0; w < slot; ++w) local += wcnt[c][w];
-            // classes 3 / 1 grow upwards from the start of their buffer, classes 2 / 0 downwards from its end
-            float4* buf = c >= 2 ? P.list_a : P.list_b;
-            const size_t at = (c & 1) ? (size_t)sbase[c] + local : P.list_cap - (size_t)sbase[c] - stotal[c] + local;
-            buf[at] = gm[k];
-        } else if (live[k]) {
-            P.raw_ws[(__float_as_uint(gm[k].w) & ID_MASK) - id0] = empty;
-        }
-    }
-}
-
-// bit l = the level-l trilinear cell at grid coordinates (gx, gy, gz) holds a non-zero voxel of frame b.  A cell with no
-// corner inside the volume (outside the box, where grid_sample pads with zeros) holds none.
-__device__ __forceinline__ uint32_t occupied_levels(const RenderParams& P, int b, float gx, float gy, float gz) {
-    const uint32_t* occ_base = reinterpret_cast<const uint32_t*>(P.volume);
-    uint32_t lm = 0;
-#pragma unroll
-    for (int lvl = 0; lvl < 4; ++lvl) {
-        const int D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-        Corners cn;
-        corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
-        if (cn.x0 != -2 && cn.x0 < W && cn.y0 < H && cn.z0 < D) {
-            const uint32_t* cellbits = occ_base + P.occ_off[lvl] / 4 + (size_t)b * P.occ_bstride[lvl];
-            const uint32_t cell = ((uint32_t)(cn.z0 + 1) * (H + 1) + (cn.y0 + 1)) * (W + 1) + (cn.x0 + 1);
-            lm |= ((__ldg(cellbits + (cell >> 5)) >> (cell & 31)) & 1u) << lvl;
-        }
-    }
-    return lm;
+    for (int k = 0; k < CLS_PER_THREAD; ++k)
+        if (cls[k] < 0 && live[k]) P.raw_ws[(__float_as_uint(gm[k].w) & ID_MASK) - id0] = empty;
 }
 
 // ------------------------------------------------------------------------------------------------ 1'. classify points
@@ -173,48 +160,24 @@ __device__ __forceinline__ uint32_t occupied_levels(const RenderParams& P, int b
 // order inside the block (neighbouring grid points share their corner voxels).  Entry: (world xyz, point id | level bits << 28).
 __global__ void __launch_bounds__(CLS_THREADS) classify_points_kernel(const __grid_constant__ RenderParams P) {
     __shared__ FrameXf xf;
-    __shared__ int wcnt[4][CLS_THREADS / 32];
-    __shared__ unsigned int sbase[4];
-    __shared__ int stotal[4];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int b = P.frame, n = P.n_points;
     const int i = blockIdx.x * CLS_THREADS + tid;
-    load_frame_xf(P, &xf, tid);
+    load_frame_xf(P, b, xf, tid);
     __syncthreads();
-    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
-    int cls = -1;                                     // 0..3 = finest occupied level (list class), -1 = not listed
+    float4 e[1] = {make_float4(0.f, 0.f, 0.f, 0.f)};
+    int cls[1] = {-1};                                // 0..3 = finest occupied level (list class), -1 = not listed
     if (i < n) {
         const float* q = P.points + (size_t)i * 3;
-        e.x = __ldg(q); e.y = __ldg(q + 1); e.z = __ldg(q + 2);
+        e[0].x = __ldg(q); e[0].y = __ldg(q + 1); e[0].z = __ldg(q + 2);
         float gx, gy, gz;
-        world_to_grid(xf, e.x, e.y, e.z, gx, gy, gz);
+        world_to_grid(xf, e[0].x, e[0].y, e[0].z, gx, gy, gz);
         const uint32_t lm = occupied_levels(P, b, gx, gy, gz);
-        if (lm != 0u || !P.skip_empty) cls = lm ? __ffs((int)lm) - 1 : 3;
-        e.w = __uint_as_float((uint32_t)i | (lm << 28));
+        if (lm != 0u || !P.skip_empty) cls[0] = lm ? __ffs((int)lm) - 1 : 3;
+        e[0].w = __uint_as_float((uint32_t)i | (lm << 28));
     }
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        const uint32_t bal = __ballot_sync(0xffffffffu, cls == c);
-        if (lane == 0) wcnt[c][warp] = __popc(bal);
-    }
-    __syncthreads();
-    if (tid < 4) {                                    // one reservation per class and block
-        int total = 0;
-        for (int w = 0; w < CLS_THREADS / 32; ++w) total += wcnt[tid][w];
-        stotal[tid] = total;
-        sbase[tid] = total ? atomicAdd(P.list_count + tid, (unsigned int)total) : 0u;
-    }
-    __syncthreads();
-    const uint32_t same = __match_any_sync(0xffffffffu, cls);
-    if (cls >= 0) {
-        int local = __popc(same & ((1u << lane) - 1));
-        for (int w = 0; w < warp; ++w) local += wcnt[cls][w];
-        float4* buf = cls >= 2 ? P.list_a : P.list_b;          // the buffers and growth directions of classify_compact_kernel
-        const size_t at = (cls & 1) ? (size_t)sbase[cls] + local : P.list_cap - (size_t)sbase[cls] - stotal[cls] + local;
-        buf[at] = e;
-    } else if (i < n) {
-        P.sigma[i] = __ldg(P.wf32 + oSigmaEmpty);
-    }
+    append_to_lists(P, e, cls);
+    if (cls[0] < 0 && i < n) P.sigma[i] = __ldg(P.wf32 + oSigmaEmpty);
 }
 
 // ------------------------------------------------------------------------------------------------ 2. decoder over the list
@@ -356,7 +319,7 @@ __device__ __forceinline__ void decode_list(const RenderParams& P) {
         tc::mbar_init(&bars[B_ROWSFREE], 8);
         tc::fence_mbar_init();
     }
-    load_frame_xf(P, xf, tid);
+    load_frame_xf(P, P.frame, *xf, tid);
     for (int i = tid; i < HEAD_FLOATS; i += NT) {
         float v;
         if (i < H_RGBW) v = __ldg(P.wf32 + oAlphaW + i);                       // [alpha_w | alpha_b]
@@ -588,7 +551,7 @@ __device__ __forceinline__ void decode_list(const RenderParams& P) {
                         const int smp = (int)(__float_as_uint(e.w) & ID_MASK);
                         const size_t ri = (size_t)P.frame * P.n_rays + (prow < nrows ? smp / S : 0);
                         const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
-                        const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+                        const float nrm = ray_norm(dx, dy, dz);
                         positional_embed_anchored<4, 4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { put(64 + j, v); });
                         put(91, 0.f); put(92, 1.f); put(93, 1.f); put(94, 0.f); put(95, 0.f);
                     }
@@ -1039,18 +1002,9 @@ __global__ void __launch_bounds__(COMP_WARPS * 32) composite_kernel(const __grid
     for (int s = lane; s < S; s += 32) zs[warp][s] = z_sample(near, far, P.t_vals, s, S, P.t_rand ? P.t_rand + rg * S : nullptr, P.z_user ? P.z_user + rg * S : nullptr);
     __syncwarp();
     const float dx = __ldg(P.ray_d + rg * 3), dy = __ldg(P.ray_d + rg * 3 + 1), dz = __ldg(P.ray_d + rg * 3 + 2);
-    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
     float* wout = P.weights ? P.weights + rg * S : nullptr;
-    RayOut o = composite_ray(P.raw_ws + (size_t)ray * S, zs[warp], S, nrm, wout, lane);
-    if (lane == 0) {
-        const float add = P.white_bkgd ? __fsub_rn(1.f, o.acc) : 0.f;
-        P.rgb_map[rg * P.rgb_stride + 0] = o.r + add;
-        P.rgb_map[rg * P.rgb_stride + 1] = o.g + add;
-        P.rgb_map[rg * P.rgb_stride + 2] = o.b + add;
-        P.depth_map[rg * P.map_stride] = o.depth;
-        P.acc_map[rg * P.map_stride] = o.acc;
-        P.disp_map[rg * P.map_stride] = disparity(o.depth, o.acc);
-    }
+    RayOut o = composite_ray(P.raw_ws + (size_t)ray * S, zs[warp], S, ray_norm(dx, dy, dz), wout, lane);
+    if (lane == 0) store_ray_outputs(P, rg, o);
 }
 
 template <int NP, typename VT, bool DENSITY>
@@ -1069,9 +1023,7 @@ static cudaError_t launch_decoder(const RenderParams& p, int volume_dtype, int p
 // one persistent CTA per SM; the tile count of a frame is only known on the device, so the grid is sized for the worst case
 // (every entry listed) and tiles past the end are no-ops
 static int decoder_grid(size_t max_entries) {
-    int dev = 0, sms = kGridSMs;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
     const long long max_tiles = ((long long)max_entries + TP - 1) / TP + 4;
     return (int)(max_tiles < sms ? max_tiles : sms);
 }
@@ -1079,13 +1031,29 @@ static int decoder_grid(size_t max_entries) {
 static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 constexpr size_t CTL_BYTES = 32;   // per frame: u32 list counts [4], u64 ~start, u64 end
 
+// A batch's list workspace: one control block per frame, then the two list buffers of cap entries each, which the frames use
+// in turn.  lists_bytes is its size; set_frame_lists points p at frame b's part and returns the end of the list buffers.
+static size_t lists_bytes(int batch, size_t cap) { return align256((size_t)batch * CTL_BYTES) + 2 * align256(cap * sizeof(float4)); }
+static unsigned char* set_frame_lists(RenderParams& p, void* workspace, int b, size_t cap) {
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    unsigned char* list = ws + align256((size_t)p.batch * CTL_BYTES);
+    const size_t per_frame = align256(cap * sizeof(float4));
+    p.frame = b;
+    p.list_a = reinterpret_cast<float4*>(list);
+    p.list_b = reinterpret_cast<float4*>(list + per_frame);
+    p.list_cap = cap;
+    p.list_count = reinterpret_cast<unsigned int*>(ws + (size_t)b * CTL_BYTES);
+    p.frame_clock = reinterpret_cast<unsigned long long*>(ws + (size_t)b * CTL_BYTES + 16);
+    return list + 2 * per_frame;
+}
+
 }  // namespace tcl
 
 bool tc_available() { return true; }
 
 size_t render_tc_list_workspace_bytes(int batch, int n_rays, int n_samples) {
-    const size_t per_frame = (size_t)n_rays * n_samples * sizeof(float4);
-    return tcl::align256((size_t)batch * tcl::CTL_BYTES) + 3 * tcl::align256(per_frame);   // control + 2 list buffers + raw records
+    const size_t cap = (size_t)n_rays * n_samples;
+    return tcl::lists_bytes(batch, cap) + tcl::align256(cap * sizeof(float4));   // + the raw records
 }
 
 bool render_tc_list_supported(const RenderParams& p) {
@@ -1118,31 +1086,18 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
                   render_tc_list_workspace_bytes(p.batch, p.n_rays, S));
         return NB_ERR_BAD_ARG;
     }
-    p.rays_per_group = tcl::MAXS / S;
-    p.tiles_per_group = 0;
-    p.groups_per_frame = (p.n_rays + p.rays_per_group - 1) / p.rays_per_group;
-    p.n_groups = p.groups_per_frame * p.batch;
     if (p.n_rays == 0) return NB_OK;
-    const size_t per_frame = tcl::align256((size_t)p.n_rays * S * sizeof(float4));
-    unsigned char* ws = static_cast<unsigned char*>(workspace);
-    float4* list = reinterpret_cast<float4*>(ws + tcl::align256((size_t)p.batch * tcl::CTL_BYTES));
-    float4* raw_ws = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(list) + 2 * per_frame);
-    cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
     if (e != cudaSuccess) { set_error("render_tc_list: memset failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     const int grid = tcl::decoder_grid((size_t)p.n_rays * S);
     for (int b = 0; b < p.batch; ++b) {
-        p.frame = b;
-        p.list_a = list;
-        p.list_b = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(list) + per_frame);
-        p.list_cap = (size_t)p.n_rays * S;
-        p.list_count = reinterpret_cast<unsigned int*>(ws + (size_t)b * tcl::CTL_BYTES);
-        p.frame_clock = reinterpret_cast<unsigned long long*>(ws + (size_t)b * tcl::CTL_BYTES + 16);
+        float4* raw_ws = reinterpret_cast<float4*>(tcl::set_frame_lists(p, workspace, b, (size_t)p.n_rays * S));
         p.raw_ws = p_in.raw ? reinterpret_cast<float4*>(p_in.raw) + (size_t)b * p.n_rays * S : raw_ws;
-        tcl::classify_compact_kernel<<<p.groups_per_frame, tcl::CLS_THREADS, 0, stream>>>(p);
+        launch_classify(p, stream);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = tcl::launch_decoder<false>(p, volume_dtype, passes, grid, stream);
         if (e == cudaSuccess) {
-            tcl::composite_kernel<<<(p.n_rays + tcl::COMP_WARPS - 1) / tcl::COMP_WARPS, tcl::COMP_WARPS * 32, 0, stream>>>(p);
+            launch_composite(p, stream);
             e = cudaGetLastError();
         }
         if (e != cudaSuccess) { set_error("render_tc_list launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
@@ -1151,7 +1106,7 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
 }
 
 size_t density_tc_list_workspace_bytes(int batch, int n_points) {
-    return tcl::align256((size_t)batch * tcl::CTL_BYTES) + 2 * tcl::align256((size_t)n_points * sizeof(float4));   // control + 2 list buffers
+    return tcl::lists_bytes(batch, (size_t)n_points);
 }
 
 // p.points / p.sigma / p.n_points set by the caller for the whole batch
@@ -1170,19 +1125,11 @@ int launch_density_tc_list(const RenderParams& p_in, int volume_dtype, int passe
                   density_tc_list_workspace_bytes(p.batch, n));
         return NB_ERR_BAD_ARG;
     }
-    const size_t per_frame = tcl::align256((size_t)n * sizeof(float4));
-    unsigned char* ws = static_cast<unsigned char*>(workspace);
-    float4* list = reinterpret_cast<float4*>(ws + tcl::align256((size_t)p.batch * tcl::CTL_BYTES));
-    cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)p.batch * tcl::CTL_BYTES, stream);
     if (e != cudaSuccess) { set_error("density_tc_list: memset failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     const int grid = tcl::decoder_grid((size_t)n);
     for (int b = 0; b < p.batch; ++b) {
-        p.frame = b;
-        p.list_a = list;
-        p.list_b = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(list) + per_frame);
-        p.list_cap = (size_t)n;
-        p.list_count = reinterpret_cast<unsigned int*>(ws + (size_t)b * tcl::CTL_BYTES);
-        p.frame_clock = reinterpret_cast<unsigned long long*>(ws + (size_t)b * tcl::CTL_BYTES + 16);
+        tcl::set_frame_lists(p, workspace, b, (size_t)n);
         p.points = p_in.points + (size_t)b * n * 3;
         p.sigma = p_in.sigma + (size_t)b * n;
         tcl::classify_points_kernel<<<(n + tcl::CLS_THREADS - 1) / tcl::CLS_THREADS, tcl::CLS_THREADS, 0, stream>>>(p);

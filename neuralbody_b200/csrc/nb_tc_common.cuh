@@ -17,11 +17,6 @@ __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
 __device__ __forceinline__ void sts_v2(uint32_t addr, uint2 v) {
     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(v.x), "r"(v.y) : "memory");
 }
-__device__ __forceinline__ float f16lo_of(float x, uint32_t hi_pair, int which) {
-    // x - float(hi) for one element of a packed fp16 pair
-    const __half2 h = *reinterpret_cast<const __half2*>(&hi_pair);
-    return x - (which ? __high2float(h) : __low2float(h));
-}
 
 // Diagnostics: CTA 0 records (code << 48 | clock) per role into P.trace[role * 4096 + n] (first ~40 tiles).
 struct Tracer {
@@ -45,7 +40,6 @@ template <typename VT> struct Quad;
 template <> struct Quad<float> {
     using raw = uint4;
     static __device__ __forceinline__ raw zero() { return make_uint4(0u, 0u, 0u, 0u); }
-    static __device__ __forceinline__ raw load(const float* p) { return ldg_nc_v4(p); }
     static __device__ __forceinline__ raw load_bytes(const unsigned char* p) { return ldg_nc_v4(p); }
     static __device__ __forceinline__ raw load_shared(uint32_t addr) {
         uint4 r;

@@ -64,19 +64,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
-// non-blocking probe of a phase (no hardware suspend): true if the phase with this parity has completed
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-
 // Wait of a THROUGHPUT role (the producers' wait for a free segment buffer).  try_wait's hardware suspend returns after a few
 // tens of cycles, so a plain mbar_wait is a 7-instruction spin: measured (ncu source view) 27 % of ALL warp instructions of
 // the decoder were 16 producer warps spinning here, on the schedulers the epilogue warps need.  Sleeping between probes
@@ -121,8 +108,6 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
     return d;
 }
-// the start-address field of a descriptor advanced by `bytes` (in-range addresses never carry out of the field)
-__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

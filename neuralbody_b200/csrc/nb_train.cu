@@ -291,28 +291,6 @@ __global__ void build_color_kernel(const float* __restrict__ wf, const float* __
     }
 }
 
-template <typename VT>
-__device__ __forceinline__ float4 load4(const VT* p);
-template <>
-__device__ __forceinline__ float4 load4<float>(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-template <>
-__device__ __forceinline__ float4 load4<__half>(const __half* p) {
-    uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-    float2 a = __half22float2(*reinterpret_cast<__half2*>(&u.x));
-    float2 b = __half22float2(*reinterpret_cast<__half2*>(&u.y));
-    return make_float4(a.x, a.y, b.x, b.y);
-}
-
-__device__ __forceinline__ void frame_xf(const RenderParams& P, int b, FrameXf& fx) {
-#pragma unroll
-    for (int j = 0; j < 9; ++j) fx.R[j] = __ldg(P.R + b * 9 + j);
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        fx.Th[j] = __ldg(P.Th + b * 3 + j); fx.min_dhw[j] = __ldg(P.bounds + b * 6 + (2 - j));
-        fx.voxel[j] = P.voxel_size[j]; fx.out_sh[j] = P.out_sh[j];
-    }
-}
-
 // One CTA per 32 list entries: grid coordinates + encodings by one thread per entry, then (entry, channel quad) work items --
 // the 8 lanes of a quad row read one corner as 128 contiguous bytes.  Accumulation order = ATen's (and the exact kernel's).
 constexpr int GP = 32;
@@ -331,7 +309,8 @@ __global__ void __launch_bounds__(256) gather_kernel(const __grid_constant__ Ren
             const int b = id / spf;
             const size_t ri = id / S;
             FrameXf fx;
-            frame_xf(P, b, fx);
+#pragma unroll
+            for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
             float gx, gy, gz;
             world_to_grid(fx, en.x, en.y, en.z, gx, gy, gz);
             gc[tid][0] = gx; gc[tid][1] = gy; gc[tid][2] = gz;
@@ -340,7 +319,7 @@ __global__ void __launch_bounds__(256) gather_kernel(const __grid_constant__ Ren
             positional_embed<10>(en.x, en.y, en.z, [&](int j, float v) { xr[kXyzCol + j] = v; });      // latent_xyzc.py:115
             xr[kXyzCol + kXyzPE] = 0.f;
             const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
-            const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+            const float nrm = ray_norm(dx, dy, dz);
             positional_embed<4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { xr[kViewCol + j] = v; });
 #pragma unroll
             for (int j = kViewCol + kViewPE; j < kH2X; ++j) xr[j] = 0.f;
@@ -350,31 +329,7 @@ __global__ void __launch_bounds__(256) gather_kernel(const __grid_constant__ Ren
         for (int item = tid; item < GP * QUADS; item += 256) {
             const int p = item / QUADS, qd = item % QUADS;
             if (e0 + p >= count) continue;
-            int lvl, c0;
-            if (qd < 8) { lvl = 0; c0 = qd * 4; }
-            else if (qd < 24) { lvl = 1; c0 = (qd - 8) * 4; }
-            else if (qd < 56) { lvl = 2; c0 = (qd - 24) * 4; }
-            else { lvl = 3; c0 = (qd - 56) * 4; }
-            const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
-            Corners cn;
-            corner_setup(unnormalize(gc[p][0], W), unnormalize(gc[p][1], H), unnormalize(gc[p][2], D), W, H, D, cn);
-            const VT* vol = reinterpret_cast<const VT*>(reinterpret_cast<const char*>(P.volume) + P.lvl_off[lvl]) + (size_t)fr[p] * P.lvl_bstride[lvl];
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int dz = 0; dz < 2; ++dz)
-#pragma unroll
-                for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-                    for (int dx = 0; dx < 2; ++dx) {
-                        if (corner_valid(cn, dx, dy, dz, W, H, D)) {
-                            const float wgt = corner_weight(cn, dx, dy, dz);
-                            const size_t vox = ((size_t)(cn.z0 + dz) * H + (cn.y0 + dy)) * W + (cn.x0 + dx);
-                            const float4 v = load4<VT>(vol + vox * C + c0);
-                            acc.x = fmaf(v.x, wgt, acc.x); acc.y = fmaf(v.y, wgt, acc.y);
-                            acc.z = fmaf(v.z, wgt, acc.z); acc.w = fmaf(v.w, wgt, acc.w);
-                        }
-                    }
-            *reinterpret_cast<float4*>(sv.F + (size_t)(e0 + p) * kFeat + qd * 4) = acc;
+            *reinterpret_cast<float4*>(sv.F + (size_t)(e0 + p) * kFeat + qd * 4) = gather_quad<VT>(P, fr[p], gc[p][0], gc[p][1], gc[p][2], qd);
         }
         __syncthreads();
     }
@@ -462,7 +417,8 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
             const float4 en = sv.list[e0 + tid];
             const int b = (__float_as_uint(en.w) & ID_MASK) / spf;
             FrameXf fx;
-            frame_xf(P, b, fx);
+#pragma unroll
+            for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
             float gx, gy, gz;
             world_to_grid(fx, en.x, en.y, en.z, gx, gy, gz);
             gc[tid][0] = gx; gc[tid][1] = gy; gc[tid][2] = gz;
@@ -474,24 +430,16 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
             const int p = item / QUADS, qd = item % QUADS;
             if (e0 + p >= count) continue;
             int lvl, c0;
-            if (qd < 8) { lvl = 0; c0 = qd * 4; }
-            else if (qd < 24) { lvl = 1; c0 = (qd - 8) * 4; }
-            else if (qd < 56) { lvl = 2; c0 = (qd - 24) * 4; }
-            else { lvl = 3; c0 = (qd - 56) * 4; }
+            feature_quad(qd, lvl, c0);
             const float4 g = *reinterpret_cast<const float4*>(DF + (size_t)(e0 + p) * kFeat + qd * 4);
             if (g.x == 0.f && g.y == 0.f && g.z == 0.f && g.w == 0.f) continue;
             const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
             Corners cn;
             corner_setup(unnormalize(gc[p][0], W), unnormalize(gc[p][1], H), unnormalize(gc[p][2], D), W, H, D, cn);
             float* dv = dblob + gb.off[lvl] + (size_t)fr[p] * gb.bstride[lvl];
-#pragma unroll
-            for (int c8 = 0; c8 < 8; ++c8) {
-                const int dx = c8 & 1, dy = (c8 >> 1) & 1, dz = c8 >> 2;
-                if (!corner_valid(cn, dx, dy, dz, W, H, D)) continue;
-                const float wgt = corner_weight(cn, dx, dy, dz);
-                const size_t vox = ((size_t)(cn.z0 + dz) * H + (cn.y0 + dy)) * W + (cn.x0 + dx);
+            for_each_corner(cn, W, H, D, [&](size_t vox, float wgt) {
                 atomicAdd(reinterpret_cast<float4*>(dv + vox * C + c0), make_float4(wgt * g.x, wgt * g.y, wgt * g.z, wgt * g.w));
-            }
+            });
         }
         __syncthreads();
     }
