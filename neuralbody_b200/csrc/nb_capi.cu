@@ -16,8 +16,6 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-static inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
-
 // ------------------------------------------------------------------------------------------
 // Volume pack: (B,C,D,H,W) fp32 -> [B][D][H][W][C] fp32/fp16 through a shared-memory
 // transpose tile so that both the NCDHW reads (along W..DHW) and the channels-last writes
@@ -424,30 +422,31 @@ size_t nb_render_fwd_workspace_bytes(int batch, int n_rays, int n_samples) {
     return render_tc_list_workspace_bytes(batch, n_rays, n_samples);
 }
 
-// validate a forward call's arguments and translate them into the kernels' parameter block (shared with nb_render_bwd)
-int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out) {
-    if (!a) { set_error("nb_render_fwd: null args"); return NB_ERR_BAD_ARG; }
-    if (a->batch <= 0 || a->n_rays < 0 || a->n_samples <= 0) { set_error("nb_render_fwd: bad batch/n_rays/n_samples"); return NB_ERR_BAD_ARG; }
-    if (!a->ray_o || !a->ray_d || !a->near || !a->far || !a->R || !a->Th || !a->bounds || !a->volume_blob || !a->weights_blob ||
-        !a->rgb_map || !a->disp_map || !a->acc_map || !a->depth_map) {
-        set_error("nb_render_fwd: a required device pointer is null");
+}  // extern "C"
+
+namespace nb {
+
+int fill_frame_params(const nb_render_args* a, const char* who, RenderParams* out) {
+    if (!a) { set_error("%s: null args", who); return NB_ERR_BAD_ARG; }
+    if (a->batch <= 0) { set_error("%s: batch must be > 0", who); return NB_ERR_BAD_ARG; }
+    if (!a->R || !a->Th || !a->bounds || !a->volume_blob || !a->weights_blob) {
+        set_error("%s: a frame pointer (R, Th, bounds, volume_blob, weights_blob) is null", who);
         return NB_ERR_BAD_ARG;
     }
-    if (a->volume_dtype != NB_DTYPE_F32 && a->volume_dtype != NB_DTYPE_F16) { set_error("nb_render_fwd: bad volume_dtype"); return NB_ERR_BAD_ARG; }
+    if (a->volume_dtype != NB_DTYPE_F32 && a->volume_dtype != NB_DTYPE_F16) { set_error("%s: bad volume_dtype", who); return NB_ERR_BAD_ARG; }
     static const int expectC[4] = {32, 64, 128, 128};
     for (int l = 0; l < NB_NUM_LEVELS; ++l) {
         if (a->level_dims[l][0] != expectC[l]) {
-            set_error("nb_render_fwd: level %d has %d channels, decoder expects %d (fc_0 is 352-wide)", l, a->level_dims[l][0], expectC[l]);
+            set_error("%s: level %d has %d channels, decoder expects %d (fc_0 is 352-wide)", who, l, a->level_dims[l][0], expectC[l]);
             return NB_ERR_UNSUPPORTED;
         }
-        if (a->level_dims[l][1] <= 0 || a->level_dims[l][2] <= 0 || a->level_dims[l][3] <= 0) { set_error("nb_render_fwd: bad level dims"); return NB_ERR_BAD_ARG; }
+        if (a->level_dims[l][1] <= 0 || a->level_dims[l][2] <= 0 || a->level_dims[l][3] <= 0) { set_error("%s: bad level dims", who); return NB_ERR_BAD_ARG; }
     }
     for (int i = 0; i < 3; ++i)
-        if (!(a->voxel_size[i] > 0.f) || a->out_sh[i] <= 0) { set_error("nb_render_fwd: voxel_size/out_sh must be > 0"); return NB_ERR_BAD_ARG; }
+        if (!(a->voxel_size[i] > 0.f) || a->out_sh[i] <= 0) { set_error("%s: voxel_size/out_sh must be > 0", who); return NB_ERR_BAD_ARG; }
 
-    RenderParams& p = *out;
-    p.batch = a->batch; p.n_rays = a->n_rays; p.n_samples = a->n_samples;
-    p.ray_o = a->ray_o; p.ray_d = a->ray_d; p.near = a->near; p.far = a->far; p.t_vals = a->t_vals; p.t_rand = a->t_rand; p.z_user = a->z_vals;
+    RenderParams p{};
+    p.batch = a->batch;
     p.R = a->R; p.Th = a->Th; p.bounds = a->bounds;
     for (int i = 0; i < 3; ++i) { p.voxel_size[i] = a->voxel_size[i]; p.out_sh[i] = (float)a->out_sh[i]; }
     for (int l = 0; l < NB_NUM_LEVELS; ++l) {
@@ -463,7 +462,26 @@ int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out) {
     p.wf16 = (const __half*)(wb + kF16ByteOffset);
     p.bc = (const float*)(wb + kBcByteOffset);
     p.wframe = (const __half*)(wb + frame_step_byte_offset(a->batch));
-    if (a->out_ray_stride < 0) { set_error("nb_render_fwd: out_ray_stride < 0"); return NB_ERR_BAD_ARG; }
+    *out = p;
+    return NB_OK;
+}
+
+int fill_ray_params(const nb_render_args* a, const char* who, RenderParams* out) {
+    if (a->n_rays < 0 || a->n_samples <= 0) { set_error("%s: bad n_rays/n_samples", who); return NB_ERR_BAD_ARG; }
+    if (!a->ray_o || !a->ray_d || !a->near || !a->far || !a->rgb_map || !a->disp_map || !a->acc_map || !a->depth_map) {
+        set_error("%s: a ray or output-map pointer (ray_o, ray_d, near, far, rgb_map, disp_map, acc_map, depth_map) is null", who);
+        return NB_ERR_BAD_ARG;
+    }
+    if (a->out_ray_stride < 0) { set_error("%s: out_ray_stride < 0", who); return NB_ERR_BAD_ARG; }
+    if (a->mask_msks && (a->mask_R0 != nullptr) != (a->mask_Th0 != nullptr)) { set_error("%s: mask_R0 and mask_Th0 go together", who); return NB_ERR_BAD_ARG; }
+    if (a->mask_msks && (a->batch != 1 || !a->mask_RT || !a->mask_Ks || a->mask_nv <= 0 || a->mask_H <= 0 || a->mask_W <= 0)) {
+        set_error("%s: mask views need batch == 1 (as upstream), RT, Ks and positive nv/H/W", who);
+        return NB_ERR_BAD_ARG;
+    }
+
+    RenderParams& p = *out;
+    p.n_rays = a->n_rays; p.n_samples = a->n_samples;
+    p.ray_o = a->ray_o; p.ray_d = a->ray_d; p.near = a->near; p.far = a->far; p.t_vals = a->t_vals; p.t_rand = a->t_rand; p.z_user = a->z_vals;
     p.rgb_stride = a->out_ray_stride ? a->out_ray_stride : 3;
     p.map_stride = a->out_ray_stride ? a->out_ray_stride : 1;
     p.white_bkgd = a->white_bkgd;
@@ -472,17 +490,12 @@ int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out) {
     p.mask_msks = a->mask_msks; p.mask_RT = a->mask_RT; p.mask_Ks = a->mask_Ks;
     p.mask_nv = a->mask_msks ? a->mask_nv : 0; p.mask_H = a->mask_H; p.mask_W = a->mask_W;
     p.mask_R0 = a->mask_msks ? a->mask_R0 : nullptr; p.mask_Th0 = a->mask_msks ? a->mask_Th0 : nullptr;
-    if ((p.mask_R0 != nullptr) != (p.mask_Th0 != nullptr)) { set_error("nb_render_fwd: mask_R0 and mask_Th0 go together"); return NB_ERR_BAD_ARG; }
-    if (a->mask_msks && (a->batch != 1 || !a->mask_RT || !a->mask_Ks || a->mask_nv <= 0 || a->mask_H <= 0 || a->mask_W <= 0)) {
-        set_error("nb_render_fwd: mask views need batch == 1 (as upstream), RT, Ks and positive nv/H/W");
-        return NB_ERR_BAD_ARG;
-    }
-    p.rays_per_group = p.tiles_per_group = p.n_groups = p.groups_per_frame = 0;
-    p.frame = 0; p.train_list = 0; p.list_a = p.list_b = nullptr; p.list_cap = 0; p.list_count = nullptr; p.frame_clock = nullptr; p.raw_ws = nullptr;
-    p.points = nullptr; p.sigma = nullptr; p.n_points = 0;
-
     return NB_OK;
 }
+
+}  // namespace nb
+
+extern "C" {
 
 int nb_gen_rays(const nb_camera* cam, float* ray_o, float* ray_d, float* near, float* far, unsigned char* mask_at_box, void* stream) {
     if (!cam || !ray_o || !ray_d || !near || !far || !mask_at_box || cam->H <= 0 || cam->W <= 0) {
@@ -511,23 +524,10 @@ int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, in
     return NB_OK;
 }
 
-// the density calls reuse the forward call's validation: only the frame / volume / weight fields (and the tensor-core
-// options) matter there
-static int fill_density_params(const nb_render_args* a, RenderParams* p) {
-    nb_render_args tmp = *a;
-    static float dummy;   // never dereferenced: the density kernels touch no ray or output-map pointer
-    float* d = &dummy;
-    tmp.n_rays = 1; tmp.n_samples = 1;
-    tmp.ray_o = tmp.ray_d = tmp.near = tmp.far = d;
-    tmp.rgb_map = tmp.disp_map = tmp.acc_map = tmp.depth_map = d;
-    tmp.mask_msks = nullptr; tmp.save = nullptr;
-    return nbi_fill_render_params(&tmp, p);
-}
-
 int nb_decode_density(const nb_render_args* a, const float* points, int n_points, float* sigma, void* stream) {
     if (!a || !points || !sigma || n_points < 0) { set_error("nb_decode_density: null argument"); return NB_ERR_BAD_ARG; }
     RenderParams p;
-    const int stp = fill_density_params(a, &p);
+    const int stp = fill_frame_params(a, "nb_decode_density", &p);
     if (stp != NB_OK) return stp;
     return launch_density_f32(p, a->volume_dtype, points, n_points, sigma, (cudaStream_t)stream);
 }
@@ -545,17 +545,18 @@ int nb_decode_density_list(const nb_render_args* a, const float* points, int n_p
         return NB_ERR_BAD_ARG;
     }
     RenderParams p;
-    const int stp = fill_density_params(a, &p);
+    const int stp = fill_frame_params(a, "nb_decode_density_list", &p);
     if (stp != NB_OK) return stp;
-    p.points = points; p.sigma = sigma; p.n_points = n_points;
-    return launch_density_tc_list(p, a->volume_dtype, a->precision == NB_PRECISION_TC_FP16X3 ? 3 : 1, a->workspace,
-                                  a->workspace_bytes, (cudaStream_t)stream);
+    p.skip_empty = a->skip_empty ? 1 : 0; p.stats = a->stats; p.trace = a->trace;
+    return launch_density_tc_list(p, a->volume_dtype, a->precision == NB_PRECISION_TC_FP16X3 ? 3 : 1, points, n_points, sigma,
+                                  a->workspace, a->workspace_bytes, (cudaStream_t)stream);
 }
 
 int nb_render_fwd(const nb_render_args* a, void* stream) {
     if (a && a->n_rays == 0 && a->batch > 0 && a->n_samples > 0) return NB_OK;
     RenderParams p;
-    const int stp = nbi_fill_render_params(a, &p);
+    int stp = fill_frame_params(a, "nb_render_fwd", &p);
+    if (stp == NB_OK) stp = fill_ray_params(a, "nb_render_fwd", &p);
     if (stp != NB_OK) return stp;
     if (a->save && a->mask_msks) { set_error("nb_render_fwd: mask views are an inference feature (no activation record)"); return NB_ERR_UNSUPPORTED; }
     if (a->save && a->precision != NB_PRECISION_FP32 && a->precision != NB_PRECISION_TC_TF32X3) {

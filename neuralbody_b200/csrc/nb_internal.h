@@ -20,7 +20,15 @@ inline int sm_count() {
     return sms;
 }
 
-// Kernel-side view of one nb_render_fwd call (passed by value as a __grid_constant__).
+inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+
+// Sample / point lists of the tensor-core pipelines: an entry's .w is its id | occupied-level bits << 28, so a list holds
+// < 2^28 ids; a classification block and a composite warp take whole rays of at most kListMaxSamples samples.
+constexpr uint32_t kListIdMask = 0x0FFFFFFFu;
+constexpr int kListMaxSamples = 1024;
+
+// Kernel-side view of one call (passed by value as a __grid_constant__): the caller's arguments as fill_frame_params and
+// fill_ray_params translate them, then the per-launch state the list launchers set.
 struct RenderParams {
     int batch, n_rays, n_samples;
     const float *ray_o, *ray_d, *near, *far, *t_vals, *t_rand;
@@ -46,15 +54,12 @@ struct RenderParams {
     const unsigned char* mask_msks; const float* mask_RT; const float* mask_Ks;   // f-1 mask views (null = none)
     int mask_nv, mask_H, mask_W;
     const float *mask_R0, *mask_Th0;   // single-view _msk variant: SMPL -> snapshot-world transform, or null
-    unsigned long long* stats; // u64[8] or null: [4] += layer-0 K-steps executed (x 128 rows); [0] += tiles executed, [1] += listed samples,
-                               // [2] += decoder-kernel ns, [3] += decoder launches, [5] / [6] += coarse-level half tiles
-                               // gathered from the staging / directly
-    float* save;               // (B,n,S,kSaveDim) activation record for nb_render_bwd (exact kernel only) or null
-    int rays_per_group;        // rays handled together by one CTA work item
-    int tiles_per_group;       // point tiles per group
-    int n_groups;              // total work items = batch * ceil(n_rays / rays_per_group)
-    int groups_per_frame;
-    // list pipeline (nb_render_tc_list.cu): one frame per launch
+    unsigned long long* stats; // u64[8] or null: [0] += tiles executed, [1] += listed samples, [2] += decoder-kernel ns,
+                               // [3] += decoder launches, [4] += layer-0 K-steps executed (x 128 rows), [5] / [6] += coarse-level
+                               // half tiles gathered from the staging / directly, [7] += fine-level half tiles gathered directly
+    float* save;               // activation record for nb_render_bwd or null: (B,n,S,kSaveDim) for NB_PRECISION_FP32,
+                               // trn::map_save's layout for NB_PRECISION_TC_TF32X3
+    // list pipelines (nb_render_tc_list.cu, nb_train.cu), set by their launchers: one frame per launch
     int frame;                 // frame of this launch
     int train_list;            // training path (nb_train.cu): ONE list for all classes and frames (list_a upwards, list_count[3]),
                                // entry ids count samples across the whole batch; raw_ws stays the frame's
@@ -72,12 +77,18 @@ struct RenderParams {
     int n_points;
 };
 
+// Check a call's fields and translate them into *p, or set an error that starts with `who` and return NB_ERR_*.  The frame
+// (batch, R, Th, bounds, voxel_size, out_sh, level_dims, volume and weight blobs) is read by every entry point; the rays,
+// samples, output maps and options by nb_render_fwd / nb_render_bwd only, which fill the frame first.
+int fill_frame_params(const nb_render_args* a, const char* who, RenderParams* p);   // value-initialises *p
+int fill_ray_params(const nb_render_args* a, const char* who, RenderParams* p);
+
 int launch_render_f32(const RenderParams& p, int volume_dtype, cudaStream_t stream);
 int launch_render_tc_list(const RenderParams& p, int volume_dtype, int passes, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t render_tc_list_workspace_bytes(int batch, int n_rays, int n_samples);
-bool render_tc_list_supported(const RenderParams& p);
 int launch_density_f32(const RenderParams& p, int volume_dtype, const float* pts, int n_points, float* sigma, cudaStream_t stream);
-int launch_density_tc_list(const RenderParams& p, int volume_dtype, int passes, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_density_tc_list(const RenderParams& p, int volume_dtype, int passes, const float* pts, int n_points, float* sigma,
+                           void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t density_tc_list_workspace_bytes(int batch, int n_points);
 bool tc_available();
 

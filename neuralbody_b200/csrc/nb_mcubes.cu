@@ -19,8 +19,6 @@ namespace {
 
 constexpr int kMcThreads = 256;
 
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 struct McGrid {
     const float* v;
     int nx, ny, nz;

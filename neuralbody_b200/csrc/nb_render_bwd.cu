@@ -432,8 +432,6 @@ extern "C" size_t nb_render_save_bytes(int batch, int n_rays, int n_samples) {
     return (size_t)batch * n_rays * n_samples * kSaveDim * 4;
 }
 
-extern "C" int nbi_fill_render_params(const nb_render_args* a, nb::RenderParams* out);   // nb_capi.cu (internal)
-
 extern "C" size_t nb_render_save_bytes_for(const nb_render_args* f) {
     if (!f) return 0;
     if (f->precision == NB_PRECISION_TC_TF32X3) return train_save_bytes(f->batch, f->n_rays, f->n_samples);
@@ -441,12 +439,10 @@ extern "C" size_t nb_render_save_bytes_for(const nb_render_args* f) {
 }
 extern "C" size_t nb_render_bwd_workspace_bytes_for(const nb_render_args* f) {
     if (!f) return 0;
-    if (f->precision == NB_PRECISION_TC_TF32X3) {
-        nb::RenderParams p;
-        if (nbi_fill_render_params(f, &p) != NB_OK) return 0;
-        return train_bwd_workspace_bytes(p);
-    }
-    return nb_render_bwd_workspace_bytes(f->batch, f->n_rays, f->n_samples);
+    if (f->precision != NB_PRECISION_TC_TF32X3) return nb_render_bwd_workspace_bytes(f->batch, f->n_rays, f->n_samples);
+    RenderParams p;
+    if (f->n_rays < 0 || f->n_samples <= 0 || fill_frame_params(f, "nb_render_bwd_workspace_bytes_for", &p) != NB_OK) return 0;
+    return train_bwd_workspace_bytes(p, f->n_rays, f->n_samples);
 }
 
 extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
@@ -455,12 +451,13 @@ extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
         return NB_ERR_BAD_ARG;
     }
     const nb_render_args* f = a->fwd;
+    RenderParams p;
+    int st = fill_frame_params(f, "nb_render_bwd", &p);
+    if (st == NB_OK) st = fill_ray_params(f, "nb_render_bwd", &p);
+    if (st != NB_OK) return st;
+    if (f->n_samples > bwd::kBwdMaxSamples) { set_error("nb_render_bwd: n_samples <= %d supported (got %d)", bwd::kBwdMaxSamples, f->n_samples); return NB_ERR_UNSUPPORTED; }
     if (f->precision == NB_PRECISION_TC_TF32X3) {
-        if (f->n_samples > bwd::kBwdMaxSamples) { set_error("nb_render_bwd: n_samples <= %d supported (got %d)", bwd::kBwdMaxSamples, f->n_samples); return NB_ERR_UNSUPPORTED; }
-        if (a->workspace_bytes < nb_render_bwd_workspace_bytes_for(f)) { set_error("nb_render_bwd: workspace too small (see nb_render_bwd_workspace_bytes_for)"); return NB_ERR_BAD_ARG; }
-        nb::RenderParams p;
-        int st = nbi_fill_render_params(f, &p);
-        if (st != NB_OK) return st;
+        if (a->workspace_bytes < train_bwd_workspace_bytes(p, f->n_rays, f->n_samples)) { set_error("nb_render_bwd: workspace too small (see nb_render_bwd_workspace_bytes_for)"); return NB_ERR_BAD_ARG; }
         trn::TrainBwd t;
         t.save = a->save; t.raw = a->raw; t.d_rgb = a->d_rgb_map; t.d_depth = a->d_depth_map; t.d_acc = a->d_acc_map;
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
@@ -471,14 +468,12 @@ extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
         set_error("nb_render_bwd: the training path runs the exact kernel (NB_PRECISION_FP32 + fp32 volume)");
         return NB_ERR_UNSUPPORTED;
     }
-    if (f->n_samples > bwd::kBwdMaxSamples) { set_error("nb_render_bwd: n_samples <= %d supported (got %d)", bwd::kBwdMaxSamples, f->n_samples); return NB_ERR_UNSUPPORTED; }
     if (a->workspace_bytes < nb_render_bwd_workspace_bytes(f->batch, f->n_rays, f->n_samples)) {
         set_error("nb_render_bwd: workspace too small");
         return NB_ERR_BAD_ARG;
     }
-    bwd::BwdParams Q;
-    int st = nbi_fill_render_params(f, &Q.f);
-    if (st != NB_OK) return st;
+    bwd::BwdParams Q{};
+    Q.f = p;
     Q.save = a->save; Q.raw = a->raw;
     Q.d_rgb = a->d_rgb_map; Q.d_depth = a->d_depth_map; Q.d_acc = a->d_acc_map;
     Q.ws = (float*)a->workspace;

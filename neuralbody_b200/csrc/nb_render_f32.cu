@@ -144,8 +144,12 @@ struct RayInfo {
     float o[3], d[3], near, far, norm, vd[3];
 };
 
+// Work items of render_f32_kernel: groups of whole rays, 64 / S rays in one tile when S <= 64, else one ray of ceil(S / 64)
+// tiles.  rays / tiles per group, groups per frame / in the launch.
+struct Groups { int rays, tiles, per_frame, total; };
+
 template <typename VT>
-__global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant__ RenderParams P) {
+__global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant__ RenderParams P, const Groups grp) {
     extern __shared__ __align__(16) float smem[];
     float* X = smem;                           // [64][356]
     float* Y = X + TP * LDX;                   // [64][324]
@@ -155,7 +159,7 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
     int* prayc = pray + TP;                                // [64] same, padding clamped to ray 0
     int* pins = prayc + TP;                                // [64] f-1: sample projects into every mask view
     float* vt = reinterpret_cast<float*>(pins + TP);       // [G][128] per-ray view term
-    const int G = P.rays_per_group, S = P.n_samples;
+    const int G = grp.rays, S = P.n_samples;
     float* zbuf = vt + G * kColor;             // [G][S]
     float4* rawbuf = reinterpret_cast<float4*>(zbuf + ((G * S + 3) & ~3));  // [G][S]
     RayInfo* rays = reinterpret_cast<RayInfo*>(rawbuf + G * S);            // [G]
@@ -164,9 +168,9 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* wf = P.wf32;
 
-    for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x) {
-        const int b = g / P.groups_per_frame;
-        const int r0 = (g % P.groups_per_frame) * G;
+    for (int g = blockIdx.x; g < grp.total; g += gridDim.x) {
+        const int b = g / grp.per_frame;
+        const int r0 = (g % grp.per_frame) * G;
         const int nr = min(G, P.n_rays - r0);
 
         // ---- per-frame transform + per-ray set-up
@@ -193,7 +197,7 @@ __global__ void __launch_bounds__(NT, 1) render_f32_kernel(const __grid_constant
             vt[idx] = acc;
         }
 
-        for (int tile = 0; tile < P.tiles_per_group; ++tile) {
+        for (int tile = 0; tile < grp.tiles; ++tile) {
             // ---- phase 1: geometry of the tile's points (one thread per point)
             if (tid < TP) {
                 const int pgidx = tile * TP + tid;
@@ -367,17 +371,17 @@ static int launch_by_dtype(const char* name, Kernel k32, Kernel k16, int volume_
     return NB_OK;
 }
 
-int launch_render_f32(const RenderParams& p_in, int volume_dtype, cudaStream_t stream) {
-    RenderParams p = p_in;
+int launch_render_f32(const RenderParams& p, int volume_dtype, cudaStream_t stream) {
     const int S = p.n_samples;
-    if (S <= f32::TP) { p.rays_per_group = f32::TP / S; p.tiles_per_group = 1; }
-    else { p.rays_per_group = 1; p.tiles_per_group = (S + f32::TP - 1) / f32::TP; }
-    p.groups_per_frame = (p.n_rays + p.rays_per_group - 1) / p.rays_per_group;
-    p.n_groups = p.groups_per_frame * p.batch;
-    const size_t smem = f32::smem_bytes(p.rays_per_group, S);
+    f32::Groups grp;
+    if (S <= f32::TP) { grp.rays = f32::TP / S; grp.tiles = 1; }
+    else { grp.rays = 1; grp.tiles = (S + f32::TP - 1) / f32::TP; }
+    grp.per_frame = (p.n_rays + grp.rays - 1) / grp.rays;
+    grp.total = grp.per_frame * p.batch;
+    const size_t smem = f32::smem_bytes(grp.rays, S);
     if (smem > 227 * 1024) { set_error("n_samples=%d needs %zu B of shared memory (> 227 KB)", S, smem); return NB_ERR_UNSUPPORTED; }
     return launch_by_dtype("render_f32", f32::render_f32_kernel<float>, f32::render_f32_kernel<__half>, volume_dtype,
-                           p.n_groups, smem, stream, p);
+                           grp.total, smem, stream, p, grp);
 }
 
 int launch_density_f32(const RenderParams& p, int volume_dtype, const float* pts, int n_points, float* sigma, cudaStream_t stream) {

@@ -33,8 +33,6 @@ using tcr::Quad;
 
 constexpr int TP = 128;                                            // list rows per tile
 constexpr int NUM_SEGS = 6;
-constexpr int MAXS = 1024;                                         // samples per classification block
-constexpr uint32_t ID_MASK = 0x0FFFFFFFu;                          // list entry .w = frame sample id | level bits << 28
 
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
@@ -104,16 +102,16 @@ __device__ __forceinline__ void append_to_lists(const RenderParams& P, const flo
     }
 }
 
-// One CTA per block of rays_per_group rays (<= 1024 samples), CLS_PER_THREAD samples per thread, SAMPLE-major inside the
-// block so that consecutive list entries are the same depth sample of neighbouring rays (they share their corner lines).
+// One CTA per block of rays_per_block = kListMaxSamples / S rays, CLS_PER_THREAD samples per thread, SAMPLE-major inside
+// the block so that consecutive list entries are the same depth sample of neighbouring rays (they share their corner lines).
 // 256-thread CTAs: eight of them are resident per SM, which hides the one atomicAdd round trip each block waits for.
-constexpr int CLS_PER_THREAD = MAXS / CLS_THREADS;
-__global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __grid_constant__ RenderParams P) {
+constexpr int CLS_PER_THREAD = kListMaxSamples / CLS_THREADS;
+__global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __grid_constant__ RenderParams P, int rays_per_block) {
     __shared__ FrameXf xf;
     const int tid = threadIdx.x;
     const int S = P.n_samples, b = P.frame;
-    const int r0 = blockIdx.x * P.rays_per_group;
-    const int nr = min(P.rays_per_group, P.n_rays - r0);
+    const int r0 = blockIdx.x * rays_per_block;
+    const int nr = min(rays_per_block, P.n_rays - r0);
     load_frame_xf(P, b, xf, tid);
     __syncthreads();
     // robustly negative sigma on all-zero features => such a sample has compositing weight exactly 0 and is not evaluated
@@ -126,7 +124,7 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
 #pragma unroll
     for (int k = 0; k < CLS_PER_THREAD; ++k) {
         const int j = k * CLS_THREADS + tid;
-        const int ry = j % P.rays_per_group, s = j / P.rays_per_group;
+        const int ry = j % rays_per_block, s = j / rays_per_block;
         live[k] = ry < nr && s < S;
         cls[k] = -1;
         gm[k] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -150,7 +148,7 @@ __global__ void __launch_bounds__(CLS_THREADS) classify_compact_kernel(const __g
     const float4 empty = make_float4(0.f, 0.f, 0.f, fminf(__ldg(P.wf32 + oSigmaEmpty), 0.f));   // skipped sample: weight exactly 0
 #pragma unroll
     for (int k = 0; k < CLS_PER_THREAD; ++k)
-        if (cls[k] < 0 && live[k]) P.raw_ws[(__float_as_uint(gm[k].w) & ID_MASK) - id0] = empty;
+        if (cls[k] < 0 && live[k]) P.raw_ws[(__float_as_uint(gm[k].w) & kListIdMask) - id0] = empty;
 }
 
 // ------------------------------------------------------------------------------------------------ 1'. classify points
@@ -548,7 +546,7 @@ __device__ __forceinline__ void decode_list(const RenderParams& P) {
                         positional_embed_anchored<10, 5>(e.x, e.y, e.z, [&](int j, float v) { put(j, v); });
                         put(63, 0.f);
                     } else {
-                        const int smp = (int)(__float_as_uint(e.w) & ID_MASK);
+                        const int smp = (int)(__float_as_uint(e.w) & kListIdMask);
                         const size_t ri = (size_t)P.frame * P.n_rays + (prow < nrows ? smp / S : 0);
                         const float dx = __ldg(P.ray_d + ri * 3), dy = __ldg(P.ray_d + ri * 3 + 1), dz = __ldg(P.ray_d + ri * 3 + 2);
                         const float nrm = ray_norm(dx, dy, dz);
@@ -878,7 +876,7 @@ __device__ __forceinline__ void decode_list(const RenderParams& P) {
                     for (int o = 1; o <= 2; o <<= 1) sg[hr] += __shfl_xor_sync(0xffffffffu, sg[hr], o);
                     const int row = r0 + 8 * hr;
                     if ((lane & 3) == 0 && row < nrows) {
-                        const uint32_t id = __float_as_uint(rows[row].w) & ID_MASK;
+                        const uint32_t id = __float_as_uint(rows[row].w) & kListIdMask;
                         P.sigma[id] = sg[hr] + head[H_ALPHA + kHidden];
                     }
                 }
@@ -947,7 +945,7 @@ __device__ __forceinline__ void decode_list(const RenderParams& P) {
                 }
                 const int row = r0 + 8 * hr;
                 if ((lane & 3) == 0 && row < nrows) {
-                    const int smp = (int)(__float_as_uint(rows[row].w) & ID_MASK);
+                    const int smp = (int)(__float_as_uint(rows[row].w) & kListIdMask);
                     P.raw_ws[smp] = make_float4(cr[hr] + head[H_RGBB], cg[hr] + head[H_RGBB + 1], cbl[hr] + head[H_RGBB + 2],
                                                 sg[hr] + head[H_ALPHA + kHidden]);
                 }
@@ -991,7 +989,7 @@ __global__ void decoder_time_kernel(const __grid_constant__ RenderParams P) { ad
 // ------------------------------------------------------------------------------------------------ 3. raw2outputs
 constexpr int COMP_WARPS = 8;
 __global__ void __launch_bounds__(COMP_WARPS * 32) composite_kernel(const __grid_constant__ RenderParams P) {
-    __shared__ float zs[COMP_WARPS][MAXS];          // rays of up to MAXS samples (the decoder itself does not care about S)
+    __shared__ float zs[COMP_WARPS][kListMaxSamples];   // rays of up to kListMaxSamples samples (the decoder does not care about S)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ray = blockIdx.x * COMP_WARPS + warp;
     if (blockIdx.x == 0 && threadIdx.x == 0 && P.stats) add_decoder_time(P);
@@ -1028,7 +1026,6 @@ static int decoder_grid(size_t max_entries) {
     return (int)(max_tiles < sms ? max_tiles : sms);
 }
 
-static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 constexpr size_t CTL_BYTES = 32;   // per frame: u32 list counts [4], u64 ~start, u64 end
 
 // A batch's list workspace: one control block per frame, then the two list buffers of cap entries each, which the frames use
@@ -1053,22 +1050,15 @@ bool tc_available() { return true; }
 
 size_t render_tc_list_workspace_bytes(int batch, int n_rays, int n_samples) {
     const size_t cap = (size_t)n_rays * n_samples;
-    return tcl::lists_bytes(batch, cap) + tcl::align256(cap * sizeof(float4));   // + the raw records
-}
-
-bool render_tc_list_supported(const RenderParams& p) {
-    return p.n_samples <= tcl::MAXS && (size_t)p.n_rays * p.n_samples <= (size_t)tcl::ID_MASK;
+    return tcl::lists_bytes(batch, cap) + align256(cap * sizeof(float4));   // + the raw records
 }
 
 // the two frame-level kernels the training path (nb_train.cu) shares with this pipeline
-void launch_classify(RenderParams& p, cudaStream_t stream) {
-    p.rays_per_group = tcl::MAXS / p.n_samples;
-    p.tiles_per_group = 0;
-    p.groups_per_frame = (p.n_rays + p.rays_per_group - 1) / p.rays_per_group;
-    p.n_groups = p.groups_per_frame * p.batch;
-    tcl::classify_compact_kernel<<<p.groups_per_frame, tcl::CLS_THREADS, 0, stream>>>(p);
+void launch_classify(const RenderParams& p, cudaStream_t stream) {
+    const int rays_per_block = kListMaxSamples / p.n_samples;
+    tcl::classify_compact_kernel<<<(p.n_rays + rays_per_block - 1) / rays_per_block, tcl::CLS_THREADS, 0, stream>>>(p, rays_per_block);
 }
-void launch_composite(RenderParams& p, cudaStream_t stream) {
+void launch_composite(const RenderParams& p, cudaStream_t stream) {
     tcl::composite_kernel<<<(p.n_rays + tcl::COMP_WARPS - 1) / tcl::COMP_WARPS, tcl::COMP_WARPS * 32, 0, stream>>>(p);
 }
 
@@ -1076,8 +1066,8 @@ int launch_render_tc_list(const RenderParams& p_in, int volume_dtype, int passes
                           cudaStream_t stream) {
     RenderParams p = p_in;
     const int S = p.n_samples;
-    if (!render_tc_list_supported(p)) {
-        set_error("the tensor-core render path supports n_samples <= %d and n_rays * n_samples < 2^28 per frame", tcl::MAXS);
+    if (S > kListMaxSamples || (size_t)p.n_rays * S > (size_t)kListIdMask) {
+        set_error("the tensor-core render path supports n_samples <= %d and n_rays * n_samples < 2^28 per frame", kListMaxSamples);
         return NB_ERR_UNSUPPORTED;
     }
     if (!workspace || workspace_bytes < render_tc_list_workspace_bytes(p.batch, p.n_rays, S)) {
@@ -1109,12 +1099,12 @@ size_t density_tc_list_workspace_bytes(int batch, int n_points) {
     return tcl::lists_bytes(batch, (size_t)n_points);
 }
 
-// p.points / p.sigma / p.n_points set by the caller for the whole batch
-int launch_density_tc_list(const RenderParams& p_in, int volume_dtype, int passes, void* workspace, size_t workspace_bytes,
-                           cudaStream_t stream) {
+// pts (B, n, 3) and sigma (B, n) of the whole batch
+int launch_density_tc_list(const RenderParams& p_in, int volume_dtype, int passes, const float* pts, int n, float* sigma,
+                           void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     RenderParams p = p_in;
-    const int n = p.n_points;
-    if ((size_t)n > (size_t)tcl::ID_MASK) {
+    p.n_points = n;
+    if ((size_t)n > (size_t)kListIdMask) {
         set_error("nb_decode_density_list: n_points = %d; the tensor-core list holds < 2^28 points per frame", n);
         return NB_ERR_UNSUPPORTED;
     }
@@ -1130,8 +1120,8 @@ int launch_density_tc_list(const RenderParams& p_in, int volume_dtype, int passe
     const int grid = tcl::decoder_grid((size_t)n);
     for (int b = 0; b < p.batch; ++b) {
         tcl::set_frame_lists(p, workspace, b, (size_t)n);
-        p.points = p_in.points + (size_t)b * n * 3;
-        p.sigma = p_in.sigma + (size_t)b * n;
+        p.points = pts + (size_t)b * n * 3;
+        p.sigma = sigma + (size_t)b * n;
         tcl::classify_points_kernel<<<(n + tcl::CLS_THREADS - 1) / tcl::CLS_THREADS, tcl::CLS_THREADS, 0, stream>>>(p);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = tcl::launch_decoder<true>(p, volume_dtype, passes, grid, stream);

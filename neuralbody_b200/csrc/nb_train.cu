@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(GT, CTAS_PER_SM) gemm_tf32x3_kernel(const __gr
         if (row >= M) continue;
         const float* bias = G.bias;
         if (bias && G.bias_frame_stride)
-            bias += (size_t)((__float_as_uint(__ldg(&G.list[row].w)) & 0x0FFFFFFFu) / G.samples_per_frame) * G.bias_frame_stride;
+            bias += (size_t)((__float_as_uint(__ldg(&G.list[row].w)) & kListIdMask) / G.samples_per_frame) * G.bias_frame_stride;
 #pragma unroll
         for (int j = 0; j < B_ROWS / 8; ++j) {
             const int cl = 8 * j + cq;
@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(256) gather_kernel(const __grid_constant__ Ren
         const int tid = threadIdx.x;
         if (tid < GP && e0 + tid < count) {
             const float4 en = sv.list[e0 + tid];
-            const unsigned int id = __float_as_uint(en.w) & ID_MASK;
+            const unsigned int id = __float_as_uint(en.w) & kListIdMask;
             const int b = id / spf;
             const size_t ri = id / S;
             FrameXf fx;
@@ -353,7 +353,7 @@ __global__ void __launch_bounds__(256) head_kernel(const float* __restrict__ wf,
         float a2 = w.x * rw[2][0] + w.y * rw[2][1] + w.z * rw[2][2] + w.w * rw[2][3];
         a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
         if (lane == 0) {
-            const unsigned int id = __float_as_uint(sv.list[e].w) & ID_MASK;
+            const unsigned int id = __float_as_uint(sv.list[e].w) & kListIdMask;
             raw[id] = make_float4(a0 + __ldg(wf + oRgbB), a1 + __ldg(wf + oRgbB + 1), a2 + __ldg(wf + oRgbB + 2), ws[kColor]);
         }
     }
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(256) bwd_head_kernel(const float* __restrict__
 #pragma unroll
         for (int j = 0; j < 4; ++j) rw[c][j] = __ldg(wf + oRgbW + c * kColor + 4 * lane + j);
     for (unsigned int e = blockIdx.x * (blockDim.x >> 5) + warp; e < count; e += warps) {
-        const unsigned int id = __float_as_uint(sv.list[e].w) & ID_MASK;
+        const unsigned int id = __float_as_uint(sv.list[e].w) & kListIdMask;
         const float4 d = __ldg(d_raw + id);
         const float4 w = *reinterpret_cast<const float4*>(sv.WS + (size_t)e * kWS + 4 * lane);
         const float wv[4] = {w.x, w.y, w.z, w.w};
@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
         const int tid = threadIdx.x;
         if (tid < GP && e0 + tid < count) {
             const float4 en = sv.list[e0 + tid];
-            const int b = (__float_as_uint(en.w) & ID_MASK) / spf;
+            const int b = (__float_as_uint(en.w) & kListIdMask) / spf;
             FrameXf fx;
 #pragma unroll
             for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
@@ -471,10 +471,10 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ A
     const int col = threadIdx.x;
     if (col >= ncols || r0 >= r1) return;
     float acc = 0.f;
-    int cur = by_frame ? (int)((__float_as_uint(sv.list[r0].w) & ID_MASK) / spf) : 0;
+    int cur = by_frame ? (int)((__float_as_uint(sv.list[r0].w) & kListIdMask) / spf) : 0;
     for (unsigned int r = r0; r < r1; ++r) {
         if (by_frame) {
-            const int f = (int)((__float_as_uint(sv.list[r].w) & ID_MASK) / spf);
+            const int f = (int)((__float_as_uint(sv.list[r].w) & kListIdMask) / spf);
             if (f != cur) { if (acc != 0.f) atomicAdd(out + (size_t)cur * out_stride + col, acc); acc = 0.f; cur = f; }
         }
         acc += A[(size_t)r * ld + col];
@@ -525,8 +525,8 @@ static GradBlob grad_blob_map(const RenderParams& p) {
 
 size_t train_save_bytes(int batch, int n_rays, int n_samples) { return save_bytes(batch, (size_t)batch * n_rays * n_samples); }
 
-size_t train_bwd_workspace_bytes(const RenderParams& p) {
-    const size_t pmax = (size_t)p.batch * p.n_rays * p.n_samples;
+size_t train_bwd_workspace_bytes(const RenderParams& p, int n_rays, int n_samples) {
+    const size_t pmax = (size_t)p.batch * n_rays * n_samples;
     const size_t per_point = 4 + kWS + 3 * kHidden + kFeat;
     const size_t fixed = (size_t)kWS * kH2X + (size_t)p.batch * kWS + 64 /* dwcol, dbias3 */ +
                          (size_t)kColor * kColorK + (size_t)p.batch * kColor + 2 * (size_t)kColor * kHidden + 2 * (size_t)p.batch * kHidden + 256;
@@ -534,12 +534,12 @@ size_t train_bwd_workspace_bytes(const RenderParams& p) {
 }
 
 bool train_supported(const RenderParams& p) {
-    return p.n_samples <= 1024 && (long long)p.batch * p.n_rays * p.n_samples < (1ll << 28);
+    return p.n_samples <= kListMaxSamples && (long long)p.batch * p.n_rays * p.n_samples <= (long long)kListIdMask;
 }
 
 int launch_train_fwd(const RenderParams& p_in, int volume_dtype, cudaStream_t stream) {
     RenderParams p = p_in;
-    if (!train_supported(p)) { set_error("tc_tf32x3: n_samples <= 1024 and batch * n_rays * n_samples < 2^28"); return NB_ERR_UNSUPPORTED; }
+    if (!train_supported(p)) { set_error("tc_tf32x3: n_samples <= %d and batch * n_rays * n_samples < 2^28", kListMaxSamples); return NB_ERR_UNSUPPORTED; }
     if (!p.save || !p.raw) { set_error("tc_tf32x3 (training precision) needs nb_render_args.save and .raw"); return NB_ERR_BAD_ARG; }
     if (p.n_rays == 0 || p.batch == 0) return NB_OK;
     const size_t pmax = (size_t)p.batch * p.n_rays * p.n_samples;

@@ -5,7 +5,6 @@
 namespace nb {
 namespace trn {
 
-constexpr uint32_t ID_MASK = 0x0FFFFFFFu;   // list entry .w = global sample id | level bits << 28
 constexpr int kH2X = 352;                   // colour-layer input record: [h2 256 | PE(xyz) 63 | 0 | PE(viewdir) 27 | 0 x 5]
 constexpr int kWS = 144;                    // colour-layer output record: [w 128 | sigma | 0 x 15]
 constexpr int kXyzCol = 256, kViewCol = 320;
@@ -51,14 +50,14 @@ struct TrainBwd {
 }  // namespace trn
 
 size_t train_save_bytes(int batch, int n_rays, int n_samples);
-size_t train_bwd_workspace_bytes(const RenderParams& p);
+size_t train_bwd_workspace_bytes(const RenderParams& p, int n_rays, int n_samples);   // p: the frame (batch, level dims)
 bool train_supported(const RenderParams& p);
 int launch_train_fwd(const RenderParams& p, int volume_dtype, cudaStream_t stream);
 int launch_train_bwd(const RenderParams& p, const trn::TrainBwd& t, cudaStream_t stream);
 
 // shared pieces living in other translation units
-void launch_classify(RenderParams& p, cudaStream_t stream);          // nb_render_tc_list.cu (p.frame, lists, raw_ws set by the caller)
-void launch_composite(RenderParams& p, cudaStream_t stream);         // nb_render_tc_list.cu
+void launch_classify(const RenderParams& p, cudaStream_t stream);    // nb_render_tc_list.cu (p.frame, lists, raw_ws set by the caller)
+void launch_composite(const RenderParams& p, cudaStream_t stream);   // nb_render_tc_list.cu
 void launch_composite_bwd(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
                           float* d_raw_out, int d_raw_stride, cudaStream_t stream);   // nb_render_bwd.cu
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,

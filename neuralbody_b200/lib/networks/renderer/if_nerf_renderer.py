@@ -19,6 +19,8 @@ from neuralbody_b200.lib.config import get_active_cfg
 
 _PRECISIONS = {"fp32": capi.NB_PRECISION_FP32, "tc_fp16": capi.NB_PRECISION_TC_FP16,
                "tc_fp16x3": capi.NB_PRECISION_TC_FP16X3}
+# the fields of nb_decoder_weights that point at the 17 tensors of Network.decoder_tensors(), in that order
+_DECODER_FIELDS = tuple(f[0] for f in capi.nb_decoder_weights._fields_[:17])
 
 
 def _ptr(t):
@@ -71,10 +73,11 @@ class Renderer:
         cfg = get_active_cfg()
         return cfg[name] if name in cfg else default
 
-    def _precision(self):
-        name = str(self._opt("render_precision", "tc_fp16x3"))
+    def _precision(self, key, default):
+        """NB_PRECISION_* named by cfg[key] (render_precision, density_precision)."""
+        name = str(self._opt(key, default))
         if name not in _PRECISIONS:
-            raise ValueError("cfg.render_precision must be one of %s" % sorted(_PRECISIONS))
+            raise ValueError("cfg.%s must be one of %s" % (key, sorted(_PRECISIONS)))
         return _PRECISIONS[name]
 
     def _train_precision(self, B, n, S):
@@ -229,7 +232,7 @@ class Renderer:
         params = self.net.decoder_tensors()
         needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
                                                   any(v.requires_grad for v in feature_volume))
-        precision = self._train_precision(B, n, S) if needs_grad else self._precision()
+        precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
             # the tensor-core pipeline works on a frame-wide sample list: rays of up to 1024 samples, < 2^28 samples per frame
@@ -242,10 +245,7 @@ class Renderer:
         call = {
             "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": self._volume_dtype(precision),
             "ray_o": _f32c(ray_o, dev), "ray_d": _f32c(ray_d, dev), "near": _f32c(near, dev), "far": _f32c(far, dev),
-            "R": _f32c(sp_input['R'], dev), "Th": _f32c(sp_input['Th'], dev).reshape(B, 3),   # (B,1,3) or (B,3) upstream
-            "bounds": _f32c(sp_input['bounds'], dev), "latent_index": sp_input['latent_index'],
-            "out_sh": [int(v) for v in sp_input['out_sh']], "voxel_size": [float(v) for v in cfg.voxel_size],
-            "t_rand": None if t_rand is None else _f32c(t_rand, dev), "white_bkgd": bool(cfg.white_bkgd),
+            "sp_input": sp_input, "t_rand": None if t_rand is None else _f32c(t_rand, dev), "white_bkgd": bool(cfg.white_bkgd),
             "z_vals": None if z_vals is None else _f32c(z_vals.detach(), dev),
             "feature_volume": list(feature_volume), "want_raw": want_raw or needs_grad, "user_raw": bool(want_raw), "out": out, "trace": trace,
             "want_weights": (bool(self._opt("render_return_weights", True)) if want_weights is None else bool(want_weights))
@@ -329,8 +329,7 @@ class Renderer:
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         precision, vdtype = call["precision"], call["vdtype"]
         with torch.cuda.device(dev), torch.no_grad():
-            vol_blob, dims = self.pack_volume(call["feature_volume"], vdtype)
-            w_blob = self.pack_weights(call["latent_index"], dev)
+            a, frame = self._frame_args(B, call["feature_volume"], call["sp_input"], vdtype, dev)
             t_vals = self._t_vals(S, dev)
             out = call["out"]
             if out is None:
@@ -350,8 +349,7 @@ class Renderer:
                     raw = self._pool_take("raw", B * n * S * 4, torch.float32, dev)[:B * n * S * 4].view(B, n, S, 4)
                 else:
                     raw = torch.empty((B, n, S, 4), dtype=torch.float32, device=dev)
-            a = capi.nb_render_args()
-            a.batch, a.n_rays, a.n_samples = B, n, S
+            a.n_rays, a.n_samples = n, S
             a.precision = precision
             sv = None
             if save:
@@ -363,17 +361,7 @@ class Renderer:
             a.t_vals = t_vals.data_ptr()
             a.t_rand = call["t_rand"].data_ptr() if call["t_rand"] is not None else None
             a.z_vals = call["z_vals"].data_ptr() if call["z_vals"] is not None else None
-            a.R, a.Th, a.bounds = call["R"].data_ptr(), call["Th"].data_ptr(), call["bounds"].data_ptr()
-            for i in range(3):
-                a.voxel_size[i] = call["voxel_size"][i]
-                a.out_sh[i] = call["out_sh"][i]
-            for l in range(capi.NB_NUM_LEVELS):
-                for j in range(4):
-                    a.level_dims[l][j] = dims[l][j]
-            a.volume_blob, a.volume_dtype = vol_blob.data_ptr(), vdtype
-            a.weights_blob = w_blob.data_ptr()
             a.white_bkgd = 1 if call["white_bkgd"] else 0
-            a.precision = precision
             a.rgb_map, a.disp_map = out['rgb_map'].data_ptr(), out['disp_map'].data_ptr()
             a.acc_map, a.depth_map = out['acc_map'].data_ptr(), out['depth_map'].data_ptr()
             a.out_ray_stride = self._out_stride(out, B, n)
@@ -404,7 +392,7 @@ class Renderer:
                     del recs[:-4]
                 # NOT the output tensors: they carry grad_fn -> this call's autograd node -> ctx.call, a reference cycle only the
                 # cyclic garbage collector can free (measured: ~7 MB leaked per training step and a 50-130 ms gc pause every few steps)
-                call["keep"] = (vol_blob, w_blob, t_vals)
+                call["keep"] = frame + (t_vals,)
         if raw is not None and call["want_raw"] and not save:
             out = dict(out)
             out['raw'] = raw
@@ -422,13 +410,12 @@ class Renderer:
             def cf(t):
                 return None if t is None else t.to(device=dev, dtype=torch.float32).contiguous()
             d_rgb, d_depth, d_acc = cf(d_rgb), cf(d_depth), cf(d_acc)
-            w = self._weights_struct(params, call["latent_index"], dev)
+            w = self._weights_struct(params, call["sp_input"]['latent_index'], dev)
             # 17 small tensors (they stay in the allocator's small pool), zeroed by one multi-tensor launch
             gparams = [torch.empty_like(t, dtype=torch.float32, device=dev) for t in params]
             torch._foreach_zero_(gparams)
             g = capi.nb_decoder_weights()
-            names = [f[0] for f in capi.nb_decoder_weights._fields_][:17]
-            for name, t in zip(names, gparams):
+            for name, t in zip(_DECODER_FIELDS, gparams):
                 setattr(g, name, t.data_ptr())
             g.latent_index, g.num_train_frame, g.batch = w[0].latent_index, w[0].num_train_frame, B
             want_vol = any(needs[:len(vols)])
@@ -459,9 +446,8 @@ class Renderer:
     def _weights_struct(self, tensors, latent_index, device):
         """nb_decoder_weights over the raw parameter tensors (+ the tensors kept alive)."""
         w = capi.nb_decoder_weights()
-        names = [f[0] for f in capi.nb_decoder_weights._fields_][:17]
         keep = []
-        for name, t in zip(names, tensors):
+        for name, t in zip(_DECODER_FIELDS, tensors):
             t = t.detach()
             if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
                 t = t.to(device=device, dtype=torch.float32).contiguous()
@@ -474,38 +460,42 @@ class Renderer:
         w.batch = int(latent_index.shape[0])
         return w, keep
 
+    def _frame_args(self, B, feature_volume, sp_input, vdtype, dev):
+        """nb_render_args with the frame fields every entry point reads filled in: batch, R, Th, bounds, voxel_size, out_sh
+        and the packed volume (level_dims, volume_blob / dtype) and weights.  Returns (args, tensors the args point into):
+        the caller keeps those alive while any call reads the args (nb_render_bwd reads R / Th / bounds again)."""
+        cfg = get_active_cfg()
+        vol_blob, dims = self.pack_volume(feature_volume, vdtype)
+        w_blob = self.pack_weights(sp_input['latent_index'], dev)
+        R, Th = _f32c(sp_input['R'], dev), _f32c(sp_input['Th'], dev).reshape(B, 3)   # Th: (B,1,3) or (B,3) upstream
+        bounds = _f32c(sp_input['bounds'], dev)
+        a = capi.nb_render_args()
+        a.batch = B
+        a.R, a.Th, a.bounds = R.data_ptr(), Th.data_ptr(), bounds.data_ptr()
+        for i in range(3):
+            a.voxel_size[i] = float(cfg.voxel_size[i])
+            a.out_sh[i] = int(sp_input['out_sh'][i])
+        for l in range(capi.NB_NUM_LEVELS):
+            for j in range(4):
+                a.level_dims[l][j] = dims[l][j]
+        a.volume_blob, a.volume_dtype, a.weights_blob = vol_blob.data_ptr(), vdtype, w_blob.data_ptr()
+        return a, (vol_blob, w_blob, R, Th, bounds)
+
     def calculate_density(self, wpts, feature_volume, sp_input):
         """Network.calculate_density (latent_xyzc.py:74-89) on arbitrary world points: (B,P,3) -> (B,P,1), raw sigma.
         f-3: the alpha decoder of the mesh renderer (if_mesh_renderer.py:36-41).  `cfg.density_precision`: 'fp32' (default,
         the exact kernel nb_decode_density), or 'tc_fp16x3' / 'tc_fp16' (nb_decode_density_list on the tensor cores; with
         `cfg.render_skip_empty` a point with all-zero features gets sigma(empty) without running the decoder)."""
-        cfg = get_active_cfg()
         dev = wpts.device
         if dev.type != "cuda":
             raise RuntimeError("calculate_density needs CUDA tensors: there is no CPU implementation")
-        name = str(self._opt("density_precision", "fp32"))
-        if name not in _PRECISIONS:
-            raise ValueError("cfg.density_precision must be one of %s" % sorted(_PRECISIONS))
-        precision = _PRECISIONS[name]
+        precision = self._precision("density_precision", "fp32")
         vdtype = capi.NB_DTYPE_F32 if precision == capi.NB_PRECISION_FP32 else self._volume_dtype(precision)
         B, Pn = int(wpts.shape[0]), int(wpts.shape[1])
         with torch.cuda.device(dev), torch.no_grad():
-            vol_blob, dims = self.pack_volume(feature_volume, vdtype)
-            w_blob = self.pack_weights(sp_input['latent_index'], dev)
+            a, keep = self._frame_args(B, feature_volume, sp_input, vdtype, dev)
             pts = _f32c(wpts, dev)
-            R, Th = _f32c(sp_input['R'], dev), _f32c(sp_input['Th'], dev).reshape(B, 3)
-            bounds = _f32c(sp_input['bounds'], dev)
             sigma = torch.empty((B, Pn, 1), dtype=torch.float32, device=dev)
-            a = capi.nb_render_args()
-            a.batch = B
-            a.R, a.Th, a.bounds = R.data_ptr(), Th.data_ptr(), bounds.data_ptr()
-            for i in range(3):
-                a.voxel_size[i] = float(cfg.voxel_size[i])
-                a.out_sh[i] = int(sp_input['out_sh'][i])
-            for l in range(capi.NB_NUM_LEVELS):
-                for j in range(4):
-                    a.level_dims[l][j] = dims[l][j]
-            a.volume_blob, a.volume_dtype, a.weights_blob = vol_blob.data_ptr(), vdtype, w_blob.data_ptr()
             a.precision = precision
             stream = torch.cuda.current_stream(dev).cuda_stream
             if precision == capi.NB_PRECISION_FP32:
