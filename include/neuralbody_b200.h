@@ -303,6 +303,14 @@ size_t nb_render_bwd_workspace_bytes(int batch, int n_rays, int n_samples);   /*
 size_t nb_render_save_bytes_for(const nb_render_args* fwd);
 size_t nb_render_bwd_workspace_bytes_for(const nb_render_args* fwd);
 int    nb_render_bwd(const nb_render_bwd_args* args, void* stream);
+/* nb_render_bwd plus the gradients of the frame transform the forward call read (nb_render_args.R / .Th): what pose
+ * refinement needs, i.e. upstream autograd through pts_to_can_pts -> get_grid_coords -> F.grid_sample's grid input
+ * (latent_xyzc.py:41-72).  d_R: device (B,3,3) fp32, d_Th: device (B,3) fp32; both are ACCUMULATED into and either may
+ * be NULL.  R and Th reach the outputs only through the grid coordinates (the positional encoding takes the world points),
+ * so this is the trilinear backward with respect to the sample position, chained through the transform.  Both training
+ * precisions; it reads the volume blob the forward gathered from.  nb_render_bwd(args, stream) is
+ * nb_render_bwd_frame(args, NULL, NULL, stream) and enqueues no frame-gradient work.  No extra workspace. */
+int    nb_render_bwd_frame(const nb_render_bwd_args* args, float* d_R, float* d_Th, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Diagnostics.

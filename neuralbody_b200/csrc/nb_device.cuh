@@ -110,10 +110,10 @@ __device__ __forceinline__ void corner_setup(float ix, float iy, float iz, int W
     c.wy[0] = __fsub_rn(__fadd_rn(fy, 1.f), iy); c.wy[1] = __fsub_rn(iy, fy);
     c.wz[0] = __fsub_rn(__fadd_rn(fz, 1.f), iz); c.wz[1] = __fsub_rn(iz, fz);
 }
-// f(voxel index, weight) for the corners of the cell that lie inside the W x H x D volume, in ATen's accumulation order:
-// tnw, tne, tsw, tse, bnw, bne, bsw, bse (x fastest)
+// f(voxel index, dx, dy, dz) for the corners (x0 + dx, y0 + dy, z0 + dz) of the cell that lie inside the W x H x D volume,
+// in ATen's accumulation order: tnw, tne, tsw, tse, bnw, bne, bsw, bse (x fastest)
 template <typename F>
-__device__ __forceinline__ void for_each_corner(const Corners& c, int W, int H, int D, F&& f) {
+__device__ __forceinline__ void for_each_corner_at(const Corners& c, int W, int H, int D, F&& f) {
 #pragma unroll
     for (int dz = 0; dz < 2; ++dz)
 #pragma unroll
@@ -122,8 +122,15 @@ __device__ __forceinline__ void for_each_corner(const Corners& c, int W, int H, 
             for (int dx = 0; dx < 2; ++dx) {
                 const int x = c.x0 + dx, y = c.y0 + dy, z = c.z0 + dz;
                 if ((c.x0 != -2) && x >= 0 && x < W && y >= 0 && y < H && z >= 0 && z < D)
-                    f(((size_t)z * H + y) * W + x, __fmul_rn(__fmul_rn(c.wx[dx], c.wy[dy]), c.wz[dz]));
+                    f(((size_t)z * H + y) * W + x, dx, dy, dz);
             }
+}
+// f(voxel index, weight) for the same corners in the same order
+template <typename F>
+__device__ __forceinline__ void for_each_corner(const Corners& c, int W, int H, int D, F&& f) {
+    for_each_corner_at(c, W, H, D, [&](size_t vox, int dx, int dy, int dz) {
+        f(vox, __fmul_rn(__fmul_rn(c.wx[dx], c.wy[dy]), c.wz[dz]));
+    });
 }
 
 // Channel quad q (0..87) of the 352-wide feature, level 0 first (latent_xyzc.py:66-71): its level and first channel there
@@ -164,6 +171,83 @@ __device__ __forceinline__ float4 gather_quad(const RenderParams& P, int b, floa
         acc.z = fmaf(v.z, wgt, acc.z); acc.w = fmaf(v.w, wgt, acc.w);
     });
     return acc;
+}
+
+// Backward of gather_quad with respect to the sample position: sum_c df_c * d f_c / d(i_x, i_y, i_z), where i are the
+// level's un-normalised coordinates (ATen's grid_sampler_3d backward for the grid, zeros padding: the weight of corner
+// (dx, dy, dz) is w_x[dx] w_y[dy] w_z[dz] with d w_x[0] / d i_x = -1 and d w_x[1] / d i_x = +1; corners outside the volume
+// are 0 and contribute nothing).  The caller scales by d i / d g = (size - 1) / 2 and sums the levels.
+template <typename VT>
+__device__ __forceinline__ float3 gather_quad_dpos(const RenderParams& P, int b, float gx, float gy, float gz, int q, float4 df) {
+    int lvl, c0;
+    feature_quad(q, lvl, c0);
+    const int C = P.lvl_C[lvl], D = P.lvl_D[lvl], H = P.lvl_H[lvl], W = P.lvl_W[lvl];
+    Corners cn;
+    corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
+    const VT* vol = reinterpret_cast<const VT*>(reinterpret_cast<const char*>(P.volume) + P.lvl_off[lvl]) + (size_t)b * P.lvl_bstride[lvl];
+    float3 acc = make_float3(0.f, 0.f, 0.f);
+    for_each_corner_at(cn, W, H, D, [&](size_t vox, int dx, int dy, int dz) {
+        const float4 v = load4<VT>(vol + vox * C + c0);
+        const float s = fmaf(v.w, df.w, fmaf(v.z, df.z, fmaf(v.y, df.y, v.x * df.x)));   // dF . V at this corner
+        const float sx = cn.wy[dy] * cn.wz[dz] * s, sy = cn.wx[dx] * cn.wz[dz] * s, sz = cn.wx[dx] * cn.wy[dy] * s;
+        acc.x += dx ? sx : -sx;
+        acc.y += dy ? sy : -sy;
+        acc.z += dz ? sz : -sz;
+    });
+    return acc;
+}
+
+// d loss / d(grid coordinate g) -> d loss / d(canonical point c) for one axis: g = ((c - min) / voxel / out_sh) * 2 - 1
+__device__ __forceinline__ float grid_to_can_scale(const FrameXf& f, int axis_dhw) {
+    return 2.f / (f.voxel[axis_dhw] * f.out_sh[axis_dhw]);
+}
+
+// Frame-transform gradients of one sample (world_to_grid: c = (w - Th) R, c_j = sum_i p_i R[i][j]) from d loss / d c:
+// t[3 i + j] = d loss / d R[i][j] = p_i dc_j,  t[9 + i] = d loss / d Th[i] = -sum_j R[i][j] dc_j
+__device__ __forceinline__ void frame_grad_terms(const FrameXf& f, float wx, float wy, float wz, float dcx, float dcy, float dcz,
+                                                 float (&t)[12]) {
+    const float p[3] = {__fsub_rn(wx, f.Th[0]), __fsub_rn(wy, f.Th[1]), __fsub_rn(wz, f.Th[2])};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        t[3 * i + 0] = p[i] * dcx; t[3 * i + 1] = p[i] * dcy; t[3 * i + 2] = p[i] * dcz;
+        t[9 + i] = -fmaf(f.R[3 * i + 2], dcz, fmaf(f.R[3 * i + 1], dcy, f.R[3 * i] * dcx));
+    }
+}
+
+// Per-frame sums of the 12 frame-transform gradients (dR 9, dTh 3) across one warp's calls: lane k < 12 holds element k of
+// the running frame's sum and adds it to the caller's dR / dTh (either may be null) with one atomic when the frame changes.
+// Callers that visit frames in order (sample lists are frame-major) therefore issue one atomic per warp, frame and element.
+struct FrameGradAcc {
+    int frame = -1;
+    float v = 0.f;
+};
+__device__ __forceinline__ void frame_grad_flush(FrameGradAcc& a, float* __restrict__ dR, float* __restrict__ dTh, int lane) {
+    if (a.frame >= 0 && a.v != 0.f) {
+        if (lane < 9 && dR) atomicAdd(dR + (size_t)a.frame * 9 + lane, a.v);
+        else if (lane >= 9 && lane < 12 && dTh) atomicAdd(dTh + (size_t)a.frame * 3 + lane - 9, a.v);
+    }
+    a.v = 0.f;
+}
+// Whole warp: each lane contributes t for frame b (b < 0: nothing).
+__device__ __forceinline__ void frame_grad_add(FrameGradAcc& a, int b, const float (&t)[12], float* __restrict__ dR,
+                                               float* __restrict__ dTh, int lane) {
+    constexpr int kNone = 0x7fffffff;
+    int f = b < 0 ? kNone : b;
+    for (;;) {
+        const int fm = __reduce_min_sync(0xffffffffu, f);
+        if (fm == kNone) break;
+        float mine = 0.f;
+#pragma unroll
+        for (int k = 0; k < 12; ++k) {
+            float s = f == fm ? t[k] : 0.f;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == k) mine = s;
+        }
+        if (fm != a.frame) { frame_grad_flush(a, dR, dTh, lane); a.frame = fm; }
+        a.v += mine;
+        if (f == fm) f = kNone;
+    }
 }
 
 // ---------------------------------------------------------------- f-1: if_clight_renderer_mmsk.py:12-45

@@ -1,5 +1,6 @@
 // Backward of the fused render (nb_render_bwd): gradients of rgb_map / depth_map / acc_map with respect to
-// the four dense feature volumes, every decoder parameter and the latent table.
+// the four dense feature volumes, every decoder parameter and the latent table; nb_render_bwd_frame adds the frame
+// transform R / Th.
 //
 // Upstream this is PyTorch autograd through raw2outputs (nerf_net_utils.py:6-51), the eight Conv1d layers
 // and F.grid_sample (latent_xyzc.py:62-126), driven by Trainer.train (lib/train/trainers/trainer.py:46-53).
@@ -26,6 +27,7 @@ struct BwdParams {
     float* ws;                      // (B*n*S, kGradDim) scratch
     nb_decoder_weights w;           // raw decoder tensors
     float* d_vol[4];                // NCDHW fp32, caller-zeroed, accumulated into
+    float *d_R, *d_Th;              // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
     float* d_raw_out;               // composite backward writes d(rgb logits, sigma) of sample i at d_raw_out + i * d_raw_stride
     int d_raw_stride;
 };
@@ -144,6 +146,8 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
     const size_t npts = (size_t)P.batch * P.n_rays * S;
     const int tid = threadIdx.x;
     const float* wf = P.wf32;
+    const bool frame_grads = Q.d_R || Q.d_Th;
+    FrameGradAcc acc;                   // warp 0: running per-frame sums of dR / dTh
     for (size_t tile = blockIdx.x; tile * TP < npts; tile += gridDim.x) {
         const size_t p0 = tile * TP;
         auto gp = [&](int p) { return p0 + p; };
@@ -183,10 +187,13 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
         });
         // e. d_f = d_h0pre fc_0        ([256][352])
         gemm_tile<kHidden, kFeat, LDY, LDX>(Y, X, Q.w.fc0_w, Ws, [&](int, int, float v) { return v; });
-        // f. trilinear scatter-add (backward of F.grid_sample, zeros padding) into the NCDHW volume gradients
-        if (Q.d_vol[0]) {
+        // f. backward of F.grid_sample (zeros padding): scatter-add into the NCDHW volume gradients and / or, for the frame
+        // transform's gradients, d loss / d(canonical point) per (point, level) into Y (free after step e):
+        // Y[p * 16 + 3 lvl + axis], the world point at + 12..14 and the frame (-1: none) at + 15
+        if (Q.d_vol[0] || frame_grads) {
             for (int item = tid; item < TP * 4; item += NT) {   // (point, level): recompute the corner set-up
                 const int p = item >> 2, lvl = item & 3;
+                if (frame_grads && lvl == 0) Y[p * 16 + 15] = __int_as_float(-1);
                 if (!in_range(p)) continue;
                 const size_t g = gp(p);
                 const size_t ri = g / S;
@@ -205,18 +212,60 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                 const int cbase = level_feature_base(lvl);
                 Corners cn;
                 corner_setup(unnormalize(gx, W), unnormalize(gy, H), unnormalize(gz, D), W, H, D, cn);
-                float* dv = Q.d_vol[lvl] + (size_t)b * C * D * H * W;
-                const size_t cs = (size_t)D * H * W;
-                for_each_corner(cn, W, H, D, [&](size_t vox, float wgt) {
-                    for (int c = 0; c < C; ++c) {
-                        const float dfv = X[p * LDX + cbase + c];
-                        if (dfv != 0.f) atomicAdd(dv + (size_t)c * cs + vox, wgt * dfv);
+                if (Q.d_vol[0]) {
+                    float* dv = Q.d_vol[lvl] + (size_t)b * C * D * H * W;
+                    const size_t cs = (size_t)D * H * W;
+                    for_each_corner(cn, W, H, D, [&](size_t vox, float wgt) {
+                        for (int c = 0; c < C; ++c) {
+                            const float dfv = X[p * LDX + cbase + c];
+                            if (dfv != 0.f) atomicAdd(dv + (size_t)c * cs + vox, wgt * dfv);
+                        }
+                    });
+                }
+                if (frame_grads) {
+                    float3 d = make_float3(0.f, 0.f, 0.f);
+                    for (int q = cbase / 4; q < (cbase + C) / 4; ++q) {
+                        const float4 df = *reinterpret_cast<const float4*>(X + p * LDX + 4 * q);
+                        if (df.x == 0.f && df.y == 0.f && df.z == 0.f && df.w == 0.f) continue;
+                        const float3 dq = gather_quad_dpos<float>(P, b, gx, gy, gz, q, df);
+                        d.x += dq.x; d.y += dq.y; d.z += dq.z;
                     }
-                });
+                    // d i / d g = (size - 1) / 2; the level-independent d g / d c is applied per point below
+                    Y[p * 16 + 3 * lvl + 0] = d.x * (0.5f * (float)(W - 1));
+                    Y[p * 16 + 3 * lvl + 1] = d.y * (0.5f * (float)(H - 1));
+                    Y[p * 16 + 3 * lvl + 2] = d.z * (0.5f * (float)(D - 1));
+                    if (lvl == 0) {
+                        Y[p * 16 + 12] = wx; Y[p * 16 + 13] = wy; Y[p * 16 + 14] = wz;
+                        Y[p * 16 + 15] = __int_as_float(b);
+                    }
+                }
+            }
+        }
+        if (frame_grads) {   // warp 0: the tile's points -> dR / dTh terms, summed per frame
+            __syncthreads();
+            if (tid < 32) {
+#pragma unroll 1
+                for (int h = 0; h < TP / 32; ++h) {
+                    const float* y = Y + (32 * h + tid) * 16;
+                    const int b = __float_as_int(y[15]);
+                    float t[12] = {};
+                    if (b >= 0) {
+                        FrameXf fx;
+#pragma unroll
+                        for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
+                        // levels summed in order; grid x / y / z pair with the dhw axes 2 / 1 / 0
+                        const float dcx = ((y[0] + y[3]) + y[6]) + y[9], dcy = ((y[1] + y[4]) + y[7]) + y[10],
+                                    dcz = ((y[2] + y[5]) + y[8]) + y[11];
+                        frame_grad_terms(fx, y[12], y[13], y[14], dcx * grid_to_can_scale(fx, 2), dcy * grid_to_can_scale(fx, 1),
+                                         dcz * grid_to_can_scale(fx, 0), t);
+                    }
+                    frame_grad_add(acc, b, t, Q.d_R, Q.d_Th, tid);
+                }
             }
         }
         __syncthreads();
     }
+    if (frame_grads && tid < 32) frame_grad_flush(acc, Q.d_R, Q.d_Th, tid);
 }
 
 // ------------------------------------------------------------------------------------------ 3. weight gradients
@@ -445,7 +494,9 @@ extern "C" size_t nb_render_bwd_workspace_bytes_for(const nb_render_args* f) {
     return train_bwd_workspace_bytes(p, f->n_rays, f->n_samples);
 }
 
-extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
+extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) { return nb_render_bwd_frame(a, nullptr, nullptr, stream); }
+
+extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, float* d_Th, void* stream) {
     if (!a || !a->fwd || !a->save || !a->raw || !a->workspace || !a->weights || !a->grads) {
         set_error("nb_render_bwd: null argument");
         return NB_ERR_BAD_ARG;
@@ -462,6 +513,7 @@ extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
         t.save = a->save; t.raw = a->raw; t.d_rgb = a->d_rgb_map; t.d_depth = a->d_depth_map; t.d_acc = a->d_acc_map;
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
         for (int l = 0; l < 4; ++l) t.d_vol[l] = a->d_volumes[l];
+        t.d_R = d_R; t.d_Th = d_Th; t.volume_dtype = f->volume_dtype;
         return launch_train_bwd(p, t, (cudaStream_t)stream);
     }
     if (f->precision != NB_PRECISION_FP32 || f->volume_dtype != NB_DTYPE_F32) {
@@ -480,6 +532,7 @@ extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) {
     Q.d_raw_out = Q.ws + kGradRaw; Q.d_raw_stride = kGradDim;
     Q.w = *a->weights;
     for (int l = 0; l < 4; ++l) Q.d_vol[l] = a->d_volumes[l];
+    Q.d_R = d_R; Q.d_Th = d_Th;
     cudaStream_t s = (cudaStream_t)stream;
     const size_t nrays = (size_t)f->batch * f->n_rays, npts = nrays * f->n_samples;
     if (npts == 0) return NB_OK;

@@ -14,7 +14,8 @@
 //             head_kernel        rgb_fc, raw records; then composite_kernel (shared with the inference path)
 //   backward  composite_bwd_kernel (nb_render_bwd.cu) -> bwd_head_kernel -> 4 x gemm (dgrad, relu masks in the epilogue)
 //             -> scatter_kernel (trilinear backward, 16-byte vector atomics into a channels-last gradient blob, then one
-//             transposing add into the NCDHW gradients autograd expects) ; 4 x gemm (wgrad, split over the list, fp32 atomics)
+//             transposing add into the NCDHW gradients autograd expects) ; frame_grad_kernel (only when the frame
+//             transform's gradients are asked for) ; 4 x gemm (wgrad, split over the list, fp32 atomics)
 //             ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu).
 //
 // gemm_tf32x3_kernel: C[128 x <=256 tile] = epilogue(A B^T), fp32 in HBM on both sides.  Operands are split on the way into
@@ -445,6 +446,70 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
     }
 }
 
+// Frame-transform gradients (sp_input R, Th): the trilinear backward with respect to the sample position.  Same work items as
+// scatter_kernel; each (entry, quad) adds sum_c dF_c d f_c / d i, scaled to d / d(canonical point), into its entry's shared
+// slot; warp 0 then turns the 32 entries into dR / dTh terms and sums them per frame (one atomic per CTA, frame and element:
+// the list is frame-major and each CTA walks it in order).  Reads the packed blob the forward gathered from.
+template <typename VT>
+__global__ void __launch_bounds__(256) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
+                                                         float* __restrict__ dR, float* __restrict__ dTh) {
+    __shared__ float gc[GP][3], dc[GP][3];
+    __shared__ int fr[GP];
+    const unsigned int count = *sv.count;
+    const unsigned int spf = (unsigned int)P.n_rays * P.n_samples;
+    const int tid = threadIdx.x;
+    FrameGradAcc acc;
+    for (unsigned int e0 = blockIdx.x * GP; e0 < count; e0 += gridDim.x * GP) {
+        if (tid < GP) {
+            fr[tid] = -1;
+            dc[tid][0] = dc[tid][1] = dc[tid][2] = 0.f;
+            if (e0 + tid < count) {
+                const float4 en = sv.list[e0 + tid];
+                const int b = (__float_as_uint(en.w) & kListIdMask) / spf;
+                FrameXf fx;
+#pragma unroll
+                for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
+                float gx, gy, gz;
+                world_to_grid(fx, en.x, en.y, en.z, gx, gy, gz);
+                gc[tid][0] = gx; gc[tid][1] = gy; gc[tid][2] = gz;
+                fr[tid] = b;
+            }
+        }
+        __syncthreads();
+        constexpr int QUADS = kFeat / 4;
+        for (int item = tid; item < GP * QUADS; item += 256) {
+            const int p = item / QUADS, qd = item % QUADS;
+            if (e0 + p >= count) continue;
+            const float4 g = *reinterpret_cast<const float4*>(DF + (size_t)(e0 + p) * kFeat + qd * 4);
+            if (g.x == 0.f && g.y == 0.f && g.z == 0.f && g.w == 0.f) continue;
+            int lvl, c0;
+            feature_quad(qd, lvl, c0);
+            const float3 d = gather_quad_dpos<VT>(P, fr[p], gc[p][0], gc[p][1], gc[p][2], qd, g);
+            // d i / d g = (size - 1) / 2 per level; the level-independent d g / d c is applied once per entry below
+            atomicAdd(&dc[p][0], d.x * (0.5f * (float)(P.lvl_W[lvl] - 1)));
+            atomicAdd(&dc[p][1], d.y * (0.5f * (float)(P.lvl_H[lvl] - 1)));
+            atomicAdd(&dc[p][2], d.z * (0.5f * (float)(P.lvl_D[lvl] - 1)));
+        }
+        __syncthreads();
+        if (tid < 32) {
+            float t[12] = {};
+            const int b = fr[tid];
+            if (b >= 0) {
+                const float4 en = sv.list[e0 + tid];
+                FrameXf fx;
+#pragma unroll
+                for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
+                // grid x / y / z pair with the dhw axes 2 / 1 / 0
+                frame_grad_terms(fx, en.x, en.y, en.z, dc[tid][0] * grid_to_can_scale(fx, 2), dc[tid][1] * grid_to_can_scale(fx, 1),
+                                 dc[tid][2] * grid_to_can_scale(fx, 0), t);
+            }
+            frame_grad_add(acc, b, t, dR, dTh, tid);
+        }
+        __syncthreads();
+    }
+    if (tid < 32) frame_grad_flush(acc, dR, dTh, tid);
+}
+
 // d_vol[b][c][v] += blob[b][v][c] for one level: 32 voxels x 32 channels through shared memory
 __global__ void __launch_bounds__(256) unpack_grad_kernel(const float* __restrict__ blob, float* __restrict__ dvol, int C, size_t nvox, int batch) {
     __shared__ float t[32][33];
@@ -628,18 +693,25 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     a.a = G1; a.b = w.fc1_w; a.c = G0; a.mask = sv.H0;
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
-    if (t.d_vol[0]) {
+    const bool frame_grads = t.d_R || t.d_Th;
+    if (t.d_vol[0] || frame_grads) {
         a.a = G0; a.b = w.fc0_w; a.ldb = kFeat; a.N = kFeat; a.c = DF; a.ldc = kFeat; a.mask = nullptr;
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
+    }
+    const int grid_pts = (int)((pmax + GP - 1) / GP < kGridSMs * 8 ? (pmax + GP - 1) / GP : kGridSMs * 8);
+    if (t.d_vol[0]) {
         // 4. trilinear backward
         cudaMemsetAsync(dblob, 0, gb.floats * 4, stream);
-        const int grid_pts = (int)((pmax + GP - 1) / GP < kGridSMs * 8 ? (pmax + GP - 1) / GP : kGridSMs * 8);
         scatter_kernel<<<grid_pts, 256, 0, stream>>>(p, sv, DF, dblob, gb);
         for (int l = 0; l < 4; ++l) {
             const size_t nvox = (size_t)p.lvl_D[l] * p.lvl_H[l] * p.lvl_W[l];
             dim3 grid((unsigned)((nvox + 31) / 32), (p.lvl_C[l] + 31) / 32, p.batch);
             unpack_grad_kernel<<<grid, 256, 0, stream>>>(dblob + gb.off[l], t.d_vol[l], p.lvl_C[l], nvox, p.batch);
         }
+    }
+    if (frame_grads) {   // 4b. the frame transform's gradients, from the same DF
+        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th);
+        else frame_grad_kernel<__half><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th);
     }
     // 5. weight gradients: dW[out][in] += G^T X, split over the list
     const int splits = 74;      // 2 x 2 tiles x 74 = two CTAs on every SM

@@ -44,6 +44,8 @@ struct TrainBwd {
     const float *d_rgb, *d_depth, *d_acc;
     const nb_decoder_weights* weights; const nb_decoder_weights* grads;
     float* d_vol[4];
+    float *d_R, *d_Th;               // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
+    int volume_dtype;                // of the forward's volume blob (the frame-gradient pass reads it)
     float* workspace;
 };
 

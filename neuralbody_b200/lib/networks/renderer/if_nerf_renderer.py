@@ -36,7 +36,8 @@ class _FusedRender(torch.autograd.Function):
     kernel + activation record, backward = nb_render_bwd.  Differentiable outputs: rgb_map, depth_map,
     acc_map (what lib/train/trainers/if_nerf_clight.py:25-32 and depth/mask losses consume); disp_map and
     weights are returned detached.  Differentiable inputs: the four dense volumes (so gradients keep flowing
-    into the reference's SparseConvNet / code embedding) and the 17 decoder tensors."""
+    into the reference's SparseConvNet / code embedding), the 17 decoder tensors and the frame transform
+    sp_input['R'] / ['Th'] (pose refinement; nb_render_bwd_frame)."""
 
     @staticmethod
     def forward(ctx, renderer, call, *tensors):
@@ -215,8 +216,8 @@ class Renderer:
     def render_rays(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, want_raw=False,
                     out=None, trace=None, masks=None, z_vals=None, want_weights=None):
         """One nb_render_fwd launch for (B,n) rays.  Returns the dict of get_pixel_value.
-        When autograd is recording and any volume / decoder tensor requires grad, the call goes through
-        the exact kernel and `_FusedRender` so that `loss.backward()` works as it does upstream."""
+        When autograd is recording and any volume / decoder tensor or sp_input['R'] / ['Th'] requires grad, the call goes
+        through the training precision and `_FusedRender` so that `loss.backward()` works as it does upstream."""
         cfg = get_active_cfg()
         if int(self._opt("xyz_res", 10)) != 10 or int(self._opt("view_res", 4)) != 4:
             # embedder.py:53-54: the kernels (and view_fc's 346 input columns) are built for PE widths 63 / 27
@@ -230,8 +231,10 @@ class Renderer:
         B, n = int(ray_o.shape[0]), int(ray_o.shape[1])
         S = int(cfg.N_samples) if z_vals is None else int(z_vals.shape[-1])   # z_vals: caller-supplied depths (fine pass, f-4)
         params = self.net.decoder_tensors()
+        frame = [sp_input['R'], sp_input['Th']]
         needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
-                                                  any(v.requires_grad for v in feature_volume))
+                                                  any(v.requires_grad for v in feature_volume) or
+                                                  any(torch.is_tensor(t) and t.requires_grad for t in frame))
         precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
@@ -264,7 +267,7 @@ class Renderer:
         if call["t_rand"] is not None:
             assert tuple(call["t_rand"].shape) == (B, n, S)
         if needs_grad:
-            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params)
+            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame)
             ret = {'rgb_map': rgb, 'disp_map': disp, 'acc_map': acc, 'weights': weights, 'depth_map': depth}
             if want_raw:
                 ret['raw'] = call["raw"]
@@ -399,7 +402,7 @@ class Renderer:
         return out
 
     def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs):
-        """nb_render_bwd: gradients for (volumes..., decoder tensors...) in the order of _FusedRender.apply."""
+        """nb_render_bwd_frame: gradients for (volumes..., decoder tensors..., R, Th) in the order of _FusedRender.apply."""
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         if call.get("save") is None:
             raise RuntimeError("the activation record of this render call was already consumed by a backward pass "
@@ -432,15 +435,25 @@ class Renderer:
             for l in range(capi.NB_NUM_LEVELS):
                 ba.d_volumes[l] = gvols[l].data_ptr() if want_vol else None
             ba.workspace, ba.workspace_bytes = ws.data_ptr(), nbytes
+            # frame transform (pose refinement): fp32 (B,3,3) / (B,3) accumulators, only for the inputs autograd asks about
+            want_R, want_Th = needs[-2], needs[-1]
+            dR = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev) if want_R else None
+            dTh = torch.zeros((B, 3), dtype=torch.float32, device=dev) if want_Th else None
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_render_bwd(C.byref(ba), C.c_void_p(stream)), "nb_render_bwd")
+            capi.check(self.lib.nb_render_bwd_frame(C.byref(ba), _ptr(dR), _ptr(dTh), C.c_void_p(stream)),
+                       "nb_render_bwd_frame")
             # stream-ordered reuse: the next forward / backward on this stream runs after the kernels just enqueued
             self._pool_give("bwd_ws", ws)
             self._pool_give("save", call.pop("save"))
             if not call.get("user_raw"):
                 r = call.pop("raw")
                 self._pool_give("raw", r._base if r._base is not None else r)
-        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)]
+        R, Th = call["sp_input"]['R'], call["sp_input"]['Th']
+        if dR is not None:     # the caller's shape, dtype and device ((B,1,3) or (B,3) for Th)
+            dR = dR.to(device=R.device, dtype=R.dtype).view(R.shape)
+        if dTh is not None:
+            dTh = dTh.to(device=Th.device, dtype=Th.dtype).view(Th.shape)
+        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh]
         return [gr if need else None for gr, need in zip(grads, needs)]
 
     def _weights_struct(self, tensors, latent_index, device):

@@ -1,7 +1,10 @@
 """Diagnostics (GPU): BASELINE config 3 -- one N_rand = 1024 training chunk on the synth-313 body, 64 coarse samples +
-128 importance samples (cfg.render_importance), gradient path on: forward (exact fp32 kernels with activation record,
-coarse + fine) + nb_sample_pdf + backward through both passes.  Prints one JSON line (rays/s for fwd+bwd).
-Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30]"""
+128 importance samples (cfg.render_importance), gradient path on: forward (the training precision cfg.render_train_precision,
+default tc_tf32x3: sample list + TF32x3 GEMM chains, with activation record, coarse + fine) + nb_sample_pdf + backward through
+both passes.  Prints one JSON line (rays/s for fwd+bwd).
+With --frame-grads the same process alternates steps without and with gradients for the frame transform
+(sp_input['R'] / ['Th'] requiring grad, as pose refinement does) and reports both step times.
+Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--precision tc_tf32x3|fp32]"""
 import json
 import os
 import sys
@@ -13,8 +16,15 @@ import torch  # noqa: E402
 
 
 def main():
-    ni = int(sys.argv[1]) if len(sys.argv) > 1 else 128
-    iters = int(sys.argv[2]) if len(sys.argv) > 2 else 30
+    args = sys.argv[1:]
+    frame_grads = "--frame-grads" in args
+    precision = "tc_tf32x3"
+    if "--precision" in args:
+        precision = args[args.index("--precision") + 1]
+        del args[args.index("--precision"):args.index("--precision") + 2]
+    pos = [a for a in args if not a.startswith("--")]
+    ni = int(pos[0]) if len(pos) > 0 else 128
+    iters = int(pos[1]) if len(pos) > 1 else 30
     from oracle import synth
     from neuralbody_b200.lib.config import cfg
     import gpu_utils as G
@@ -26,38 +36,54 @@ def main():
     net, ren = G.make_net_and_renderer(scene)
     cfg.N_samples, cfg.perturb, cfg.white_bkgd, cfg.raw_noise_std, cfg.chunk = 64, 1.0, False, 0, 0
     cfg.render_precision, cfg.render_volume_dtype, cfg.render_importance = "tc_fp16x3", "auto", ni
+    cfg.render_train_precision = precision
     net.train()
     vols = [v.cuda().requires_grad_(True) for v in scene["volumes"]]
     net.set_feature_volume(vols)
     batch = {k: scene[k].cuda() for k in G.BATCH_KEYS}
     sp = ren.prepare_sp_input(batch)
+    pose = dict(batch, R=batch["R"].clone().requires_grad_(True), Th=batch["Th"].clone().requires_grad_(True))
+    sp_pose = ren.prepare_sp_input(pose)
     target = torch.rand((1, 1024, 3), device="cuda")
 
-    def step():
+    def step(with_frame):
         for p in net.parameters():
             p.grad = None
         for v in vols:
             v.grad = None
-        out = ren.get_pixel_value(batch["ray_o"], batch["ray_d"], batch["near"], batch["far"], vols, sp, batch)
+        s, b = (sp_pose, pose) if with_frame else (sp, batch)
+        b["R"].grad = b["Th"].grad = None
+        out = ren.get_pixel_value(b["ray_o"], b["ray_d"], b["near"], b["far"], vols, s, b)
         loss = ((out["rgb_map"] - target) ** 2).mean()
         if "rgb0" in out:
             loss = loss + ((out["rgb0"] - target) ** 2).mean()          # img_loss0, if_nerf_clight.py:29-32
         loss.backward()
-        return float(loss.detach()) if False else None
 
+    modes = (False, True) if frame_grads else (False,)
     for _ in range(5):
-        step()
+        for m in modes:
+            step(m)
     torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
+    # alternate the modes step by step so that both see the same clocks and host load; one event pair per step
+    ev = {m: [] for m in modes}
     for _ in range(iters):
-        step()
-    e1.record()
+        for m in modes:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            step(m)
+            e1.record()
+            ev[m].append((e0, e1))
     torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / iters
-    print(json.dumps({"config": "c3: 1024-ray training chunk, 64 + %d samples, fwd + bwd, exact fp32 kernels" % ni,
-                      "ms_per_step": ms, "rays_per_s_fwd_bwd": 1024 / (ms * 1e-3),
-                      "grad_norm_fc0": float(dict(net.named_parameters())["fc_0.weight"].grad.norm())}))
+    ms = {m: sum(a.elapsed_time(b) for a, b in ev[m]) / iters for m in modes}
+    res = {"config": "c3: 1024-ray training chunk, 64 + %d samples, fwd + bwd, %s" % (ni, precision),
+           "gpu": torch.cuda.get_device_name(0),
+           "ms_per_step": ms[False], "rays_per_s_fwd_bwd": 1024 / (ms[False] * 1e-3),
+           "grad_norm_fc0": float(dict(net.named_parameters())["fc_0.weight"].grad.norm())}
+    if frame_grads:
+        res["ms_per_step_frame_grads"] = ms[True]
+        res["frame_grads_overhead_ms"] = ms[True] - ms[False]
+        res["dR_norm"], res["dTh_norm"] = float(pose["R"].grad.norm()), float(pose["Th"].grad.norm())
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":
