@@ -311,6 +311,14 @@ int    nb_render_bwd(const nb_render_bwd_args* args, void* stream);
  * precisions; it reads the volume blob the forward gathered from.  nb_render_bwd(args, stream) is
  * nb_render_bwd_frame(args, NULL, NULL, stream) and enqueues no frame-gradient work.  No extra workspace. */
 int    nb_render_bwd_frame(const nb_render_bwd_args* args, float* d_R, float* d_Th, void* stream);
+/* nb_render_bwd_frame plus the gradients of the rays the forward call read (nb_render_args.ray_o / .ray_d): what camera
+ * refinement needs, i.e. upstream autograd through pts = ray_o + ray_d * z (if_clight_renderer.py:25), the view direction
+ * ray_d / |ray_d| (:68) and PE(world xyz) into view_fc (latent_xyzc.py:115), the canonical transform into grid_sample, and
+ * dists * |ray_d| in raw2outputs (nerf_net_utils.py:28).  d_ray_o, d_ray_d: device (B,n,3) fp32; both are ACCUMULATED into
+ * and either may be NULL.  The depths z are not differentiated (upstream never differentiates near / far); after a z_vals
+ * (fine-pass) forward they are taken as given.  Both training precisions.  nb_render_bwd_frame(args, dR, dTh, stream) is
+ * nb_render_bwd_rays(args, dR, dTh, NULL, NULL, stream) and enqueues no ray-gradient work.  No extra workspace. */
+int    nb_render_bwd_rays(const nb_render_bwd_args* args, float* d_R, float* d_Th, float* d_ray_o, float* d_ray_d, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Diagnostics.

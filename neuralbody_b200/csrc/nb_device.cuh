@@ -304,6 +304,19 @@ __device__ __forceinline__ void positional_embed(float x, float y, float z, Stor
     }
 }
 
+// Backward of positional_embed<L> for input axis a: d = d loss / d(encoding), enc = the encoding itself (its saved sin / cos),
+// both in the layout above.  d sin(2^l x) = 2^l cos(2^l x) dx, d cos(2^l x) = -2^l sin(2^l x) dx.
+template <int L>
+__device__ __forceinline__ float positional_embed_bwd(const float* d, const float* enc, int a) {
+    float v = d[a], f = 1.f;
+#pragma unroll
+    for (int l = 0; l < L; ++l) {
+        v = fmaf(f, fmaf(d[3 + 6 * l + a], enc[6 + 6 * l + a], -d[6 + 6 * l + a] * enc[3 + 6 * l + a]), v);
+        f *= 2.f;
+    }
+    return v;
+}
+
 // Same layout, cheaper: an accurate sincosf only every ANCHOR-th octave, the octaves in between by the
 // double-angle recurrence (sin 2a = 2 sin a cos a, cos 2a = 1 - 2 sin^2 a).  Each doubling at most doubles the
 // absolute error, so with ANCHOR <= 5 the values stay within ~2e-6 of sincosf -- far below the fp16 rounding

@@ -1,6 +1,6 @@
 // Backward of the fused render (nb_render_bwd): gradients of rgb_map / depth_map / acc_map with respect to
 // the four dense feature volumes, every decoder parameter and the latent table; nb_render_bwd_frame adds the frame
-// transform R / Th.
+// transform R / Th, nb_render_bwd_rays also the rays ray_o / ray_d.
 //
 // Upstream this is PyTorch autograd through raw2outputs (nerf_net_utils.py:6-51), the eight Conv1d layers
 // and F.grid_sample (latent_xyzc.py:62-126), driven by Trainer.train (lib/train/trainers/trainer.py:46-53).
@@ -11,6 +11,7 @@
 //                             features, then the trilinear scatter-add into the NCDHW volume grads
 //   3. wgrad_kernel (x6), colsum_kernel, view_wgrad_kernel     weight / bias gradients (split over points)
 //   4. unfold_* kernels       gradients of the folded Wc / bc back to feature_fc, latent_fc, view_fc, latent
+//   5. ray gradients only:    pe_grad_kernel (the positional encodings' part per point), ray_grad_kernel (per ray)
 // Training chunks are small (N_rand = 1024 rays), so this path is sized for correctness and simplicity:
 // fp32 FFMA, no tensor cores; the forward hot path is untouched.
 #include "nb_device.cuh"
@@ -30,6 +31,7 @@ struct BwdParams {
     float *d_R, *d_Th;              // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
     float* d_raw_out;               // composite backward writes d(rgb logits, sigma) of sample i at d_raw_out + i * d_raw_stride
     int d_raw_stride;
+    float *d_ray_o, *d_ray_d;       // (B,n,3) ray gradients, accumulated into; either may be null
 };
 
 constexpr int kBwdMaxSamples = 256;     // coarse + importance samples of a fine pass (64 + 128) fit
@@ -97,6 +99,121 @@ __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdP
     }
 }
 
+// Ray gradients (nb_render_bwd_rays), one WARP per ray, after the per-sample records are complete: rec + i * rec_stride holds
+// sample i's [d loss / d(world point) 3 | d loss / d(view direction) 3] (zero for a skipped sample).  With p_i = o + z_i d,
+// u = d / |d| and dists_i = delta_i |d| (nerf_net_utils.py:28):
+//   d o += sum_i g_i,   d d += sum_i z_i g_i + (du - u (u . du)) / |d| + u sum_i dL/d dists_i delta_i,
+// where du = sum_i du_i and dL/d dists_i = dalpha_i relu(sigma_i) e_i; z, dist and the T / U recurrences are re-derived exactly
+// as composite_bwd_kernel does.  z is not differentiated (near / far and z_vals are not inputs of the gradient).
+__global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams Q, const float* __restrict__ rec, int rec_stride) {
+    __shared__ float s_alpha[CB_WARPS][kBwdMaxSamples], s_f[CB_WARPS][kBwdMaxSamples], s_g[CB_WARPS][kBwdMaxSamples],
+        s_T[CB_WARPS][kBwdMaxSamples], s_U[CB_WARPS][kBwdMaxSamples], s_z[CB_WARPS][kBwdMaxSamples + 1];
+    const RenderParams& P = Q.f;
+    const int S = P.n_samples;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const size_t ri = (size_t)blockIdx.x * CB_WARPS + warp;
+    if (ri >= (size_t)P.batch * P.n_rays) return;
+    const float near = P.near[ri], far = P.far[ri];
+    const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
+    const float nrm = ray_norm(dx, dy, dz);
+    const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
+    const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
+    const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
+    float dC[3] = {0.f, 0.f, 0.f};
+    if (Q.d_rgb) { dC[0] = Q.d_rgb[ri * 3]; dC[1] = Q.d_rgb[ri * 3 + 1]; dC[2] = Q.d_rgb[ri * 3 + 2]; }
+    const float dD = Q.d_depth ? Q.d_depth[ri] : 0.f;
+    float dA = Q.d_acc ? Q.d_acc[ri] : 0.f;
+    if (P.white_bkgd) dA -= dC[0] + dC[1] + dC[2];
+    for (int s = lane; s < S; s += 32) s_z[warp][s] = z_sample(near, far, P.t_vals, s, S, tr, zu);
+    __syncwarp();
+    for (int s = lane; s < S; s += 32) {
+        const float4 rw = raw[s];
+        const float z = s_z[warp][s];
+        const float dist = ((s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f) * nrm;
+        const float alpha = 1.f - expf(-fmaxf(rw.w, 0.f) * dist);
+        const float c0 = 1.f / (1.f + expf(-rw.x)), c1 = 1.f / (1.f + expf(-rw.y)), c2 = 1.f / (1.f + expf(-rw.z));
+        s_alpha[warp][s] = alpha;
+        s_f[warp][s] = 1.f - alpha + 1e-10f;
+        s_g[warp][s] = dC[0] * c0 + dC[1] * c1 + dC[2] * c2 + dD * z + dA;
+    }
+    __syncwarp();
+    if (lane == 0) {
+        float T = 1.f;
+        for (int s = 0; s < S; ++s) { s_T[warp][s] = T; T *= s_f[warp][s]; }
+        float U = 0.f;
+        for (int s = S - 1; s >= 0; --s) { s_U[warp][s] = U; U = s_g[warp][s] * s_alpha[warp][s] + s_f[warp][s] * U; }
+    }
+    __syncwarp();
+    float go[3] = {0.f, 0.f, 0.f}, gd[3] = {0.f, 0.f, 0.f}, du[3] = {0.f, 0.f, 0.f}, dn = 0.f;
+    for (int s = lane; s < S; s += 32) {
+        const float z = s_z[warp][s];
+        const float delta = (s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f;
+        const float sg = fmaxf(raw[s].w, 0.f);
+        const float e = expf(-sg * (delta * nrm));
+        const float Ti = s_T[warp][s];
+        const float dalpha = s_g[warp][s] * Ti - Ti * s_U[warp][s];
+        dn = fmaf(dalpha * sg * e, delta, dn);          // a skipped (empty) sample has sigma < 0: no term
+        const float* r = rec + (ri * S + s) * rec_stride;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { go[k] += r[k]; gd[k] = fmaf(z, r[k], gd[k]); du[k] += r[3 + k]; }
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { go[k] = warp_sum(go[k]); gd[k] = warp_sum(gd[k]); du[k] = warp_sum(du[k]); }
+    dn = warp_sum(dn);
+    if (lane == 0) {
+        if (Q.d_ray_o) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) Q.d_ray_o[ri * 3 + k] += go[k];
+        }
+        if (Q.d_ray_d) {
+            const float u[3] = {__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm)};
+            const float udu = fmaf(u[2], du[2], fmaf(u[1], du[1], u[0] * du[0]));
+#pragma unroll
+            for (int k = 0; k < 3; ++k) Q.d_ray_d[ri * 3 + k] += gd[k] + fmaf(-u[k], udu, du[k]) / nrm + u[k] * dn;
+        }
+    }
+}
+
+// fp32 path, ray gradients: per point, d(positional encodings) = view_fc[:, 256:346]^T d_wpre (the colour layer's input
+// columns [PE(viewdir) 27 | PE(xyz) 63], latent_xyzc.py:104), back through both encodings -> rec + point * rec_stride =
+// [d / d(world point) from PE(xyz) 3 | d / d(view direction) 3].  One warp per point; PE(xyz) is read from the activation
+// record, PE(viewdir) recomputed as the forward computes it.
+constexpr int PG_WARPS = 8;
+__global__ void __launch_bounds__(PG_WARPS * 32) pe_grad_kernel(const BwdParams Q, float* __restrict__ rec, int rec_stride) {
+    __shared__ float s_d[PG_WARPS][96], s_pe[PG_WARPS][kViewPE];
+    const RenderParams& P = Q.f;
+    const int S = P.n_samples;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const size_t npts = (size_t)P.batch * P.n_rays * S;
+    const float* vw = Q.w.view_w + kHidden;          // (128, 346) row-major: column 256 + j
+    for (size_t g = (size_t)blockIdx.x * PG_WARPS + warp; g < npts; g += (size_t)gridDim.x * PG_WARPS) {
+        const size_t ri = g / S;
+        if (lane == 0) {
+            const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
+            const float nrm = ray_norm(dx, dy, dz);
+            positional_embed<4>(__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm), [&](int j, float v) { s_pe[warp][j] = v; });
+        }
+        const float* dw = Q.ws + g * kGradDim + kGradW;
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+        for (int n = 0; n < kColor; ++n) {
+            const float d = dw[n];
+            if (d == 0.f) continue;                      // relu: same address for the whole warp, so a uniform branch
+            a0 = fmaf(d, vw[n * 346 + lane], a0);
+            a1 = fmaf(d, vw[n * 346 + 32 + lane], a1);
+            if (lane < kViewPE + kXyzPE - 64) a2 = fmaf(d, vw[n * 346 + 64 + lane], a2);
+        }
+        s_d[warp][lane] = a0; s_d[warp][32 + lane] = a1; s_d[warp][64 + lane] = a2;
+        __syncwarp();
+        if (lane < 6) {
+            const int ax = lane % 3;
+            const float v = lane < 3 ? positional_embed_bwd<10>(&s_d[warp][kViewPE], Q.save + g * kSaveDim + kSaveH2 + kHidden, ax)
+                                     : positional_embed_bwd<4>(&s_d[warp][0], &s_pe[warp][0], ax);
+            rec[g * rec_stride + lane] = v;
+        }
+        __syncwarp();
+    }
+}
+
 // ------------------------------------------------------------------------------------------ 2. decoder dgrad
 constexpr int TP = 64, NT = 256, LDX = 356, LDY = 324, KC = 8;
 
@@ -136,6 +253,26 @@ __device__ __forceinline__ void gemm_tile(const float* __restrict__ in, float* _
     __syncthreads();
 }
 
+// Whole warp, ray gradients: adds each lane's d loss / d(world point) g to its ray ri (~0u: none) -- d ray_o += g,
+// d ray_d += z g.  The lanes of one ray are summed first: one atomic per ray and element (a warp holds consecutive points).
+__device__ __forceinline__ void ray_pos_add(unsigned int ri, float z, const float (&g)[3], float* __restrict__ d_ray_o,
+                                            float* __restrict__ d_ray_d, int lane) {
+    for (;;) {
+        const unsigned int rm = __reduce_min_sync(0xffffffffu, ri);
+        if (rm == ~0u) break;
+        const bool mine = ri == rm;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const float so = warp_sum(mine ? g[k] : 0.f), sd = warp_sum(mine ? z * g[k] : 0.f);
+            if (lane == 0 && d_ray_o) atomicAdd(d_ray_o + (size_t)rm * 3 + k, so);
+            if (lane == 0 && d_ray_d) atomicAdd(d_ray_d + (size_t)rm * 3 + k, sd);
+        }
+        if (mine) ri = ~0u;
+    }
+}
+
+// RAYS: also the grid part of the ray gradients (nb_render_bwd_rays), from the same d loss / d(canonical point) as dR / dTh
+template <bool RAYS>
 __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q) {
     extern __shared__ __align__(16) float smem[];
     float* X = smem;                    // [64][356]
@@ -146,7 +283,7 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
     const size_t npts = (size_t)P.batch * P.n_rays * S;
     const int tid = threadIdx.x;
     const float* wf = P.wf32;
-    const bool frame_grads = Q.d_R || Q.d_Th;
+    const bool frame_grads = RAYS || Q.d_R || Q.d_Th;   // any gradient with respect to the sample position
     FrameGradAcc acc;                   // warp 0: running per-frame sums of dR / dTh
     for (size_t tile = blockIdx.x; tile * TP < npts; tile += gridDim.x) {
         const size_t p0 = tile * TP;
@@ -259,7 +396,15 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                         frame_grad_terms(fx, y[12], y[13], y[14], dcx * grid_to_can_scale(fx, 2), dcy * grid_to_can_scale(fx, 1),
                                          dcz * grid_to_can_scale(fx, 0), t);
                     }
-                    frame_grad_add(acc, b, t, Q.d_R, Q.d_Th, tid);
+                    if (!RAYS || Q.d_R || Q.d_Th) frame_grad_add(acc, b, t, Q.d_R, Q.d_Th, tid);
+                    if constexpr (RAYS) {   // d loss / d(world point) through the grid: R dc = -(the dTh term)
+                        const size_t g = gp(32 * h + tid);
+                        const size_t ri = g / S;
+                        const float gw[3] = {-t[9], -t[10], -t[11]};
+                        const float z = b < 0 ? 0.f : z_sample(P.near[ri], P.far[ri], P.t_vals, (int)(g % S), S,
+                                                               P.t_rand ? P.t_rand + ri * S : nullptr, P.z_user ? P.z_user + ri * S : nullptr);
+                        ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
+                    }
                 }
             }
         }
@@ -452,6 +597,15 @@ void launch_composite_bwd(const RenderParams& p, const float* raw, const float* 
     bwd::composite_bwd_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q);
 }
 
+void launch_ray_grad(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
+                     const float* rec, int rec_stride, float* d_ray_o, float* d_ray_d, cudaStream_t stream) {
+    bwd::BwdParams Q{};
+    Q.f = p; Q.raw = raw; Q.d_rgb = d_rgb; Q.d_depth = d_depth; Q.d_acc = d_acc;
+    Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
+    const size_t nrays = (size_t)p.batch * p.n_rays;
+    bwd::ray_grad_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
+}
+
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
                   float* u, float* du, cudaStream_t stream) {
     bwd::Unfold U;
@@ -497,6 +651,10 @@ extern "C" size_t nb_render_bwd_workspace_bytes_for(const nb_render_args* f) {
 extern "C" int nb_render_bwd(const nb_render_bwd_args* a, void* stream) { return nb_render_bwd_frame(a, nullptr, nullptr, stream); }
 
 extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, float* d_Th, void* stream) {
+    return nb_render_bwd_rays(a, d_R, d_Th, nullptr, nullptr, stream);
+}
+
+extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float* d_Th, float* d_ray_o, float* d_ray_d, void* stream) {
     if (!a || !a->fwd || !a->save || !a->raw || !a->workspace || !a->weights || !a->grads) {
         set_error("nb_render_bwd: null argument");
         return NB_ERR_BAD_ARG;
@@ -513,7 +671,7 @@ extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, floa
         t.save = a->save; t.raw = a->raw; t.d_rgb = a->d_rgb_map; t.d_depth = a->d_depth_map; t.d_acc = a->d_acc_map;
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
         for (int l = 0; l < 4; ++l) t.d_vol[l] = a->d_volumes[l];
-        t.d_R = d_R; t.d_Th = d_Th; t.volume_dtype = f->volume_dtype;
+        t.d_R = d_R; t.d_Th = d_Th; t.d_ray_o = d_ray_o; t.d_ray_d = d_ray_d; t.volume_dtype = f->volume_dtype;
         return launch_train_bwd(p, t, (cudaStream_t)stream);
     }
     if (f->precision != NB_PRECISION_FP32 || f->volume_dtype != NB_DTYPE_F32) {
@@ -533,6 +691,8 @@ extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, floa
     Q.w = *a->weights;
     for (int l = 0; l < 4; ++l) Q.d_vol[l] = a->d_volumes[l];
     Q.d_R = d_R; Q.d_Th = d_Th;
+    Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
+    const bool ray_grads = d_ray_o || d_ray_d;
     cudaStream_t s = (cudaStream_t)stream;
     const size_t nrays = (size_t)f->batch * f->n_rays, npts = nrays * f->n_samples;
     if (npts == 0) return NB_OK;
@@ -541,9 +701,15 @@ extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, floa
     bwd::composite_bwd_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, s>>>(Q);
 
     const size_t smem = ((size_t)bwd::TP * bwd::LDX + (size_t)bwd::TP * bwd::LDY + (size_t)bwd::KC * kFeat) * 4;
-    cudaFuncSetAttribute(bwd::decoder_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const size_t ntiles = (npts + bwd::TP - 1) / bwd::TP;
-    bwd::decoder_dgrad_kernel<<<(unsigned)(ntiles < kGridSMs ? ntiles : kGridSMs), bwd::NT, smem, s>>>(Q);
+    const unsigned dgrad_grid = (unsigned)(ntiles < kGridSMs ? ntiles : kGridSMs);
+    if (ray_grads) {   // + the grid part of the ray gradients, added straight into d_ray_o / d_ray_d
+        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        bwd::decoder_dgrad_kernel<true><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
+    } else {
+        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        bwd::decoder_dgrad_kernel<false><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
+    }
 
     // scratch after the per-point region
     float* extra = Q.ws + npts * kGradDim;
@@ -580,6 +746,13 @@ extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, floa
 
     st = launch_unfold(*a->weights, g, dWcx, dbc, T, dT, u, du, s);
     if (st != NB_OK) return st;
+    if (ray_grads) {   // the encodings' part per point into the d_h1pre columns (read by the weight / bias gradients above), then per ray
+        float* rec = Q.ws + kGradH1;
+        bwd::pe_grad_kernel<<<(unsigned)((npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS < (size_t)kGridSMs * 16
+                                             ? (npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS : (size_t)kGridSMs * 16),
+                              bwd::PG_WARPS * 32, 0, s>>>(Q, rec, kGradDim);
+        launch_ray_grad(p, a->raw, a->d_rgb_map, a->d_depth_map, a->d_acc_map, rec, kGradDim, d_ray_o, d_ray_d, s);
+    }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_render_bwd: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     return NB_OK;

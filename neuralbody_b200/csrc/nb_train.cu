@@ -16,7 +16,9 @@
 //             -> scatter_kernel (trilinear backward, 16-byte vector atomics into a channels-last gradient blob, then one
 //             transposing add into the NCDHW gradients autograd expects) ; frame_grad_kernel (only when the frame
 //             transform's gradients are asked for) ; 4 x gemm (wgrad, split over the list, fp32 atomics)
-//             ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu).
+//             ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu) ; only when the rays'
+//             gradients are asked for: gemm (the encodings' input gradient), frame_grad_kernel<VT, true> (per-sample
+//             records, and dR / dTh in place of the earlier frame pass), ray_grad_kernel (nb_render_bwd.cu).
 //
 // gemm_tf32x3_kernel: C[128 x <=256 tile] = epilogue(A B^T), fp32 in HBM on both sides.  Operands are split on the way into
 // shared memory into hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi, and three wgmma tf32 passes
@@ -450,11 +452,19 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
 // scatter_kernel; each (entry, quad) adds sum_c dF_c d f_c / d i, scaled to d / d(canonical point), into its entry's shared
 // slot; warp 0 then turns the 32 entries into dR / dTh terms and sums them per frame (one atomic per CTA, frame and element:
 // the list is frame-major and each CTA walks it in order).  Reads the packed blob the forward gathered from.
-template <typename VT>
-__global__ void __launch_bounds__(256) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
-                                                         float* __restrict__ dR, float* __restrict__ dTh) {
+// RAYS (nb_render_bwd_rays): also each entry's ray-gradient record rec + id * kRayRec = [d loss / d(world point) 3 |
+// d loss / d(view direction) 3]: the grid part R dc plus the two encodings' parts, from dPE (count x kPECols, the colour
+// layer's input gradient in columns kXyzCol..) and the sin / cos the forward saved in H2X.  dR / dTh may both be null then.
+constexpr int kPECols = kH2X - kXyzCol;     // [PE(xyz) 63 | 0 | PE(view) 27 | 0 x 5]
+constexpr int kRayRec = 8;
+// (RAYS: at least 2 CTAs per SM, so ptxas does not squeeze it into 64 registers and spill; 0 = no minimum, as before)
+template <typename VT, bool RAYS>
+__global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
+                                                         float* __restrict__ dR, float* __restrict__ dTh, const float* __restrict__ dPE,
+                                                         float* __restrict__ rec) {
     __shared__ float gc[GP][3], dc[GP][3];
     __shared__ int fr[GP];
+    __shared__ float pe[RAYS ? 2 : 1][GP][3];   // RAYS: [PE(xyz) | PE(view)][entry][axis]
     const unsigned int count = *sv.count;
     const unsigned int spf = (unsigned int)P.n_rays * P.n_samples;
     const int tid = threadIdx.x;
@@ -490,6 +500,18 @@ __global__ void __launch_bounds__(256) frame_grad_kernel(const __grid_constant__
             atomicAdd(&dc[p][1], d.y * (0.5f * (float)(P.lvl_H[lvl] - 1)));
             atomicAdd(&dc[p][2], d.z * (0.5f * (float)(P.lvl_D[lvl] - 1)));
         }
+        if constexpr (RAYS) {   // (encoding, entry, axis) items
+            if (tid < 2 * GP * 3) {
+                const int v = tid / (GP * 3), p = tid % (GP * 3) / 3, ax = tid % 3;
+                float r = 0.f;
+                if (e0 + p < count) {
+                    const float* d = dPE + (size_t)(e0 + p) * kPECols + (v ? kViewCol - kXyzCol : 0);
+                    const float* enc = sv.H2X + (size_t)(e0 + p) * kH2X + (v ? kViewCol : kXyzCol);
+                    r = v ? positional_embed_bwd<4>(d, enc, ax) : positional_embed_bwd<10>(d, enc, ax);
+                }
+                pe[v][p][ax] = r;
+            }
+        }
         __syncthreads();
         if (tid < 32) {
             float t[12] = {};
@@ -502,8 +524,13 @@ __global__ void __launch_bounds__(256) frame_grad_kernel(const __grid_constant__
                 // grid x / y / z pair with the dhw axes 2 / 1 / 0
                 frame_grad_terms(fx, en.x, en.y, en.z, dc[tid][0] * grid_to_can_scale(fx, 2), dc[tid][1] * grid_to_can_scale(fx, 1),
                                  dc[tid][2] * grid_to_can_scale(fx, 0), t);
+                if constexpr (RAYS) {   // the grid part R dc is -(the dTh term)
+                    float* r = rec + (size_t)(__float_as_uint(en.w) & kListIdMask) * kRayRec;
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) { r[k] = pe[0][tid][k] - t[9 + k]; r[3 + k] = pe[1][tid][k]; }
+                }
             }
-            frame_grad_add(acc, b, t, dR, dTh, tid);
+            if (!RAYS || dR || dTh) frame_grad_add(acc, b, t, dR, dTh, tid);
         }
         __syncthreads();
     }
@@ -693,8 +720,8 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     a.a = G1; a.b = w.fc1_w; a.c = G0; a.mask = sv.H0;
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
-    const bool frame_grads = t.d_R || t.d_Th;
-    if (t.d_vol[0] || frame_grads) {
+    const bool frame_grads = t.d_R || t.d_Th, ray_grads = t.d_ray_o || t.d_ray_d;
+    if (t.d_vol[0] || frame_grads || ray_grads) {
         a.a = G0; a.b = w.fc0_w; a.ldb = kFeat; a.N = kFeat; a.c = DF; a.ldc = kFeat; a.mask = nullptr;
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     }
@@ -709,9 +736,9 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
             unpack_grad_kernel<<<grid, 256, 0, stream>>>(dblob + gb.off[l], t.d_vol[l], p.lvl_C[l], nvox, p.batch);
         }
     }
-    if (frame_grads) {   // 4b. the frame transform's gradients, from the same DF
-        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th);
-        else frame_grad_kernel<__half><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th);
+    if (frame_grads && !ray_grads) {   // 4b. the frame transform's gradients, from the same DF (with ray gradients: step 8)
+        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
+        else frame_grad_kernel<__half, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
     }
     // 5. weight gradients: dW[out][in] += G^T X, split over the list
     const int splits = 74;      // 2 x 2 tiles x 74 = two CTAs on every SM
@@ -737,6 +764,18 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     finish_color_kernel<<<(nfin + 255) / 256, 256, 0, stream>>>(dwcol, dbias3, p.batch, dWcx, dbc, G_(g.view_w), G_(g.alpha_w), G_(g.alpha_b));
     st = launch_unfold(w, g, dWcx, dbc, T, dT, u, du, stream);
     if (st != NB_OK) return st;
+    if (ray_grads) {
+        // 8. ray gradients (+ dR / dTh when asked for), in G2 / G1, which steps 5 and 6 were the last to read: the encodings'
+        // input gradient dPE = G3 Wcol[:, 256:352]^T, then the per-entry records by sample id (skipped samples: 0), then per ray
+        float* dPE = G2;
+        float* rec = G1;
+        a.a = G3; a.lda = kWS; a.b = sv.wcol + kXyzCol; a.ldb = kH2X; a.N = kPECols; a.K = kWS; a.c = dPE; a.ldc = kPECols; a.mask = nullptr;
+        if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
+        cudaMemsetAsync(rec, 0, pmax * kRayRec * 4, stream);
+        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
+        else frame_grad_kernel<__half, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
+        launch_ray_grad(p, t.raw, t.d_rgb, t.d_depth, t.d_acc, rec, kRayRec, t.d_ray_o, t.d_ray_d, stream);
+    }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("train bwd launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     return NB_OK;

@@ -45,6 +45,7 @@ struct TrainBwd {
     const nb_decoder_weights* weights; const nb_decoder_weights* grads;
     float* d_vol[4];
     float *d_R, *d_Th;               // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
+    float *d_ray_o, *d_ray_d;        // (B,n,3) ray gradients, accumulated into; either may be null
     int volume_dtype;                // of the forward's volume blob (the frame-gradient pass reads it)
     float* workspace;
 };
@@ -62,6 +63,10 @@ void launch_classify(const RenderParams& p, cudaStream_t stream);    // nb_rende
 void launch_composite(const RenderParams& p, cudaStream_t stream);   // nb_render_tc_list.cu
 void launch_composite_bwd(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
                           float* d_raw_out, int d_raw_stride, cudaStream_t stream);   // nb_render_bwd.cu
+// per ray: the per-sample records rec + i * rec_stride = [d / d(world point) 3 | d / d(view direction) 3] plus the compositing
+// term -> d_ray_o / d_ray_d (accumulated into; either may be null)                                              nb_render_bwd.cu
+void launch_ray_grad(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
+                     const float* rec, int rec_stride, float* d_ray_o, float* d_ray_d, cudaStream_t stream);
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
                   float* u, float* du, cudaStream_t stream);                          // nb_render_bwd.cu
 

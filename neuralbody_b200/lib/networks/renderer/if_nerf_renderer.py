@@ -36,8 +36,8 @@ class _FusedRender(torch.autograd.Function):
     kernel + activation record, backward = nb_render_bwd.  Differentiable outputs: rgb_map, depth_map,
     acc_map (what lib/train/trainers/if_nerf_clight.py:25-32 and depth/mask losses consume); disp_map and
     weights are returned detached.  Differentiable inputs: the four dense volumes (so gradients keep flowing
-    into the reference's SparseConvNet / code embedding), the 17 decoder tensors and the frame transform
-    sp_input['R'] / ['Th'] (pose refinement; nb_render_bwd_frame)."""
+    into the reference's SparseConvNet / code embedding), the 17 decoder tensors, the frame transform
+    sp_input['R'] / ['Th'] (pose refinement) and the rays ray_o / ray_d (camera refinement; nb_render_bwd_rays)."""
 
     @staticmethod
     def forward(ctx, renderer, call, *tensors):
@@ -216,8 +216,8 @@ class Renderer:
     def render_rays(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, want_raw=False,
                     out=None, trace=None, masks=None, z_vals=None, want_weights=None):
         """One nb_render_fwd launch for (B,n) rays.  Returns the dict of get_pixel_value.
-        When autograd is recording and any volume / decoder tensor or sp_input['R'] / ['Th'] requires grad, the call goes
-        through the training precision and `_FusedRender` so that `loss.backward()` works as it does upstream."""
+        When autograd is recording and any volume / decoder tensor, sp_input['R'] / ['Th'] or ray_o / ray_d requires grad, the
+        call goes through the training precision and `_FusedRender` so that `loss.backward()` works as it does upstream."""
         cfg = get_active_cfg()
         if int(self._opt("xyz_res", 10)) != 10 or int(self._opt("view_res", 4)) != 4:
             # embedder.py:53-54: the kernels (and view_fc's 346 input columns) are built for PE widths 63 / 27
@@ -234,7 +234,8 @@ class Renderer:
         frame = [sp_input['R'], sp_input['Th']]
         needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
                                                   any(v.requires_grad for v in feature_volume) or
-                                                  any(torch.is_tensor(t) and t.requires_grad for t in frame))
+                                                  any(torch.is_tensor(t) and t.requires_grad for t in frame) or
+                                                  ray_o.requires_grad or ray_d.requires_grad)
         precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
@@ -247,7 +248,8 @@ class Renderer:
             t_rand = self._draw_t_rand(B, n, S, dev)
         call = {
             "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": self._volume_dtype(precision),
-            "ray_o": _f32c(ray_o, dev), "ray_d": _f32c(ray_d, dev), "near": _f32c(near, dev), "far": _f32c(far, dev),
+            "ray_o": _f32c(ray_o.detach(), dev), "ray_d": _f32c(ray_d.detach(), dev), "near": _f32c(near, dev), "far": _f32c(far, dev),
+            "ray_like": [(t.shape, t.dtype, t.device) for t in (ray_o, ray_d)],
             "sp_input": sp_input, "t_rand": None if t_rand is None else _f32c(t_rand, dev), "white_bkgd": bool(cfg.white_bkgd),
             "z_vals": None if z_vals is None else _f32c(z_vals.detach(), dev),
             "feature_volume": list(feature_volume), "want_raw": want_raw or needs_grad, "user_raw": bool(want_raw), "out": out, "trace": trace,
@@ -267,7 +269,7 @@ class Renderer:
         if call["t_rand"] is not None:
             assert tuple(call["t_rand"].shape) == (B, n, S)
         if needs_grad:
-            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame)
+            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame, ray_o, ray_d)
             ret = {'rgb_map': rgb, 'disp_map': disp, 'acc_map': acc, 'weights': weights, 'depth_map': depth}
             if want_raw:
                 ret['raw'] = call["raw"]
@@ -402,7 +404,8 @@ class Renderer:
         return out
 
     def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs):
-        """nb_render_bwd_frame: gradients for (volumes..., decoder tensors..., R, Th) in the order of _FusedRender.apply."""
+        """nb_render_bwd_rays: gradients for (volumes..., decoder tensors..., R, Th, ray_o, ray_d) in the order of
+        _FusedRender.apply."""
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         if call.get("save") is None:
             raise RuntimeError("the activation record of this render call was already consumed by a backward pass "
@@ -436,12 +439,14 @@ class Renderer:
                 ba.d_volumes[l] = gvols[l].data_ptr() if want_vol else None
             ba.workspace, ba.workspace_bytes = ws.data_ptr(), nbytes
             # frame transform (pose refinement): fp32 (B,3,3) / (B,3) accumulators, only for the inputs autograd asks about
-            want_R, want_Th = needs[-2], needs[-1]
+            want_R, want_Th = needs[-4], needs[-3]
             dR = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev) if want_R else None
             dTh = torch.zeros((B, 3), dtype=torch.float32, device=dev) if want_Th else None
+            # rays (camera refinement): fp32 (B,n,3) accumulators, likewise
+            drays = [torch.zeros((B, n, 3), dtype=torch.float32, device=dev) if want else None for want in needs[-2:]]
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_render_bwd_frame(C.byref(ba), _ptr(dR), _ptr(dTh), C.c_void_p(stream)),
-                       "nb_render_bwd_frame")
+            capi.check(self.lib.nb_render_bwd_rays(C.byref(ba), _ptr(dR), _ptr(dTh), _ptr(drays[0]), _ptr(drays[1]),
+                                                   C.c_void_p(stream)), "nb_render_bwd_rays")
             # stream-ordered reuse: the next forward / backward on this stream runs after the kernels just enqueued
             self._pool_give("bwd_ws", ws)
             self._pool_give("save", call.pop("save"))
@@ -453,7 +458,9 @@ class Renderer:
             dR = dR.to(device=R.device, dtype=R.dtype).view(R.shape)
         if dTh is not None:
             dTh = dTh.to(device=Th.device, dtype=Th.dtype).view(Th.shape)
-        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh]
+        drays = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])   # the caller's shape, dtype and device
+                 for d, like in zip(drays, call["ray_like"])]
+        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh] + drays
         return [gr if need else None for gr, need in zip(grads, needs)]
 
     def _weights_struct(self, tensors, latent_index, device):

@@ -3,8 +3,9 @@
 default tc_tf32x3: sample list + TF32x3 GEMM chains, with activation record, coarse + fine) + nb_sample_pdf + backward through
 both passes.  Prints one JSON line (rays/s for fwd+bwd).
 With --frame-grads the same process alternates steps without and with gradients for the frame transform
-(sp_input['R'] / ['Th'] requiring grad, as pose refinement does) and reports both step times.
-Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--precision tc_tf32x3|fp32]"""
+(sp_input['R'] / ['Th'] requiring grad, as pose refinement does) and reports both step times; --ray-grads does the same
+with ray_o / ray_d requiring grad (camera refinement).
+Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--ray-grads] [--precision tc_tf32x3|fp32]"""
 import json
 import os
 import sys
@@ -18,6 +19,7 @@ import torch  # noqa: E402
 def main():
     args = sys.argv[1:]
     frame_grads = "--frame-grads" in args
+    ray_grads = "--ray-grads" in args
     precision = "tc_tf32x3"
     if "--precision" in args:
         precision = args[args.index("--precision") + 1]
@@ -44,22 +46,23 @@ def main():
     sp = ren.prepare_sp_input(batch)
     pose = dict(batch, R=batch["R"].clone().requires_grad_(True), Th=batch["Th"].clone().requires_grad_(True))
     sp_pose = ren.prepare_sp_input(pose)
+    cam = dict(batch, ray_o=batch["ray_o"].clone().requires_grad_(True), ray_d=batch["ray_d"].clone().requires_grad_(True))
     target = torch.rand((1, 1024, 3), device="cuda")
 
-    def step(with_frame):
+    def step(mode):
         for p in net.parameters():
             p.grad = None
         for v in vols:
             v.grad = None
-        s, b = (sp_pose, pose) if with_frame else (sp, batch)
-        b["R"].grad = b["Th"].grad = None
+        s, b = {"plain": (sp, batch), "frame": (sp_pose, pose), "rays": (sp, cam)}[mode]
+        b["R"].grad = b["Th"].grad = b["ray_o"].grad = b["ray_d"].grad = None
         out = ren.get_pixel_value(b["ray_o"], b["ray_d"], b["near"], b["far"], vols, s, b)
         loss = ((out["rgb_map"] - target) ** 2).mean()
         if "rgb0" in out:
             loss = loss + ((out["rgb0"] - target) ** 2).mean()          # img_loss0, if_nerf_clight.py:29-32
         loss.backward()
 
-    modes = (False, True) if frame_grads else (False,)
+    modes = ("plain",) + (("frame",) if frame_grads else ()) + (("rays",) if ray_grads else ())
     for _ in range(5):
         for m in modes:
             step(m)
@@ -77,12 +80,16 @@ def main():
     ms = {m: sum(a.elapsed_time(b) for a, b in ev[m]) / iters for m in modes}
     res = {"config": "c3: 1024-ray training chunk, 64 + %d samples, fwd + bwd, %s" % (ni, precision),
            "gpu": torch.cuda.get_device_name(0),
-           "ms_per_step": ms[False], "rays_per_s_fwd_bwd": 1024 / (ms[False] * 1e-3),
+           "ms_per_step": ms["plain"], "rays_per_s_fwd_bwd": 1024 / (ms["plain"] * 1e-3),
            "grad_norm_fc0": float(dict(net.named_parameters())["fc_0.weight"].grad.norm())}
     if frame_grads:
-        res["ms_per_step_frame_grads"] = ms[True]
-        res["frame_grads_overhead_ms"] = ms[True] - ms[False]
+        res["ms_per_step_frame_grads"] = ms["frame"]
+        res["frame_grads_overhead_ms"] = ms["frame"] - ms["plain"]
         res["dR_norm"], res["dTh_norm"] = float(pose["R"].grad.norm()), float(pose["Th"].grad.norm())
+    if ray_grads:
+        res["ms_per_step_ray_grads"] = ms["rays"]
+        res["ray_grads_overhead_ms"] = ms["rays"] - ms["plain"]
+        res["d_ray_o_norm"], res["d_ray_d_norm"] = float(cam["ray_o"].grad.norm()), float(cam["ray_d"].grad.norm())
     print(json.dumps(res))
 
 
