@@ -319,6 +319,21 @@ int    nb_render_bwd_frame(const nb_render_bwd_args* args, float* d_R, float* d_
  * (fine-pass) forward they are taken as given.  Both training precisions.  nb_render_bwd_frame(args, dR, dTh, stream) is
  * nb_render_bwd_rays(args, dR, dTh, NULL, NULL, stream) and enqueues no ray-gradient work.  No extra workspace. */
 int    nb_render_bwd_rays(const nb_render_bwd_args* args, float* d_R, float* d_Th, float* d_ray_o, float* d_ray_d, void* stream);
+/* nb_render_bwd_rays plus the cotangents of the two remaining output maps, so that a loss on any output of the render
+ * differentiates as upstream's autograd does (raw2outputs, nerf_net_utils.py:37-45).  d_disp_map: device (B,n) fp32,
+ * d_weights: device (B,n,S) fp32, both dense; either may be NULL.  They enter the per-ray compositing backward only:
+ *   weights:  w_i = alpha_i T_i, differentiated exactly like the other maps;
+ *   disp_map: 1 / max(1e-10, depth / acc) with torch's backward rules (reciprocal; maximum: all of the gradient to
+ *             depth / acc where it is > 1e-10 or NaN, half where it equals 1e-10, none below; division).  depth and acc are
+ *             recomputed as the forward composited them, before the white background; the output maps are not read.
+ * NaN semantics are upstream's: on a ray with acc_map == 0, disp_map is NaN (0 / 0), and with a non-NULL d_disp_map its
+ * gradient is NaN whatever the cotangent (0 * NaN = NaN).  relu(sigma) masks it out of every sample's sigma, so the
+ * decoder, volume, R / Th and ray_o gradients stay finite; d_ray_d, which takes dists * relu(sigma) with relu(sigma) = 0,
+ * is NaN on exactly those rays.  Both training precisions; S <= 256 as for every backward.
+ * nb_render_bwd_rays(args, dR, dTh, do, dd, stream) is nb_render_bwd_maps(args, NULL, NULL, dR, dTh, do, dd, stream).
+ * No extra workspace and no extra launch. */
+int    nb_render_bwd_maps(const nb_render_bwd_args* args, const float* d_disp_map, const float* d_weights, float* d_R,
+                          float* d_Th, float* d_ray_o, float* d_ray_d, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Diagnostics.

@@ -14,7 +14,7 @@ NB_NUM_LEVELS = 4
 EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_volume_bytes", "nb_packed_volume_level_offset",
            "nb_pack_volume", "nb_packed_weights_bytes", "nb_pack_weights", "nb_render_fwd",
            "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_render_bwd", "nb_render_bwd_frame", "nb_render_bwd_rays",
-           "nb_render_save_bytes",
+           "nb_render_bwd_maps", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit"]
@@ -120,6 +120,9 @@ def load(path=None):
     lib.nb_render_bwd_rays.restype = C.c_int
     lib.nb_render_bwd_rays.argtypes = [C.POINTER(nb_render_bwd_args), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p]
+    lib.nb_render_bwd_maps.restype = C.c_int
+    lib.nb_render_bwd_maps.argtypes = [C.POINTER(nb_render_bwd_args), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]
     lib.nb_render_save_bytes.restype = C.c_size_t
     lib.nb_render_save_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.nb_render_bwd_workspace_bytes.restype = C.c_size_t

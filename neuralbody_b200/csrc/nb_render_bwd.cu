@@ -1,6 +1,7 @@
 // Backward of the fused render (nb_render_bwd): gradients of rgb_map / depth_map / acc_map with respect to
 // the four dense feature volumes, every decoder parameter and the latent table; nb_render_bwd_frame adds the frame
-// transform R / Th, nb_render_bwd_rays also the rays ray_o / ray_d.
+// transform R / Th, nb_render_bwd_rays also the rays ray_o / ray_d, nb_render_bwd_maps also the cotangents of disp_map
+// and weights.
 //
 // Upstream this is PyTorch autograd through raw2outputs (nerf_net_utils.py:6-51), the eight Conv1d layers
 // and F.grid_sample (latent_xyzc.py:62-126), driven by Trainer.train (lib/train/trainers/trainer.py:46-53).
@@ -25,6 +26,7 @@ struct BwdParams {
     const float* save;              // (B,n,S,kSaveDim)
     const float* raw;               // (B,n,S,4)
     const float *d_rgb, *d_depth, *d_acc;   // any may be null
+    const float *d_disp, *d_weights;        // (B,n) / (B,n,S); either may be null
     float* ws;                      // (B*n*S, kGradDim) scratch
     nb_decoder_weights w;           // raw decoder tensors
     float* d_vol[4];                // NCDHW fp32, caller-zeroed, accumulated into
@@ -42,54 +44,92 @@ constexpr int kBwdMaxSamples = 256;     // coarse + importance samples of a fine
 // division => safe when 1 - alpha underflows) -- are run by lane 0 in the reference's order; the outputs are written by all
 // lanes.  (The earlier thread-per-ray version kept 1024 threads busy on a 148-SM device: 0.16 ms per 192-sample pass.)
 constexpr int CB_WARPS = 4;
+
+struct RaySmem {                        // one warp's ray in the per-ray kernels
+    float alpha[kBwdMaxSamples], f[kBwdMaxSamples], g[kBwdMaxSamples], T[kBwdMaxSamples], U[kBwdMaxSamples], z[kBwdMaxSamples + 1];
+};
+
+// d disp_map -> d depth_map, d acc_map through disp = 1 / max(1e-10, x), x = depth / acc (nerf_net_utils.py:44), by torch's
+// own backward rules: reciprocal -d r^2; maximum hands x the whole of it where x > 1e-10 or x is NaN, half where x == 1e-10,
+// nothing below; division d / acc to depth and -d (x / acc) to acc.  On a ray with acc == 0, x = 0 / 0 is NaN and so are
+// both results, whatever d_disp is: upstream's autograd does the same.
+__device__ __forceinline__ void disparity_bwd(float depth, float acc, float d_disp, float& dD, float& dA) {
+    const float x = __fdiv_rn(depth, acc);
+    const float r = disparity(depth, acc);
+    const float dm = -(d_disp * (r * r));
+    const float dx = (x > 1e-10f || x != x) ? dm : (x == 1e-10f ? dm * 0.5f : 0.f);
+    dD += __fdiv_rn(dx, acc);
+    dA += -dx * __fdiv_rn(x, acc);
+}
+
+// The part both per-ray kernels share, run by the whole warp of ray ri: z, alpha, f = 1 - alpha + 1e-10 and the per-sample
+// cotangent g_i = dC . rgb_i + dD z_i + dA into sm, then lane 0's recurrences T (exclusive transmittance) and U; dC (the
+// cotangent of rgb_map) is returned for the rgb logits.  The cotangents of disp_map and weights enter here and nowhere else:
+//   weights:  g_i += d_weights_i -- exact, since w_i = alpha_i T_i is what the recurrences differentiate;
+//   disp_map: folded into dD / dA (disparity_bwd) at the depth and acc of the forward's own composite_ray, recomputed here
+//             so that max(1e-10, x) takes the forward's branch.  The white background does not enter disp.
+__device__ __forceinline__ void ray_bwd_recurrences(const BwdParams& Q, size_t ri, float nrm, RaySmem& sm, float (&dC)[3], int lane) {
+    const RenderParams& P = Q.f;
+    const int S = P.n_samples;
+    const float near = P.near[ri], far = P.far[ri];
+    const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
+    const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
+    const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
+    dC[0] = dC[1] = dC[2] = 0.f;
+    if (Q.d_rgb) { dC[0] = Q.d_rgb[ri * 3]; dC[1] = Q.d_rgb[ri * 3 + 1]; dC[2] = Q.d_rgb[ri * 3 + 2]; }
+    float dD = Q.d_depth ? Q.d_depth[ri] : 0.f;
+    float dA = Q.d_acc ? Q.d_acc[ri] : 0.f;
+    if (P.white_bkgd) dA -= dC[0] + dC[1] + dC[2];            // rgb_map += 1 - acc_map
+    for (int s = lane; s < S; s += 32) sm.z[s] = z_sample(near, far, P.t_vals, s, S, tr, zu);
+    __syncwarp();
+    if (Q.d_disp) {
+        const RayOut o = composite_ray(raw, sm.z, S, nrm, nullptr, lane);
+        disparity_bwd(o.depth, o.acc, Q.d_disp[ri], dD, dA);
+    }
+    const float* dW = Q.d_weights ? Q.d_weights + ri * S : nullptr;
+    for (int s = lane; s < S; s += 32) {
+        const float4 rw = raw[s];
+        const float z = sm.z[s];
+        const float dist = ((s + 1 < S) ? __fsub_rn(sm.z[s + 1], z) : 1e10f) * nrm;
+        const float alpha = 1.f - expf(-fmaxf(rw.w, 0.f) * dist);
+        const float c0 = 1.f / (1.f + expf(-rw.x)), c1 = 1.f / (1.f + expf(-rw.y)), c2 = 1.f / (1.f + expf(-rw.z));
+        sm.alpha[s] = alpha;
+        sm.f[s] = 1.f - alpha + 1e-10f;
+        float g = dC[0] * c0 + dC[1] * c1 + dC[2] * c2 + dD * z + dA;
+        if (dW) g += dW[s];
+        sm.g[s] = g;
+    }
+    __syncwarp();
+    if (lane == 0) {
+        float T = 1.f;
+        for (int s = 0; s < S; ++s) { sm.T[s] = T; T *= sm.f[s]; }       // exclusive transmittance
+        float U = 0.f;
+        for (int s = S - 1; s >= 0; --s) { sm.U[s] = U; U = sm.g[s] * sm.alpha[s] + sm.f[s] * U; }
+    }
+    __syncwarp();
+}
+
 __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdParams Q) {
-    __shared__ float s_alpha[CB_WARPS][kBwdMaxSamples], s_f[CB_WARPS][kBwdMaxSamples], s_g[CB_WARPS][kBwdMaxSamples],
-        s_T[CB_WARPS][kBwdMaxSamples], s_U[CB_WARPS][kBwdMaxSamples], s_z[CB_WARPS][kBwdMaxSamples + 1];
+    __shared__ RaySmem s_ray[CB_WARPS];
     const RenderParams& P = Q.f;
     const int S = P.n_samples;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const size_t ri = (size_t)blockIdx.x * CB_WARPS + warp;
     if (ri >= (size_t)P.batch * P.n_rays) return;
-    const float near = P.near[ri], far = P.far[ri];
-    const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
-    const float nrm = ray_norm(dx, dy, dz);
-    const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
-    const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
+    const float nrm = ray_norm(P.ray_d[ri * 3], P.ray_d[ri * 3 + 1], P.ray_d[ri * 3 + 2]);
+    RaySmem& sm = s_ray[warp];
+    float dC[3];
+    ray_bwd_recurrences(Q, ri, nrm, sm, dC, lane);
     const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
-    float dC[3] = {0.f, 0.f, 0.f};
-    if (Q.d_rgb) { dC[0] = Q.d_rgb[ri * 3]; dC[1] = Q.d_rgb[ri * 3 + 1]; dC[2] = Q.d_rgb[ri * 3 + 2]; }
-    const float dD = Q.d_depth ? Q.d_depth[ri] : 0.f;
-    float dA = Q.d_acc ? Q.d_acc[ri] : 0.f;
-    if (P.white_bkgd) dA -= dC[0] + dC[1] + dC[2];            // rgb_map += 1 - acc_map
-    for (int s = lane; s < S; s += 32) s_z[warp][s] = z_sample(near, far, P.t_vals, s, S, tr, zu);
-    __syncwarp();
     for (int s = lane; s < S; s += 32) {
         const float4 rw = raw[s];
-        const float z = s_z[warp][s];
-        const float dist = ((s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f) * nrm;
-        const float alpha = 1.f - expf(-fmaxf(rw.w, 0.f) * dist);
-        const float c0 = 1.f / (1.f + expf(-rw.x)), c1 = 1.f / (1.f + expf(-rw.y)), c2 = 1.f / (1.f + expf(-rw.z));
-        s_alpha[warp][s] = alpha;
-        s_f[warp][s] = 1.f - alpha + 1e-10f;
-        s_g[warp][s] = dC[0] * c0 + dC[1] * c1 + dC[2] * c2 + dD * z + dA;
-    }
-    __syncwarp();
-    if (lane == 0) {
-        float T = 1.f;
-        for (int s = 0; s < S; ++s) { s_T[warp][s] = T; T *= s_f[warp][s]; }       // exclusive transmittance
-        float U = 0.f;
-        for (int s = S - 1; s >= 0; --s) { s_U[warp][s] = U; U = s_g[warp][s] * s_alpha[warp][s] + s_f[warp][s] * U; }
-    }
-    __syncwarp();
-    for (int s = lane; s < S; s += 32) {
-        const float4 rw = raw[s];
-        const float z = s_z[warp][s];
-        const float dist = ((s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f) * nrm;
+        const float z = sm.z[s];
+        const float dist = ((s + 1 < S) ? __fsub_rn(sm.z[s + 1], z) : 1e10f) * nrm;
         const float e = expf(-fmaxf(rw.w, 0.f) * dist);
         const float c0 = 1.f / (1.f + expf(-rw.x)), c1 = 1.f / (1.f + expf(-rw.y)), c2 = 1.f / (1.f + expf(-rw.z));
-        const float Ti = s_T[warp][s];
-        const float w = s_alpha[warp][s] * Ti;
-        const float dalpha = s_g[warp][s] * Ti - Ti * s_U[warp][s];
+        const float Ti = sm.T[s];
+        const float w = sm.alpha[s] * Ti;
+        const float dalpha = sm.g[s] * Ti - Ti * sm.U[s];
         float4 o;
         o.x = w * dC[0] * c0 * (1.f - c0);
         o.y = w * dC[1] * c1 * (1.f - c1);
@@ -103,56 +143,32 @@ __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdP
 // sample i's [d loss / d(world point) 3 | d loss / d(view direction) 3] (zero for a skipped sample).  With p_i = o + z_i d,
 // u = d / |d| and dists_i = delta_i |d| (nerf_net_utils.py:28):
 //   d o += sum_i g_i,   d d += sum_i z_i g_i + (du - u (u . du)) / |d| + u sum_i dL/d dists_i delta_i,
-// where du = sum_i du_i and dL/d dists_i = dalpha_i relu(sigma_i) e_i; z, dist and the T / U recurrences are re-derived exactly
-// as composite_bwd_kernel does.  z is not differentiated (near / far and z_vals are not inputs of the gradient).
+// where du = sum_i du_i and dL/d dists_i = dalpha_i relu(sigma_i) e_i; z, dist and the T / U recurrences are those of
+// composite_bwd_kernel (ray_bwd_recurrences).  z is not differentiated (near / far and z_vals are not inputs of the gradient).
 __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams Q, const float* __restrict__ rec, int rec_stride) {
-    __shared__ float s_alpha[CB_WARPS][kBwdMaxSamples], s_f[CB_WARPS][kBwdMaxSamples], s_g[CB_WARPS][kBwdMaxSamples],
-        s_T[CB_WARPS][kBwdMaxSamples], s_U[CB_WARPS][kBwdMaxSamples], s_z[CB_WARPS][kBwdMaxSamples + 1];
+    __shared__ RaySmem s_ray[CB_WARPS];
     const RenderParams& P = Q.f;
     const int S = P.n_samples;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const size_t ri = (size_t)blockIdx.x * CB_WARPS + warp;
     if (ri >= (size_t)P.batch * P.n_rays) return;
-    const float near = P.near[ri], far = P.far[ri];
     const float dx = P.ray_d[ri * 3], dy = P.ray_d[ri * 3 + 1], dz = P.ray_d[ri * 3 + 2];
     const float nrm = ray_norm(dx, dy, dz);
-    const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
-    const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
+    RaySmem& sm = s_ray[warp];
+    float dC[3];
+    ray_bwd_recurrences(Q, ri, nrm, sm, dC, lane);
     const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
-    float dC[3] = {0.f, 0.f, 0.f};
-    if (Q.d_rgb) { dC[0] = Q.d_rgb[ri * 3]; dC[1] = Q.d_rgb[ri * 3 + 1]; dC[2] = Q.d_rgb[ri * 3 + 2]; }
-    const float dD = Q.d_depth ? Q.d_depth[ri] : 0.f;
-    float dA = Q.d_acc ? Q.d_acc[ri] : 0.f;
-    if (P.white_bkgd) dA -= dC[0] + dC[1] + dC[2];
-    for (int s = lane; s < S; s += 32) s_z[warp][s] = z_sample(near, far, P.t_vals, s, S, tr, zu);
-    __syncwarp();
-    for (int s = lane; s < S; s += 32) {
-        const float4 rw = raw[s];
-        const float z = s_z[warp][s];
-        const float dist = ((s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f) * nrm;
-        const float alpha = 1.f - expf(-fmaxf(rw.w, 0.f) * dist);
-        const float c0 = 1.f / (1.f + expf(-rw.x)), c1 = 1.f / (1.f + expf(-rw.y)), c2 = 1.f / (1.f + expf(-rw.z));
-        s_alpha[warp][s] = alpha;
-        s_f[warp][s] = 1.f - alpha + 1e-10f;
-        s_g[warp][s] = dC[0] * c0 + dC[1] * c1 + dC[2] * c2 + dD * z + dA;
-    }
-    __syncwarp();
-    if (lane == 0) {
-        float T = 1.f;
-        for (int s = 0; s < S; ++s) { s_T[warp][s] = T; T *= s_f[warp][s]; }
-        float U = 0.f;
-        for (int s = S - 1; s >= 0; --s) { s_U[warp][s] = U; U = s_g[warp][s] * s_alpha[warp][s] + s_f[warp][s] * U; }
-    }
-    __syncwarp();
     float go[3] = {0.f, 0.f, 0.f}, gd[3] = {0.f, 0.f, 0.f}, du[3] = {0.f, 0.f, 0.f}, dn = 0.f;
     for (int s = lane; s < S; s += 32) {
-        const float z = s_z[warp][s];
-        const float delta = (s + 1 < S) ? __fsub_rn(s_z[warp][s + 1], z) : 1e10f;
+        const float z = sm.z[s];
+        const float delta = (s + 1 < S) ? __fsub_rn(sm.z[s + 1], z) : 1e10f;
         const float sg = fmaxf(raw[s].w, 0.f);
         const float e = expf(-sg * (delta * nrm));
-        const float Ti = s_T[warp][s];
-        const float dalpha = s_g[warp][s] * Ti - Ti * s_U[warp][s];
-        dn = fmaf(dalpha * sg * e, delta, dn);          // a skipped (empty) sample has sigma < 0: no term
+        const float Ti = sm.T[s];
+        const float dalpha = sm.g[s] * Ti - Ti * sm.U[s];
+        // kept for sg == 0 too: a skipped (empty) sample adds 0, except that the NaN dalpha of a ray with acc == 0 and a
+        // disp_map cotangent makes d ray_d NaN, as upstream's dists * relu(sigma) does
+        dn = fmaf(dalpha * sg * e, delta, dn);
         const float* r = rec + (ri * S + s) * rec_stride;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { go[k] += r[k]; gd[k] = fmaf(z, r[k], gd[k]); du[k] += r[3 + k]; }
@@ -588,19 +604,19 @@ __global__ void unfold_stage3(const Unfold U) {     // d view_fc[:, :256], d lat
 
 }  // namespace bwd
 
-void launch_composite_bwd(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
-                          float* d_raw_out, int d_raw_stride, cudaStream_t stream) {
+void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCotangents& d, float* d_raw_out, int d_raw_stride,
+                          cudaStream_t stream) {
     bwd::BwdParams Q{};
-    Q.f = p; Q.raw = raw; Q.d_rgb = d_rgb; Q.d_depth = d_depth; Q.d_acc = d_acc;
+    Q.f = p; Q.raw = raw; Q.d_rgb = d.rgb; Q.d_depth = d.depth; Q.d_acc = d.acc; Q.d_disp = d.disp; Q.d_weights = d.weights;
     Q.d_raw_out = d_raw_out; Q.d_raw_stride = d_raw_stride;
     const size_t nrays = (size_t)p.batch * p.n_rays;
     bwd::composite_bwd_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q);
 }
 
-void launch_ray_grad(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
-                     const float* rec, int rec_stride, float* d_ray_o, float* d_ray_d, cudaStream_t stream) {
+void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
+                     float* d_ray_o, float* d_ray_d, cudaStream_t stream) {
     bwd::BwdParams Q{};
-    Q.f = p; Q.raw = raw; Q.d_rgb = d_rgb; Q.d_depth = d_depth; Q.d_acc = d_acc;
+    Q.f = p; Q.raw = raw; Q.d_rgb = d.rgb; Q.d_depth = d.depth; Q.d_acc = d.acc; Q.d_disp = d.disp; Q.d_weights = d.weights;
     Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
     const size_t nrays = (size_t)p.batch * p.n_rays;
     bwd::ray_grad_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
@@ -655,6 +671,11 @@ extern "C" int nb_render_bwd_frame(const nb_render_bwd_args* a, float* d_R, floa
 }
 
 extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float* d_Th, float* d_ray_o, float* d_ray_d, void* stream) {
+    return nb_render_bwd_maps(a, nullptr, nullptr, d_R, d_Th, d_ray_o, d_ray_d, stream);
+}
+
+extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_disp_map, const float* d_weights, float* d_R,
+                                  float* d_Th, float* d_ray_o, float* d_ray_d, void* stream) {
     if (!a || !a->fwd || !a->save || !a->raw || !a->workspace || !a->weights || !a->grads) {
         set_error("nb_render_bwd: null argument");
         return NB_ERR_BAD_ARG;
@@ -668,7 +689,8 @@ extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float
     if (f->precision == NB_PRECISION_TC_TF32X3) {
         if (a->workspace_bytes < train_bwd_workspace_bytes(p, f->n_rays, f->n_samples)) { set_error("nb_render_bwd: workspace too small (see nb_render_bwd_workspace_bytes_for)"); return NB_ERR_BAD_ARG; }
         trn::TrainBwd t;
-        t.save = a->save; t.raw = a->raw; t.d_rgb = a->d_rgb_map; t.d_depth = a->d_depth_map; t.d_acc = a->d_acc_map;
+        t.save = a->save; t.raw = a->raw;
+        t.d_maps = {a->d_rgb_map, a->d_depth_map, a->d_acc_map, d_disp_map, d_weights};
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
         for (int l = 0; l < 4; ++l) t.d_vol[l] = a->d_volumes[l];
         t.d_R = d_R; t.d_Th = d_Th; t.d_ray_o = d_ray_o; t.d_ray_d = d_ray_d; t.volume_dtype = f->volume_dtype;
@@ -685,7 +707,8 @@ extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float
     bwd::BwdParams Q{};
     Q.f = p;
     Q.save = a->save; Q.raw = a->raw;
-    Q.d_rgb = a->d_rgb_map; Q.d_depth = a->d_depth_map; Q.d_acc = a->d_acc_map;
+    const MapCotangents d_maps{a->d_rgb_map, a->d_depth_map, a->d_acc_map, d_disp_map, d_weights};
+    Q.d_rgb = d_maps.rgb; Q.d_depth = d_maps.depth; Q.d_acc = d_maps.acc; Q.d_disp = d_maps.disp; Q.d_weights = d_maps.weights;
     Q.ws = (float*)a->workspace;
     Q.d_raw_out = Q.ws + kGradRaw; Q.d_raw_stride = kGradDim;
     Q.w = *a->weights;
@@ -751,7 +774,7 @@ extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float
         bwd::pe_grad_kernel<<<(unsigned)((npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS < (size_t)kGridSMs * 16
                                              ? (npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS : (size_t)kGridSMs * 16),
                               bwd::PG_WARPS * 32, 0, s>>>(Q, rec, kGradDim);
-        launch_ray_grad(p, a->raw, a->d_rgb_map, a->d_depth_map, a->d_acc_map, rec, kGradDim, d_ray_o, d_ray_d, s);
+        launch_ray_grad(p, a->raw, d_maps, rec, kGradDim, d_ray_o, d_ray_d, s);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_render_bwd: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

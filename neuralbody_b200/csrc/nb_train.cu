@@ -708,7 +708,7 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     cudaMemsetAsync(dwcol, 0, ((size_t)kWS * kH2X + ((size_t)p.batch * kWS + 63) / 64 * 64) * 4, stream);
 
     // 1. d(outputs) -> d(raw) per sample (dense), 2. the colour layer's output gradient over the list
-    launch_composite_bwd(p, t.raw, t.d_rgb, t.d_depth, t.d_acc, reinterpret_cast<float*>(d_raw), 4, stream);
+    launch_composite_bwd(p, t.raw, t.d_maps, reinterpret_cast<float*>(d_raw), 4, stream);
     bwd_head_kernel<<<kGridSMs * 2, 256, 0, stream>>>(p.wf32, sv, d_raw, G3, G_(g.rgb_w), G_(g.rgb_b));
     // 3. dgrad chain (relu masks = the saved activations)
     GemmArgs a{};
@@ -774,7 +774,7 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
         cudaMemsetAsync(rec, 0, pmax * kRayRec * 4, stream);
         if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
         else frame_grad_kernel<__half, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
-        launch_ray_grad(p, t.raw, t.d_rgb, t.d_depth, t.d_acc, rec, kRayRec, t.d_ray_o, t.d_ray_d, stream);
+        launch_ray_grad(p, t.raw, t.d_maps, rec, kRayRec, t.d_ray_o, t.d_ray_d, stream);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("train bwd launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

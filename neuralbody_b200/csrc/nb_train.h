@@ -3,6 +3,11 @@
 #include "nb_internal.h"
 
 namespace nb {
+
+// the cotangents of the five output maps a backward call was given (device, dense; any may be null):
+// rgb (B,n,3), depth / acc / disp (B,n), weights (B,n,S)
+struct MapCotangents { const float *rgb, *depth, *acc, *disp, *weights; };
+
 namespace trn {
 
 constexpr int kH2X = 352;                   // colour-layer input record: [h2 256 | PE(xyz) 63 | 0 | PE(viewdir) 27 | 0 x 5]
@@ -41,7 +46,7 @@ struct GradBlob { size_t off[4], bstride[4], floats; };   // channels-last volum
 
 struct TrainBwd {
     const float* save; const float* raw;
-    const float *d_rgb, *d_depth, *d_acc;
+    MapCotangents d_maps;
     const nb_decoder_weights* weights; const nb_decoder_weights* grads;
     float* d_vol[4];
     float *d_R, *d_Th;               // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
@@ -61,12 +66,12 @@ int launch_train_bwd(const RenderParams& p, const trn::TrainBwd& t, cudaStream_t
 // shared pieces living in other translation units
 void launch_classify(const RenderParams& p, cudaStream_t stream);    // nb_render_tc_list.cu (p.frame, lists, raw_ws set by the caller)
 void launch_composite(const RenderParams& p, cudaStream_t stream);   // nb_render_tc_list.cu
-void launch_composite_bwd(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
-                          float* d_raw_out, int d_raw_stride, cudaStream_t stream);   // nb_render_bwd.cu
+void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCotangents& d, float* d_raw_out, int d_raw_stride,
+                          cudaStream_t stream);                                        // nb_render_bwd.cu
 // per ray: the per-sample records rec + i * rec_stride = [d / d(world point) 3 | d / d(view direction) 3] plus the compositing
 // term -> d_ray_o / d_ray_d (accumulated into; either may be null)                                              nb_render_bwd.cu
-void launch_ray_grad(const RenderParams& p, const float* raw, const float* d_rgb, const float* d_depth, const float* d_acc,
-                     const float* rec, int rec_stride, float* d_ray_o, float* d_ray_d, cudaStream_t stream);
+void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
+                     float* d_ray_o, float* d_ray_d, cudaStream_t stream);
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
                   float* u, float* du, cudaStream_t stream);                          // nb_render_bwd.cu
 

@@ -33,11 +33,13 @@ def _f32c(t, device):
 
 class _FusedRender(torch.autograd.Function):
     """Autograd boundary of the training path (BASELINE config 3): forward = nb_render_fwd with the exact
-    kernel + activation record, backward = nb_render_bwd.  Differentiable outputs: rgb_map, depth_map,
-    acc_map (what lib/train/trainers/if_nerf_clight.py:25-32 and depth/mask losses consume); disp_map and
-    weights are returned detached.  Differentiable inputs: the four dense volumes (so gradients keep flowing
-    into the reference's SparseConvNet / code embedding), the 17 decoder tensors, the frame transform
-    sp_input['R'] / ['Th'] (pose refinement) and the rays ray_o / ray_d (camera refinement; nb_render_bwd_rays)."""
+    kernel + activation record, backward = nb_render_bwd_maps.  Differentiable outputs: all five maps, rgb_map,
+    disp_map, acc_map, depth_map and weights, as upstream's raw2outputs (nerf_net_utils.py:37-45); an output the loss
+    does not read costs nothing (its cotangent stays None and the kernels get NULL).  disp_map follows upstream's NaN
+    rule: on a ray with acc_map == 0 its gradient is NaN, which reaches ray_d only (see nb_render_bwd_maps).
+    Differentiable inputs: the four dense volumes (so gradients keep flowing into the reference's SparseConvNet / code
+    embedding), the 17 decoder tensors, the frame transform sp_input['R'] / ['Th'] (pose refinement) and the rays
+    ray_o / ray_d (camera refinement)."""
 
     @staticmethod
     def forward(ctx, renderer, call, *tensors):
@@ -45,12 +47,13 @@ class _FusedRender(torch.autograd.Function):
         ctx.renderer, ctx.call = renderer, call
         ctx.n_vol = len(call["feature_volume"])
         ctx.save_for_backward(*tensors)
-        ctx.mark_non_differentiable(out["disp_map"], out["weights"])
+        ctx.set_materialize_grads(False)    # no zero (B,n,S) cotangent for a loss that does not read weights
         return out["rgb_map"], out["disp_map"], out["acc_map"], out["depth_map"], out["weights"]
 
     @staticmethod
     def backward(ctx, d_rgb, d_disp, d_acc, d_depth, d_weights):
-        grads = ctx.renderer._launch_bwd(ctx.call, d_rgb, d_depth, d_acc, ctx.needs_input_grad[2:])
+        grads = ctx.renderer._launch_bwd(ctx.call, d_rgb, d_depth, d_acc, ctx.needs_input_grad[2:], d_disp=d_disp,
+                                         d_weights=d_weights)
         return (None, None) + tuple(grads)
 
 
@@ -403,9 +406,9 @@ class Renderer:
             out['raw'] = raw
         return out
 
-    def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs):
-        """nb_render_bwd_rays: gradients for (volumes..., decoder tensors..., R, Th, ray_o, ray_d) in the order of
-        _FusedRender.apply."""
+    def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs, d_disp=None, d_weights=None):
+        """nb_render_bwd_maps: gradients for (volumes..., decoder tensors..., R, Th, ray_o, ray_d) in the order of
+        _FusedRender.apply, from the cotangents of the five maps (None: the loss does not read that map)."""
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         if call.get("save") is None:
             raise RuntimeError("the activation record of this render call was already consumed by a backward pass "
@@ -415,7 +418,7 @@ class Renderer:
         with torch.cuda.device(dev), torch.no_grad():
             def cf(t):
                 return None if t is None else t.to(device=dev, dtype=torch.float32).contiguous()
-            d_rgb, d_depth, d_acc = cf(d_rgb), cf(d_depth), cf(d_acc)
+            d_rgb, d_depth, d_acc, d_disp, d_weights = cf(d_rgb), cf(d_depth), cf(d_acc), cf(d_disp), cf(d_weights)
             w = self._weights_struct(params, call["sp_input"]['latent_index'], dev)
             # 17 small tensors (they stay in the allocator's small pool), zeroed by one multi-tensor launch
             gparams = [torch.empty_like(t, dtype=torch.float32, device=dev) for t in params]
@@ -445,8 +448,8 @@ class Renderer:
             # rays (camera refinement): fp32 (B,n,3) accumulators, likewise
             drays = [torch.zeros((B, n, 3), dtype=torch.float32, device=dev) if want else None for want in needs[-2:]]
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_render_bwd_rays(C.byref(ba), _ptr(dR), _ptr(dTh), _ptr(drays[0]), _ptr(drays[1]),
-                                                   C.c_void_p(stream)), "nb_render_bwd_rays")
+            capi.check(self.lib.nb_render_bwd_maps(C.byref(ba), _ptr(d_disp), _ptr(d_weights), _ptr(dR), _ptr(dTh),
+                                                   _ptr(drays[0]), _ptr(drays[1]), C.c_void_p(stream)), "nb_render_bwd_maps")
             # stream-ordered reuse: the next forward / backward on this stream runs after the kernels just enqueued
             self._pool_give("bwd_ws", ws)
             self._pool_give("save", call.pop("save"))

@@ -4,8 +4,10 @@ default tc_tf32x3: sample list + TF32x3 GEMM chains, with activation record, coa
 both passes.  Prints one JSON line (rays/s for fwd+bwd).
 With --frame-grads the same process alternates steps without and with gradients for the frame transform
 (sp_input['R'] / ['Th'] requiring grad, as pose refinement does) and reports both step times; --ray-grads does the same
-with ray_o / ray_d requiring grad (camera refinement).
-Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--ray-grads] [--precision tc_tf32x3|fp32]"""
+with ray_o / ray_d requiring grad (camera refinement), --map-grads with a loss that also reads disp_map, disp0 and the fine
+weights (an entropy regulariser on the ray weights and a disparity term, as distortion / smoothness losses do).
+Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--ray-grads] [--map-grads]
+                                         [--precision tc_tf32x3|fp32]"""
 import json
 import os
 import sys
@@ -20,6 +22,7 @@ def main():
     args = sys.argv[1:]
     frame_grads = "--frame-grads" in args
     ray_grads = "--ray-grads" in args
+    map_grads = "--map-grads" in args
     precision = "tc_tf32x3"
     if "--precision" in args:
         precision = args[args.index("--precision") + 1]
@@ -54,15 +57,20 @@ def main():
             p.grad = None
         for v in vols:
             v.grad = None
-        s, b = {"plain": (sp, batch), "frame": (sp_pose, pose), "rays": (sp, cam)}[mode]
+        s, b = {"plain": (sp, batch), "frame": (sp_pose, pose), "rays": (sp, cam), "maps": (sp, batch)}[mode]
         b["R"].grad = b["Th"].grad = b["ray_o"].grad = b["ray_d"].grad = None
         out = ren.get_pixel_value(b["ray_o"], b["ray_d"], b["near"], b["far"], vols, s, b)
         loss = ((out["rgb_map"] - target) ** 2).mean()
         if "rgb0" in out:
             loss = loss + ((out["rgb0"] - target) ** 2).mean()          # img_loss0, if_nerf_clight.py:29-32
+        if mode == "maps":
+            w = out["weights"]
+            loss = loss + 1e-3 * -(w * torch.log(w + 1e-10)).sum(-1).mean()
+            for d, a in (("disp_map", "acc_map"), ("disp0", "acc0")):
+                loss = loss + 1e-3 * torch.where(out[a] > 0, out[d], torch.zeros_like(out[d])).mean()
         loss.backward()
 
-    modes = ("plain",) + (("frame",) if frame_grads else ()) + (("rays",) if ray_grads else ())
+    modes = ("plain",) + (("frame",) if frame_grads else ()) + (("rays",) if ray_grads else ()) + (("maps",) if map_grads else ())
     for _ in range(5):
         for m in modes:
             step(m)
@@ -90,6 +98,9 @@ def main():
         res["ms_per_step_ray_grads"] = ms["rays"]
         res["ray_grads_overhead_ms"] = ms["rays"] - ms["plain"]
         res["d_ray_o_norm"], res["d_ray_d_norm"] = float(cam["ray_o"].grad.norm()), float(cam["ray_d"].grad.norm())
+    if map_grads:
+        res["ms_per_step_map_grads"] = ms["maps"]
+        res["map_grads_overhead_ms"] = ms["maps"] - ms["plain"]
     print(json.dumps(res))
 
 
