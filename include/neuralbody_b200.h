@@ -198,6 +198,10 @@ typedef struct nb_importance_args {
 } nb_importance_args;
 
 int nb_sample_pdf(const nb_importance_args* args, void* stream);
+/* nb_sample_pdf (the same launch, a bit-identical z_out) that also writes z_src: device (B*n, S + n_importance) int, for each
+ * entry of z_out the coarse sample index it came from, or -1 for an importance sample.  It routes d z_out back to the coarse
+ * depths (and so to near / far) when the fine pass is differentiated; on a tie either assignment holds the same z. */
+int nb_sample_pdf_src(const nb_importance_args* args, int* z_src, void* stream);
 
 /* f-3: density on arbitrary world points.  Replaces Network.calculate_density (lib/networks/latent_xyzc.py:74-89), the
  * alpha decoder of the mesh renderer (lib/networks/renderer/if_mesh_renderer.py:36-41).  Only the frame fields of `frame`
@@ -315,7 +319,7 @@ int    nb_render_bwd_frame(const nb_render_bwd_args* args, float* d_R, float* d_
  * refinement needs, i.e. upstream autograd through pts = ray_o + ray_d * z (if_clight_renderer.py:25), the view direction
  * ray_d / |ray_d| (:68) and PE(world xyz) into view_fc (latent_xyzc.py:115), the canonical transform into grid_sample, and
  * dists * |ray_d| in raw2outputs (nerf_net_utils.py:28).  d_ray_o, d_ray_d: device (B,n,3) fp32; both are ACCUMULATED into
- * and either may be NULL.  The depths z are not differentiated (upstream never differentiates near / far); after a z_vals
+ * and either may be NULL.  The depths z are not differentiated here (nb_render_bwd_inputs does that); after a z_vals
  * (fine-pass) forward they are taken as given.  Both training precisions.  nb_render_bwd_frame(args, dR, dTh, stream) is
  * nb_render_bwd_rays(args, dR, dTh, NULL, NULL, stream) and enqueues no ray-gradient work.  No extra workspace. */
 int    nb_render_bwd_rays(const nb_render_bwd_args* args, float* d_R, float* d_Th, float* d_ray_o, float* d_ray_d, void* stream);
@@ -334,6 +338,30 @@ int    nb_render_bwd_rays(const nb_render_bwd_args* args, float* d_R, float* d_T
  * No extra workspace and no extra launch. */
 int    nb_render_bwd_maps(const nb_render_bwd_args* args, const float* d_disp_map, const float* d_weights, float* d_R,
                           float* d_Th, float* d_ray_o, float* d_ray_d, void* stream);
+/* nb_render_bwd_maps plus the gradients of the remaining float inputs upstream's autograd reaches: the depths and the box.
+ * Every pointer is a device fp32 buffer ACCUMULATED into, and any may be NULL (a NULL struct = all NULL).
+ *   d_R, d_Th, d_ray_o, d_ray_d: as for nb_render_bwd_maps.
+ *   d_near, d_far (B,n): through z = near (1 - t) + far t and the stratified jitter (if_clight_renderer.py:11-23).  Only for
+ *     a forward that derived its depths from near / far: with nb_render_args.z_vals set they return NB_ERR_BAD_ARG before
+ *     anything is enqueued.
+ *   d_z_vals (B,n,S): d loss / d z_i per sample, after either kind of forward:
+ *     d z_i = g_i . ray_d + dD w_i + |ray_d| (c_{i-1} - c_i),  c_i = dalpha_i relu(sigma_i) exp(-relu(sigma_i) dist_i),
+ *     c_{S-1} = c_{-1} = 0 (the last dist is 1e10 |ray_d|), where g_i is d loss / d(world point i) (grid and PE(xyz) parts)
+ *     and dD the depth_map cotangent after the disp_map fold.  d_near / d_far are the sums of d z_i times z_i's coefficients.
+ *   d_bounds (B,2,3): row 0 -= the per-frame sum of d loss / d(canonical point) (get_grid_coords, latent_xyzc.py:49-60
+ *     subtracts bounds[:, 0]); row 1 is not touched.
+ * NaN semantics follow nb_render_bwd_maps: on a ray with acc_map == 0 and a d_disp_map cotangent, d_near, d_far and that
+ * ray's d_z_vals are NaN; d_bounds stays finite.  Both training precisions; S <= 256.  With the four new pointers NULL this is
+ * nb_render_bwd_maps and enqueues the same kernels.  No extra workspace. */
+typedef struct nb_render_input_grads {
+    float* d_R;  float* d_Th;          /* as nb_render_bwd_rays */
+    float* d_ray_o; float* d_ray_d;    /* as nb_render_bwd_rays */
+    float* d_near; float* d_far;       /* (B,n); only for a forward that derived z from near/far (z_vals == NULL) */
+    float* d_z_vals;                   /* (B,n,S): dL/dz_i per sample, either kind of forward */
+    float* d_bounds;                   /* (B,2,3): row 0 accumulated, row 1 untouched */
+} nb_render_input_grads;
+int    nb_render_bwd_inputs(const nb_render_bwd_args* args, const float* d_disp_map, const float* d_weights,
+                            const nb_render_input_grads* grads, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Diagnostics.

@@ -14,9 +14,9 @@ NB_NUM_LEVELS = 4
 EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_volume_bytes", "nb_packed_volume_level_offset",
            "nb_pack_volume", "nb_packed_weights_bytes", "nb_pack_weights", "nb_render_fwd",
            "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_render_bwd", "nb_render_bwd_frame", "nb_render_bwd_rays",
-           "nb_render_bwd_maps", "nb_render_save_bytes",
+           "nb_render_bwd_maps", "nb_render_bwd_inputs", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
-           "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf",
+           "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit"]
 
 
@@ -79,6 +79,10 @@ class nb_render_bwd_args(C.Structure):
     ]
 
 
+class nb_render_input_grads(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("d_R", "d_Th", "d_ray_o", "d_ray_d", "d_near", "d_far", "d_z_vals", "d_bounds")]
+
+
 _lib = None
 
 
@@ -123,6 +127,9 @@ def load(path=None):
     lib.nb_render_bwd_maps.restype = C.c_int
     lib.nb_render_bwd_maps.argtypes = [C.POINTER(nb_render_bwd_args), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.nb_render_bwd_inputs.restype = C.c_int
+    lib.nb_render_bwd_inputs.argtypes = [C.POINTER(nb_render_bwd_args), C.c_void_p, C.c_void_p,
+                                         C.POINTER(nb_render_input_grads), C.c_void_p]
     lib.nb_render_save_bytes.restype = C.c_size_t
     lib.nb_render_save_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.nb_render_bwd_workspace_bytes.restype = C.c_size_t
@@ -145,6 +152,8 @@ def load(path=None):
     lib.nb_gen_rays_sharded.argtypes = [C.POINTER(nb_camera)] + [C.c_int] * 4 + [C.c_void_p] * 6
     lib.nb_sample_pdf.restype = C.c_int
     lib.nb_sample_pdf.argtypes = [C.POINTER(nb_importance_args), C.c_void_p]
+    lib.nb_sample_pdf_src.restype = C.c_int
+    lib.nb_sample_pdf_src.argtypes = [C.POINTER(nb_importance_args), C.c_void_p, C.c_void_p]
     lib.nb_mcubes_workspace_bytes.restype = C.c_size_t
     lib.nb_mcubes_workspace_bytes.argtypes = [C.c_int] * 3
     lib.nb_mcubes_count.restype = C.c_int

@@ -48,6 +48,19 @@ __device__ __forceinline__ float z_sample(float near, float far, const float* __
     return z;
 }
 
+// d z / d near and d z / d far of sample s as z_sample derives it (no z_user): (1 - t_s, t_s) without jitter; with jitter the
+// combination lower (1 - r) + upper r makes of the mids .5 (z_{s-1} + z_s) / .5 (z_s + z_{s+1}), or of z_s at either end
+__device__ __forceinline__ void z_sample_coefs(const float* __restrict__ t_vals, int s, int S, const float* __restrict__ t_rand,
+                                               float& cn, float& cf) {
+    auto tv = [&](int i) { return t_vals ? __ldg(t_vals + i) : linspace01(i, S); };
+    const float t = tv(s);
+    if (!t_rand) { cn = 1.f - t; cf = t; return; }
+    const float tl = s > 0 ? .5f * (tv(s - 1) + t) : t, tu = s < S - 1 ? .5f * (t + tv(s + 1)) : t;
+    const float r = __ldg(t_rand + s);
+    cf = (1.f - r) * tl + r * tu;
+    cn = (1.f - r) * (1.f - tl) + r * (1.f - tu);
+}
+
 // torch.norm(ray_d, dim=-1): sqrt(x^2 + y^2 + z^2), summed left to right without contraction
 __device__ __forceinline__ float ray_norm(float x, float y, float z) {
     return sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
@@ -245,6 +258,33 @@ __device__ __forceinline__ void frame_grad_add(FrameGradAcc& a, int b, const flo
             if (lane == k) mine = s;
         }
         if (fm != a.frame) { frame_grad_flush(a, dR, dTh, lane); a.frame = fm; }
+        a.v += mine;
+        if (f == fm) f = kNone;
+    }
+}
+
+// Whole warp: per-frame sums of each lane's d loss / d(canonical point) dc for frame b (b < 0: nothing), subtracted from
+// d_bounds[frame, 0, :] (get_grid_coords subtracts bounds[:, 0] from the canonical point; row 1 is never read) with one
+// atomic per frame change, like frame_grad_add.  Lanes 0..2 hold the running sums.
+__device__ __forceinline__ void bounds_grad_flush(FrameGradAcc& a, float* __restrict__ d_bounds, int lane) {
+    if (a.frame >= 0 && a.v != 0.f && lane < 3) atomicAdd(d_bounds + (size_t)a.frame * 6 + lane, -a.v);
+    a.v = 0.f;
+}
+__device__ __forceinline__ void bounds_grad_add(FrameGradAcc& a, int b, const float (&dc)[3], float* __restrict__ d_bounds, int lane) {
+    constexpr int kNone = 0x7fffffff;
+    int f = b < 0 ? kNone : b;
+    for (;;) {
+        const int fm = __reduce_min_sync(0xffffffffu, f);
+        if (fm == kNone) break;
+        float mine = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            float s = f == fm ? dc[k] : 0.f;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == k) mine = s;
+        }
+        if (fm != a.frame) { bounds_grad_flush(a, d_bounds, lane); a.frame = fm; }
         a.v += mine;
         if (f == fm) f = kNone;
     }

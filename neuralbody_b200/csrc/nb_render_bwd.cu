@@ -1,7 +1,7 @@
 // Backward of the fused render (nb_render_bwd): gradients of rgb_map / depth_map / acc_map with respect to
 // the four dense feature volumes, every decoder parameter and the latent table; nb_render_bwd_frame adds the frame
 // transform R / Th, nb_render_bwd_rays also the rays ray_o / ray_d, nb_render_bwd_maps also the cotangents of disp_map
-// and weights.
+// and weights, nb_render_bwd_inputs also near / far, the sample depths and bounds.
 //
 // Upstream this is PyTorch autograd through raw2outputs (nerf_net_utils.py:6-51), the eight Conv1d layers
 // and F.grid_sample (latent_xyzc.py:62-126), driven by Trainer.train (lib/train/trainers/trainer.py:46-53).
@@ -12,7 +12,7 @@
 //                             features, then the trilinear scatter-add into the NCDHW volume grads
 //   3. wgrad_kernel (x6), colsum_kernel, view_wgrad_kernel     weight / bias gradients (split over points)
 //   4. unfold_* kernels       gradients of the folded Wc / bc back to feature_fc, latent_fc, view_fc, latent
-//   5. ray gradients only:    pe_grad_kernel (the positional encodings' part per point), ray_grad_kernel (per ray)
+//   5. ray / depth gradients only: pe_grad_kernel (the positional encodings' part per point), ray_grad_kernel (per ray)
 // Training chunks are small (N_rand = 1024 rays), so this path is sized for correctness and simplicity:
 // fp32 FFMA, no tensor cores; the forward hot path is untouched.
 #include "nb_device.cuh"
@@ -34,6 +34,8 @@ struct BwdParams {
     float* d_raw_out;               // composite backward writes d(rgb logits, sigma) of sample i at d_raw_out + i * d_raw_stride
     int d_raw_stride;
     float *d_ray_o, *d_ray_d;       // (B,n,3) ray gradients, accumulated into; either may be null
+    DepthGrads d_z;                 // d near / d far (B,n), d z (B,n,S), accumulated into; any may be null
+    float* d_bounds;                // (B,2,3): row 0 accumulated into; may be null
 };
 
 constexpr int kBwdMaxSamples = 256;     // coarse + importance samples of a fine pass (64 + 128) fit
@@ -68,7 +70,9 @@ __device__ __forceinline__ void disparity_bwd(float depth, float acc, float d_di
 //   weights:  g_i += d_weights_i -- exact, since w_i = alpha_i T_i is what the recurrences differentiate;
 //   disp_map: folded into dD / dA (disparity_bwd) at the depth and acc of the forward's own composite_ray, recomputed here
 //             so that max(1e-10, x) takes the forward's branch.  The white background does not enter disp.
-__device__ __forceinline__ void ray_bwd_recurrences(const BwdParams& Q, size_t ri, float nrm, RaySmem& sm, float (&dC)[3], int lane) {
+// dD_out (if given) receives the depth cotangent after the disp fold: what d z_i takes through depth_map = sum w z.
+__device__ __forceinline__ void ray_bwd_recurrences(const BwdParams& Q, size_t ri, float nrm, RaySmem& sm, float (&dC)[3], int lane,
+                                                    float* dD_out = nullptr) {
     const RenderParams& P = Q.f;
     const int S = P.n_samples;
     const float near = P.near[ri], far = P.far[ri];
@@ -86,6 +90,7 @@ __device__ __forceinline__ void ray_bwd_recurrences(const BwdParams& Q, size_t r
         const RayOut o = composite_ray(raw, sm.z, S, nrm, nullptr, lane);
         disparity_bwd(o.depth, o.acc, Q.d_disp[ri], dD, dA);
     }
+    if (dD_out) *dD_out = dD;
     const float* dW = Q.d_weights ? Q.d_weights + ri * S : nullptr;
     for (int s = lane; s < S; s += 32) {
         const float4 rw = raw[s];
@@ -144,7 +149,12 @@ __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdP
 // u = d / |d| and dists_i = delta_i |d| (nerf_net_utils.py:28):
 //   d o += sum_i g_i,   d d += sum_i z_i g_i + (du - u (u . du)) / |d| + u sum_i dL/d dists_i delta_i,
 // where du = sum_i du_i and dL/d dists_i = dalpha_i relu(sigma_i) e_i; z, dist and the T / U recurrences are those of
-// composite_bwd_kernel (ray_bwd_recurrences).  z is not differentiated (near / far and z_vals are not inputs of the gradient).
+// composite_bwd_kernel (ray_bwd_recurrences).
+// DEPTH (nb_render_bwd_inputs): also d z_i = r_i . d + dD w_i + |d| (c_{i-1} - c_i), with r_i the record's d loss / d(world
+// point), dD the depth cotangent after the disp fold and c_i = dL/d dists_i = dalpha_i relu(sigma_i) e_i (c_{S-1} = c_{-1} = 0:
+// the last dist is 1e10 |d|, independent of z).  It is added to Q.d_z.z and, with z_sample's coefficients, summed into
+// Q.d_z.near / .far.  A skipped sample has r = 0, w = 0 and relu(sigma) = 0, so skipping stays exact.
+template <bool DEPTH>
 __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams Q, const float* __restrict__ rec, int rec_stride) {
     __shared__ RaySmem s_ray[CB_WARPS];
     const RenderParams& P = Q.f;
@@ -156,7 +166,8 @@ __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams
     const float nrm = ray_norm(dx, dy, dz);
     RaySmem& sm = s_ray[warp];
     float dC[3];
-    ray_bwd_recurrences(Q, ri, nrm, sm, dC, lane);
+    float dD = 0.f;
+    ray_bwd_recurrences(Q, ri, nrm, sm, dC, lane, DEPTH ? &dD : nullptr);
     const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
     float go[3] = {0.f, 0.f, 0.f}, gd[3] = {0.f, 0.f, 0.f}, du[3] = {0.f, 0.f, 0.f}, dn = 0.f;
     for (int s = lane; s < S; s += 32) {
@@ -172,6 +183,28 @@ __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams
         const float* r = rec + (ri * S + s) * rec_stride;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { go[k] += r[k]; gd[k] = fmaf(z, r[k], gd[k]); du[k] += r[3 + k]; }
+        if constexpr (DEPTH) sm.f[s] = s + 1 < S ? dalpha * sg * e : 0.f;   // c_s (f is free after the recurrences)
+    }
+    if constexpr (DEPTH) {
+        __syncwarp();
+        const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
+        float dnear = 0.f, dfar = 0.f;
+        for (int s = lane; s < S; s += 32) {
+            const float* r = rec + (ri * S + s) * rec_stride;
+            const float w = sm.alpha[s] * sm.T[s];
+            const float dzs = fmaf(r[2], dz, fmaf(r[1], dy, r[0] * dx)) + dD * w + nrm * ((s > 0 ? sm.f[s - 1] : 0.f) - sm.f[s]);
+            if (Q.d_z.z) Q.d_z.z[ri * S + s] += dzs;
+            if (Q.d_z.near || Q.d_z.far) {
+                float cn, cf;
+                z_sample_coefs(P.t_vals, s, S, tr, cn, cf);
+                dnear = fmaf(cn, dzs, dnear);
+                dfar = fmaf(cf, dzs, dfar);
+            }
+        }
+        dnear = warp_sum(dnear);
+        dfar = warp_sum(dfar);
+        if (lane == 0 && Q.d_z.near) Q.d_z.near[ri] += dnear;
+        if (lane == 0 && Q.d_z.far) Q.d_z.far[ri] += dfar;
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { go[k] = warp_sum(go[k]); gd[k] = warp_sum(gd[k]); du[k] = warp_sum(du[k]); }
@@ -287,8 +320,34 @@ __device__ __forceinline__ void ray_pos_add(unsigned int ri, float z, const floa
     }
 }
 
-// RAYS: also the grid part of the ray gradients (nb_render_bwd_rays), from the same d loss / d(canonical point) as dR / dTh
-template <bool RAYS>
+// Whole warp, depth gradients: lane's sample s of ray ri (~0u: none) takes v = its grid part of d loss / d z.  Adds v to d z
+// (one writer per sample) and, for the ray, sum cn v / sum cf v to d near / d far with one atomic per ray and element.
+__device__ __forceinline__ void ray_depth_add(const BwdParams& Q, unsigned int ri, int s, float v, int lane) {
+    const RenderParams& P = Q.f;
+    const int S = P.n_samples;
+    if (ri != ~0u && Q.d_z.z) Q.d_z.z[(size_t)ri * S + s] += v;
+    if (!Q.d_z.near && !Q.d_z.far) return;
+    float cn = 0.f, cf = 0.f;
+    if (ri != ~0u) {
+        z_sample_coefs(P.t_vals, s, S, P.t_rand ? P.t_rand + (size_t)ri * S : nullptr, cn, cf);
+        cn *= v; cf *= v;
+    }
+    for (;;) {
+        const unsigned int rm = __reduce_min_sync(0xffffffffu, ri);
+        if (rm == ~0u) break;
+        const bool mine = ri == rm;
+        const float sn = warp_sum(mine ? cn : 0.f), sf = warp_sum(mine ? cf : 0.f);
+        if (lane == 0 && Q.d_z.near) atomicAdd(Q.d_z.near + rm, sn);
+        if (lane == 0 && Q.d_z.far) atomicAdd(Q.d_z.far + rm, sf);
+        if (mine) ri = ~0u;
+    }
+}
+
+// RAYS: also the grid part of the ray gradients (nb_render_bwd_rays), from the same d loss / d(canonical point) as dR / dTh.
+// INPUTS (with RAYS; nb_render_bwd_inputs): each of the ray, depth and bounds parts only when asked for -- the grid part of
+// d z (ray_depth_add: the records of this path hold d_h1pre until the weight gradients have read them, so it is added
+// straight into the outputs like the ray part) and d bounds[:, 0] = -sum d loss / d(canonical point) per frame.
+template <bool RAYS, bool INPUTS = false>
 __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q) {
     extern __shared__ __align__(16) float smem[];
     float* X = smem;                    // [64][356]
@@ -301,6 +360,7 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
     const float* wf = P.wf32;
     const bool frame_grads = RAYS || Q.d_R || Q.d_Th;   // any gradient with respect to the sample position
     FrameGradAcc acc;                   // warp 0: running per-frame sums of dR / dTh
+    FrameGradAcc acc_bounds;            // warp 0, INPUTS: of d bounds[:, 0]
     for (size_t tile = blockIdx.x; tile * TP < npts; tile += gridDim.x) {
         const size_t p0 = tile * TP;
         auto gp = [&](int p) { return p0 + p; };
@@ -402,6 +462,7 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                     const float* y = Y + (32 * h + tid) * 16;
                     const int b = __float_as_int(y[15]);
                     float t[12] = {};
+                    float dcan[3] = {0.f, 0.f, 0.f};    // INPUTS: d loss / d(canonical point)
                     if (b >= 0) {
                         FrameXf fx;
 #pragma unroll
@@ -411,6 +472,10 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                                     dcz = ((y[2] + y[5]) + y[8]) + y[11];
                         frame_grad_terms(fx, y[12], y[13], y[14], dcx * grid_to_can_scale(fx, 2), dcy * grid_to_can_scale(fx, 1),
                                          dcz * grid_to_can_scale(fx, 0), t);
+                        if constexpr (INPUTS) {
+                            dcan[0] = dcx * grid_to_can_scale(fx, 2); dcan[1] = dcy * grid_to_can_scale(fx, 1);
+                            dcan[2] = dcz * grid_to_can_scale(fx, 0);
+                        }
                     }
                     if (!RAYS || Q.d_R || Q.d_Th) frame_grad_add(acc, b, t, Q.d_R, Q.d_Th, tid);
                     if constexpr (RAYS) {   // d loss / d(world point) through the grid: R dc = -(the dTh term)
@@ -419,7 +484,16 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                         const float gw[3] = {-t[9], -t[10], -t[11]};
                         const float z = b < 0 ? 0.f : z_sample(P.near[ri], P.far[ri], P.t_vals, (int)(g % S), S,
                                                                P.t_rand ? P.t_rand + ri * S : nullptr, P.z_user ? P.z_user + ri * S : nullptr);
-                        ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
+                        if constexpr (!INPUTS) {
+                            ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
+                        } else {
+                            if (Q.d_ray_o || Q.d_ray_d) ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
+                            if (Q.d_z.any()) {
+                                const float v = b < 0 ? 0.f : fmaf(gw[2], P.ray_d[ri * 3 + 2], fmaf(gw[1], P.ray_d[ri * 3 + 1], gw[0] * P.ray_d[ri * 3]));
+                                ray_depth_add(Q, b < 0 ? ~0u : (unsigned int)ri, (int)(g % S), v, tid);
+                            }
+                            if (Q.d_bounds) bounds_grad_add(acc_bounds, b, dcan, Q.d_bounds, tid);
+                        }
                     }
                 }
             }
@@ -427,6 +501,7 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
         __syncthreads();
     }
     if (frame_grads && tid < 32) frame_grad_flush(acc, Q.d_R, Q.d_Th, tid);
+    if constexpr (INPUTS) if (Q.d_bounds && tid < 32) bounds_grad_flush(acc_bounds, Q.d_bounds, tid);
 }
 
 // ------------------------------------------------------------------------------------------ 3. weight gradients
@@ -614,12 +689,15 @@ void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCota
 }
 
 void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
-                     float* d_ray_o, float* d_ray_d, cudaStream_t stream) {
+                     float* d_ray_o, float* d_ray_d, const DepthGrads& dz, cudaStream_t stream) {
     bwd::BwdParams Q{};
     Q.f = p; Q.raw = raw; Q.d_rgb = d.rgb; Q.d_depth = d.depth; Q.d_acc = d.acc; Q.d_disp = d.disp; Q.d_weights = d.weights;
     Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
+    Q.d_z = dz;
     const size_t nrays = (size_t)p.batch * p.n_rays;
-    bwd::ray_grad_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
+    const unsigned grid = (unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS);
+    if (dz.any()) bwd::ray_grad_kernel<true><<<grid, bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
+    else bwd::ray_grad_kernel<false><<<grid, bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
 }
 
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
@@ -676,11 +754,27 @@ extern "C" int nb_render_bwd_rays(const nb_render_bwd_args* a, float* d_R, float
 
 extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_disp_map, const float* d_weights, float* d_R,
                                   float* d_Th, float* d_ray_o, float* d_ray_d, void* stream) {
+    nb_render_input_grads g{};
+    g.d_R = d_R; g.d_Th = d_Th; g.d_ray_o = d_ray_o; g.d_ray_d = d_ray_d;
+    return nb_render_bwd_inputs(a, d_disp_map, d_weights, &g, stream);
+}
+
+extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_disp_map, const float* d_weights,
+                                    const nb_render_input_grads* in, void* stream) {
     if (!a || !a->fwd || !a->save || !a->raw || !a->workspace || !a->weights || !a->grads) {
         set_error("nb_render_bwd: null argument");
         return NB_ERR_BAD_ARG;
     }
+    const nb_render_input_grads none{};
+    if (!in) in = &none;
+    float *d_R = in->d_R, *d_Th = in->d_Th, *d_ray_o = in->d_ray_o, *d_ray_d = in->d_ray_d;
+    const DepthGrads d_depths{in->d_near, in->d_far, in->d_z_vals};
     const nb_render_args* f = a->fwd;
+    if (f->z_vals && (in->d_near || in->d_far)) {
+        set_error("nb_render_bwd: d_near / d_far need a forward that derived its depths from near / far (z_vals was given: "
+                  "ask for d_z_vals)");
+        return NB_ERR_BAD_ARG;
+    }
     RenderParams p;
     int st = fill_frame_params(f, "nb_render_bwd", &p);
     if (st == NB_OK) st = fill_ray_params(f, "nb_render_bwd", &p);
@@ -694,6 +788,7 @@ extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_di
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
         for (int l = 0; l < 4; ++l) t.d_vol[l] = a->d_volumes[l];
         t.d_R = d_R; t.d_Th = d_Th; t.d_ray_o = d_ray_o; t.d_ray_d = d_ray_d; t.volume_dtype = f->volume_dtype;
+        t.d_depths = d_depths; t.d_bounds = in->d_bounds;
         return launch_train_bwd(p, t, (cudaStream_t)stream);
     }
     if (f->precision != NB_PRECISION_FP32 || f->volume_dtype != NB_DTYPE_F32) {
@@ -715,7 +810,8 @@ extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_di
     for (int l = 0; l < 4; ++l) Q.d_vol[l] = a->d_volumes[l];
     Q.d_R = d_R; Q.d_Th = d_Th;
     Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
-    const bool ray_grads = d_ray_o || d_ray_d;
+    Q.d_z = d_depths; Q.d_bounds = in->d_bounds;
+    const bool ray_grads = d_ray_o || d_ray_d, depth_grads = d_depths.any(), inputs = depth_grads || in->d_bounds;
     cudaStream_t s = (cudaStream_t)stream;
     const size_t nrays = (size_t)f->batch * f->n_rays, npts = nrays * f->n_samples;
     if (npts == 0) return NB_OK;
@@ -726,7 +822,10 @@ extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_di
     const size_t smem = ((size_t)bwd::TP * bwd::LDX + (size_t)bwd::TP * bwd::LDY + (size_t)bwd::KC * kFeat) * 4;
     const size_t ntiles = (npts + bwd::TP - 1) / bwd::TP;
     const unsigned dgrad_grid = (unsigned)(ntiles < kGridSMs ? ntiles : kGridSMs);
-    if (ray_grads) {   // + the grid part of the ray gradients, added straight into d_ray_o / d_ray_d
+    if (inputs) {      // + whichever of the grid parts of the ray, depth and bounds gradients was asked for
+        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        bwd::decoder_dgrad_kernel<true, true><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
+    } else if (ray_grads) {   // + the grid part of the ray gradients, added straight into d_ray_o / d_ray_d
         cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         bwd::decoder_dgrad_kernel<true><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
     } else {
@@ -769,12 +868,12 @@ extern "C" int nb_render_bwd_maps(const nb_render_bwd_args* a, const float* d_di
 
     st = launch_unfold(*a->weights, g, dWcx, dbc, T, dT, u, du, s);
     if (st != NB_OK) return st;
-    if (ray_grads) {   // the encodings' part per point into the d_h1pre columns (read by the weight / bias gradients above), then per ray
+    if (ray_grads || depth_grads) {   // the encodings' part per point into the d_h1pre columns (read by the weight / bias gradients above), then per ray
         float* rec = Q.ws + kGradH1;
         bwd::pe_grad_kernel<<<(unsigned)((npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS < (size_t)kGridSMs * 16
                                              ? (npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS : (size_t)kGridSMs * 16),
                               bwd::PG_WARPS * 32, 0, s>>>(Q, rec, kGradDim);
-        launch_ray_grad(p, a->raw, d_maps, rec, kGradDim, d_ray_o, d_ray_d, s);
+        launch_ray_grad(p, a->raw, d_maps, rec, kGradDim, d_ray_o, d_ray_d, d_depths, s);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_render_bwd: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

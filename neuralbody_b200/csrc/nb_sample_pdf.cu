@@ -14,10 +14,14 @@ namespace pdf {
 
 constexpr int MAX_COARSE = 256, MAX_TOTAL = 512, WARPS = 4;
 
-__global__ void __launch_bounds__(WARPS * 32) sample_pdf_kernel(const nb_importance_args A) {
+// SRC (nb_sample_pdf_src): each entry carries its origin (coarse index, -1 = importance sample) through the same swaps, so
+// z_out is the same bit for bit and z_src says where every entry came from
+template <bool SRC>
+__global__ void __launch_bounds__(WARPS * 32) sample_pdf_kernel(const nb_importance_args A, int* __restrict__ z_src) {
     __shared__ float zc_s[WARPS][MAX_COARSE];
     __shared__ float cdf_s[WARPS][MAX_COARSE];
     __shared__ float buf_s[WARPS][MAX_TOTAL];
+    __shared__ int src_s[SRC ? WARPS : 1][SRC ? MAX_TOTAL : 1];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long ray = (long long)blockIdx.x * WARPS + warp;
     if (ray >= A.n_rays_total) return;
@@ -61,6 +65,9 @@ __global__ void __launch_bounds__(WARPS * 32) sample_pdf_kernel(const nb_importa
     while (P < n) P <<= 1;
     for (int i = lane; i < S; i += 32) buf[i] = zc[i];
     for (int i = n + lane; i < P; i += 32) buf[i] = __int_as_float(0x7f800000);      // +inf padding sorts to the end
+    int* src = SRC ? src_s[warp] : nullptr;
+    if constexpr (SRC)
+        for (int i = lane; i < P; i += 32) src[i] = i < S ? i : -1;
     __syncwarp();
     for (int k = 2; k <= P; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
@@ -69,19 +76,26 @@ __global__ void __launch_bounds__(WARPS * 32) sample_pdf_kernel(const nb_importa
                 if (x > i) {
                     const float a = buf[i], b = buf[x];
                     const bool asc = (i & k) == 0;
-                    if ((a > b) == asc) { buf[i] = b; buf[x] = a; }
+                    if ((a > b) == asc) {
+                        buf[i] = b; buf[x] = a;
+                        if constexpr (SRC) { const int t = src[i]; src[i] = src[x]; src[x] = t; }
+                    }
                 }
             }
             __syncwarp();
         }
     }
     for (int i = lane; i < n; i += 32) A.z_out[ray * n + i] = buf[i];
+    if constexpr (SRC)
+        for (int i = lane; i < n; i += 32) z_src[ray * n + i] = src[i];
 }
 
 }  // namespace pdf
 }  // namespace nb
 
-extern "C" int nb_sample_pdf(const nb_importance_args* a, void* stream) {
+extern "C" int nb_sample_pdf(const nb_importance_args* a, void* stream) { return nb_sample_pdf_src(a, nullptr, stream); }
+
+extern "C" int nb_sample_pdf_src(const nb_importance_args* a, int* z_src, void* stream) {
     using namespace nb;
     if (!a) { set_error("nb_sample_pdf: null args"); return NB_ERR_BAD_ARG; }
     if (a->n_rays_total < 0 || a->n_samples < 3 || a->n_importance < 1) {
@@ -95,7 +109,8 @@ extern "C" int nb_sample_pdf(const nb_importance_args* a, void* stream) {
     if (!a->near || !a->far || !a->weights || !a->z_out) { set_error("nb_sample_pdf: a required device pointer is null"); return NB_ERR_BAD_ARG; }
     if (a->n_rays_total == 0) return NB_OK;
     const unsigned grid = (unsigned)((a->n_rays_total + pdf::WARPS - 1) / pdf::WARPS);
-    pdf::sample_pdf_kernel<<<grid, pdf::WARPS * 32, 0, (cudaStream_t)stream>>>(*a);
+    if (z_src) pdf::sample_pdf_kernel<true><<<grid, pdf::WARPS * 32, 0, (cudaStream_t)stream>>>(*a, z_src);
+    else pdf::sample_pdf_kernel<false><<<grid, pdf::WARPS * 32, 0, (cudaStream_t)stream>>>(*a, nullptr);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_sample_pdf launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     return NB_OK;

@@ -457,11 +457,13 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
 // layer's input gradient in columns kXyzCol..) and the sin / cos the forward saved in H2X.  dR / dTh may both be null then.
 constexpr int kPECols = kH2X - kXyzCol;     // [PE(xyz) 63 | 0 | PE(view) 27 | 0 x 5]
 constexpr int kRayRec = 8;
+// BOUNDS (nb_render_bwd_inputs): also d_bounds[b, 0, :] -= the per-frame sum of d loss / d(canonical point), the quantity
+// whose image under R is the dTh term, taken before R is applied.  dR / dTh may both be null then.
 // (RAYS: at least 2 CTAs per SM, so ptxas does not squeeze it into 64 registers and spill; 0 = no minimum, as before)
-template <typename VT, bool RAYS>
+template <typename VT, bool RAYS, bool BOUNDS = false>
 __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
                                                          float* __restrict__ dR, float* __restrict__ dTh, const float* __restrict__ dPE,
-                                                         float* __restrict__ rec) {
+                                                         float* __restrict__ rec, float* __restrict__ d_bounds = nullptr) {
     __shared__ float gc[GP][3], dc[GP][3];
     __shared__ int fr[GP];
     __shared__ float pe[RAYS ? 2 : 1][GP][3];   // RAYS: [PE(xyz) | PE(view)][entry][axis]
@@ -469,6 +471,7 @@ __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __g
     const unsigned int spf = (unsigned int)P.n_rays * P.n_samples;
     const int tid = threadIdx.x;
     FrameGradAcc acc;
+    FrameGradAcc acc_bounds;                    // BOUNDS: warp 0's running per-frame sums of d bounds[:, 0]
     for (unsigned int e0 = blockIdx.x * GP; e0 < count; e0 += gridDim.x * GP) {
         if (tid < GP) {
             fr[tid] = -1;
@@ -515,6 +518,7 @@ __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __g
         __syncthreads();
         if (tid < 32) {
             float t[12] = {};
+            float dcan[3] = {0.f, 0.f, 0.f};    // BOUNDS: d loss / d(canonical point)
             const int b = fr[tid];
             if (b >= 0) {
                 const float4 en = sv.list[e0 + tid];
@@ -524,17 +528,23 @@ __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __g
                 // grid x / y / z pair with the dhw axes 2 / 1 / 0
                 frame_grad_terms(fx, en.x, en.y, en.z, dc[tid][0] * grid_to_can_scale(fx, 2), dc[tid][1] * grid_to_can_scale(fx, 1),
                                  dc[tid][2] * grid_to_can_scale(fx, 0), t);
+                if constexpr (BOUNDS) {
+                    dcan[0] = dc[tid][0] * grid_to_can_scale(fx, 2); dcan[1] = dc[tid][1] * grid_to_can_scale(fx, 1);
+                    dcan[2] = dc[tid][2] * grid_to_can_scale(fx, 0);
+                }
                 if constexpr (RAYS) {   // the grid part R dc is -(the dTh term)
                     float* r = rec + (size_t)(__float_as_uint(en.w) & kListIdMask) * kRayRec;
 #pragma unroll
                     for (int k = 0; k < 3; ++k) { r[k] = pe[0][tid][k] - t[9 + k]; r[3 + k] = pe[1][tid][k]; }
                 }
             }
-            if (!RAYS || dR || dTh) frame_grad_add(acc, b, t, dR, dTh, tid);
+            if (!(RAYS || BOUNDS) || dR || dTh) frame_grad_add(acc, b, t, dR, dTh, tid);
+            if constexpr (BOUNDS) bounds_grad_add(acc_bounds, b, dcan, d_bounds, tid);
         }
         __syncthreads();
     }
     if (tid < 32) frame_grad_flush(acc, dR, dTh, tid);
+    if constexpr (BOUNDS) if (tid < 32) bounds_grad_flush(acc_bounds, d_bounds, tid);
 }
 
 // d_vol[b][c][v] += blob[b][v][c] for one level: 32 voxels x 32 channels through shared memory
@@ -720,7 +730,9 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     a.a = G1; a.b = w.fc1_w; a.c = G0; a.mask = sv.H0;
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
-    const bool frame_grads = t.d_R || t.d_Th, ray_grads = t.d_ray_o || t.d_ray_d;
+    const bool frame_grads = t.d_R || t.d_Th || t.d_bounds;
+    // any depth gradient needs the per-sample records of the ray gradients (d z_i takes d loss / d(world point) along ray_d)
+    const bool ray_grads = t.d_ray_o || t.d_ray_d || t.d_depths.any();
     if (t.d_vol[0] || frame_grads || ray_grads) {
         a.a = G0; a.b = w.fc0_w; a.ldb = kFeat; a.N = kFeat; a.c = DF; a.ldc = kFeat; a.mask = nullptr;
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
@@ -737,8 +749,15 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
         }
     }
     if (frame_grads && !ray_grads) {   // 4b. the frame transform's gradients, from the same DF (with ray gradients: step 8)
-        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
-        else frame_grad_kernel<__half, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
+        const bool f32 = t.volume_dtype == NB_DTYPE_F32;
+        if (t.d_bounds) {
+            if (f32) frame_grad_kernel<float, false, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr, t.d_bounds);
+            else frame_grad_kernel<__half, false, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr, t.d_bounds);
+        } else if (f32) {
+            frame_grad_kernel<float, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
+        } else {
+            frame_grad_kernel<__half, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
+        }
     }
     // 5. weight gradients: dW[out][in] += G^T X, split over the list
     const int splits = 74;      // 2 x 2 tiles x 74 = two CTAs on every SM
@@ -772,9 +791,16 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
         a.a = G3; a.lda = kWS; a.b = sv.wcol + kXyzCol; a.ldb = kH2X; a.N = kPECols; a.K = kWS; a.c = dPE; a.ldc = kPECols; a.mask = nullptr;
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
         cudaMemsetAsync(rec, 0, pmax * kRayRec * 4, stream);
-        if (t.volume_dtype == NB_DTYPE_F32) frame_grad_kernel<float, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
-        else frame_grad_kernel<__half, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
-        launch_ray_grad(p, t.raw, t.d_maps, rec, kRayRec, t.d_ray_o, t.d_ray_d, stream);
+        const bool f32 = t.volume_dtype == NB_DTYPE_F32;
+        if (t.d_bounds) {
+            if (f32) frame_grad_kernel<float, true, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec, t.d_bounds);
+            else frame_grad_kernel<__half, true, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec, t.d_bounds);
+        } else if (f32) {
+            frame_grad_kernel<float, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
+        } else {
+            frame_grad_kernel<__half, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
+        }
+        launch_ray_grad(p, t.raw, t.d_maps, rec, kRayRec, t.d_ray_o, t.d_ray_d, t.d_depths, stream);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("train bwd launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

@@ -8,6 +8,13 @@ namespace nb {
 // rgb (B,n,3), depth / acc / disp (B,n), weights (B,n,S)
 struct MapCotangents { const float *rgb, *depth, *acc, *disp, *weights; };
 
+// the depth gradients a backward call was asked for (device, accumulated into; any may be null): d near / d far (B,n), only
+// after a forward that derived z from them, and d z (B,n,S) per sample
+struct DepthGrads {
+    float *near, *far, *z;
+    __host__ __device__ bool any() const { return near || far || z; }
+};
+
 namespace trn {
 
 constexpr int kH2X = 352;                   // colour-layer input record: [h2 256 | PE(xyz) 63 | 0 | PE(viewdir) 27 | 0 x 5]
@@ -51,7 +58,9 @@ struct TrainBwd {
     float* d_vol[4];
     float *d_R, *d_Th;               // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
     float *d_ray_o, *d_ray_d;        // (B,n,3) ray gradients, accumulated into; either may be null
-    int volume_dtype;                // of the forward's volume blob (the frame-gradient pass reads it)
+    DepthGrads d_depths;             // near / far / sample-depth gradients, accumulated into; any may be null
+    float* d_bounds;                 // (B,2,3): row 0 accumulated into; may be null
+    int volume_dtype;               // of the forward's volume blob (the frame-gradient pass reads it)
     float* workspace;
 };
 
@@ -69,9 +78,11 @@ void launch_composite(const RenderParams& p, cudaStream_t stream);   // nb_rende
 void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCotangents& d, float* d_raw_out, int d_raw_stride,
                           cudaStream_t stream);                                        // nb_render_bwd.cu
 // per ray: the per-sample records rec + i * rec_stride = [d / d(world point) 3 | d / d(view direction) 3] plus the compositing
-// term -> d_ray_o / d_ray_d (accumulated into; either may be null)                                              nb_render_bwd.cu
+// term -> d_ray_o / d_ray_d (accumulated into; either may be null); with any depth gradient asked for, also d z per sample
+// (the records' world-point part along ray_d, the depth map and the dists) -> dz.z and, through z_sample, dz.near / dz.far
+//                                                                                                                  nb_render_bwd.cu
 void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
-                     float* d_ray_o, float* d_ray_d, cudaStream_t stream);
+                     float* d_ray_o, float* d_ray_d, const DepthGrads& dz, cudaStream_t stream);
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
                   float* u, float* du, cudaStream_t stream);                          // nb_render_bwd.cu
 

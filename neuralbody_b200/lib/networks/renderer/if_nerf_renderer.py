@@ -38,8 +38,9 @@ class _FusedRender(torch.autograd.Function):
     does not read costs nothing (its cotangent stays None and the kernels get NULL).  disp_map follows upstream's NaN
     rule: on a ray with acc_map == 0 its gradient is NaN, which reaches ray_d only (see nb_render_bwd_maps).
     Differentiable inputs: the four dense volumes (so gradients keep flowing into the reference's SparseConvNet / code
-    embedding), the 17 decoder tensors, the frame transform sp_input['R'] / ['Th'] (pose refinement) and the rays
-    ray_o / ray_d (camera refinement)."""
+    embedding), the 17 decoder tensors, the frame transform sp_input['R'] / ['Th'] (pose refinement), the rays
+    ray_o / ray_d (camera refinement), and near / far, sp_input['bounds'] and a caller-supplied z_vals (None in the
+    slots a call does not have: near / far are not read when z_vals is given)."""
 
     @staticmethod
     def forward(ctx, renderer, call, *tensors):
@@ -219,8 +220,9 @@ class Renderer:
     def render_rays(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, want_raw=False,
                     out=None, trace=None, masks=None, z_vals=None, want_weights=None):
         """One nb_render_fwd launch for (B,n) rays.  Returns the dict of get_pixel_value.
-        When autograd is recording and any volume / decoder tensor, sp_input['R'] / ['Th'] or ray_o / ray_d requires grad, the
-        call goes through the training precision and `_FusedRender` so that `loss.backward()` works as it does upstream."""
+        When autograd is recording and any volume / decoder tensor, sp_input['R'] / ['Th'] / ['bounds'], ray_o / ray_d,
+        near / far (or z_vals, when given) requires grad, the call goes through the training precision and `_FusedRender` so
+        that `loss.backward()` works as it does upstream."""
         cfg = get_active_cfg()
         if int(self._opt("xyz_res", 10)) != 10 or int(self._opt("view_res", 4)) != 4:
             # embedder.py:53-54: the kernels (and view_fc's 346 input columns) are built for PE widths 63 / 27
@@ -235,10 +237,14 @@ class Renderer:
         S = int(cfg.N_samples) if z_vals is None else int(z_vals.shape[-1])   # z_vals: caller-supplied depths (fine pass, f-4)
         params = self.net.decoder_tensors()
         frame = [sp_input['R'], sp_input['Th']]
+        # near, far, bounds, z_vals: the depth inputs (near / far are not read when the caller gives the depths)
+        depths = [near if z_vals is None else None, far if z_vals is None else None, sp_input['bounds'], z_vals]
+        depths = [t if torch.is_tensor(t) else None for t in depths]
         needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
                                                   any(v.requires_grad for v in feature_volume) or
                                                   any(torch.is_tensor(t) and t.requires_grad for t in frame) or
-                                                  ray_o.requires_grad or ray_d.requires_grad)
+                                                  ray_o.requires_grad or ray_d.requires_grad or
+                                                  any(t is not None and t.requires_grad for t in depths))
         precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
@@ -251,8 +257,10 @@ class Renderer:
             t_rand = self._draw_t_rand(B, n, S, dev)
         call = {
             "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": self._volume_dtype(precision),
-            "ray_o": _f32c(ray_o.detach(), dev), "ray_d": _f32c(ray_d.detach(), dev), "near": _f32c(near, dev), "far": _f32c(far, dev),
+            "ray_o": _f32c(ray_o.detach(), dev), "ray_d": _f32c(ray_d.detach(), dev),
+            "near": _f32c(near.detach(), dev), "far": _f32c(far.detach(), dev),
             "ray_like": [(t.shape, t.dtype, t.device) for t in (ray_o, ray_d)],
+            "depth_like": [None if t is None else (t.shape, t.dtype, t.device) for t in depths],
             "sp_input": sp_input, "t_rand": None if t_rand is None else _f32c(t_rand, dev), "white_bkgd": bool(cfg.white_bkgd),
             "z_vals": None if z_vals is None else _f32c(z_vals.detach(), dev),
             "feature_volume": list(feature_volume), "want_raw": want_raw or needs_grad, "user_raw": bool(want_raw), "out": out, "trace": trace,
@@ -272,7 +280,8 @@ class Renderer:
         if call["t_rand"] is not None:
             assert tuple(call["t_rand"].shape) == (B, n, S)
         if needs_grad:
-            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame, ray_o, ray_d)
+            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame, ray_o, ray_d,
+                                                                *depths)
             ret = {'rgb_map': rgb, 'disp_map': disp, 'acc_map': acc, 'weights': weights, 'depth_map': depth}
             if want_raw:
                 ret['raw'] = call["raw"]
@@ -407,8 +416,9 @@ class Renderer:
         return out
 
     def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs, d_disp=None, d_weights=None):
-        """nb_render_bwd_maps: gradients for (volumes..., decoder tensors..., R, Th, ray_o, ray_d) in the order of
-        _FusedRender.apply, from the cotangents of the five maps (None: the loss does not read that map)."""
+        """nb_render_bwd_maps, or nb_render_bwd_inputs when a depth input needs a gradient: gradients for (volumes...,
+        decoder tensors..., R, Th, ray_o, ray_d, near, far, bounds, z_vals) in the order of _FusedRender.apply, from the
+        cotangents of the five maps (None: the loss does not read that map)."""
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         if call.get("save") is None:
             raise RuntimeError("the activation record of this render call was already consumed by a backward pass "
@@ -441,15 +451,28 @@ class Renderer:
             for l in range(capi.NB_NUM_LEVELS):
                 ba.d_volumes[l] = gvols[l].data_ptr() if want_vol else None
             ba.workspace, ba.workspace_bytes = ws.data_ptr(), nbytes
+            k0 = len(vols) + len(params)
             # frame transform (pose refinement): fp32 (B,3,3) / (B,3) accumulators, only for the inputs autograd asks about
-            want_R, want_Th = needs[-4], needs[-3]
+            want_R, want_Th = needs[k0], needs[k0 + 1]
             dR = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev) if want_R else None
             dTh = torch.zeros((B, 3), dtype=torch.float32, device=dev) if want_Th else None
             # rays (camera refinement): fp32 (B,n,3) accumulators, likewise
-            drays = [torch.zeros((B, n, 3), dtype=torch.float32, device=dev) if want else None for want in needs[-2:]]
+            drays = [torch.zeros((B, n, 3), dtype=torch.float32, device=dev) if want else None for want in needs[k0 + 2:k0 + 4]]
+            # near, far (B,n), bounds (B,2,3), z_vals (B,n,S)
+            shapes = ((B, n), (B, n), (B, 2, 3), (B, n, S))
+            ddepths = [torch.zeros(sh, dtype=torch.float32, device=dev) if want else None
+                       for sh, want in zip(shapes, needs[k0 + 4:k0 + 8])]
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_render_bwd_maps(C.byref(ba), _ptr(d_disp), _ptr(d_weights), _ptr(dR), _ptr(dTh),
-                                                   _ptr(drays[0]), _ptr(drays[1]), C.c_void_p(stream)), "nb_render_bwd_maps")
+            if any(d is not None for d in ddepths):
+                ig = capi.nb_render_input_grads()
+                for name, t in zip(("d_R", "d_Th", "d_ray_o", "d_ray_d", "d_near", "d_far", "d_bounds", "d_z_vals"),
+                                   [dR, dTh] + drays + ddepths):
+                    setattr(ig, name, t.data_ptr() if t is not None else None)
+                capi.check(self.lib.nb_render_bwd_inputs(C.byref(ba), _ptr(d_disp), _ptr(d_weights), C.byref(ig),
+                                                         C.c_void_p(stream)), "nb_render_bwd_inputs")
+            else:
+                capi.check(self.lib.nb_render_bwd_maps(C.byref(ba), _ptr(d_disp), _ptr(d_weights), _ptr(dR), _ptr(dTh),
+                                                       _ptr(drays[0]), _ptr(drays[1]), C.c_void_p(stream)), "nb_render_bwd_maps")
             # stream-ordered reuse: the next forward / backward on this stream runs after the kernels just enqueued
             self._pool_give("bwd_ws", ws)
             self._pool_give("save", call.pop("save"))
@@ -463,7 +486,9 @@ class Renderer:
             dTh = dTh.to(device=Th.device, dtype=Th.dtype).view(Th.shape)
         drays = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])   # the caller's shape, dtype and device
                  for d, like in zip(drays, call["ray_like"])]
-        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh] + drays
+        ddepths = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])
+                   for d, like in zip(ddepths, call["depth_like"])]
+        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh] + drays + ddepths
         return [gr if need else None for gr, need in zip(grads, needs)]
 
     def _weights_struct(self, tensors, latent_index, device):
@@ -547,14 +572,19 @@ class Renderer:
     def importance_z_vals(self, near, far, weights, n_samples, n_importance, t_rand=None, u=None):
         """z_vals_mid + sample_pdf + sort-merge (volume_renderer.py:84-93, nerf_net_utils.py:55-90) as one nb_sample_pdf launch.
         weights (B,n,S) from the coarse pass; t_rand its jitter (or None); u (B,n,n_importance) uniforms or None for the
-        deterministic branch.  Returns (z_all (B,n,S+n_importance) ascending, z_samples (B,n,n_importance))."""
+        deterministic branch.  Returns (z_all (B,n,S+n_importance) ascending, z_samples (B,n,n_importance)).
+        When autograd is recording and near or far requires grad, z_all is an autograd node: as upstream's
+        sort(cat(z_vals, z_samples.detach())), each entry that came from the coarse depths (nb_sample_pdf_src says which)
+        passes its gradient to that coarse depth and so to near / far; the importance samples get none."""
         dev = weights.device
         B, n, S = int(weights.shape[0]), int(weights.shape[1]), int(n_samples)
         Ni = int(n_importance)
+        routed = torch.is_grad_enabled() and (near.requires_grad or far.requires_grad)
         with torch.cuda.device(dev), torch.no_grad():
             z_all = torch.empty((B, n, S + Ni), dtype=torch.float32, device=dev)
             z_smp = torch.empty((B, n, Ni), dtype=torch.float32, device=dev)
-            keep = [_f32c(near, dev), _f32c(far, dev), self._t_vals(S, dev), _f32c(weights.detach(), dev),
+            z_src = torch.empty((B, n, S + Ni), dtype=torch.int32, device=dev) if routed else None
+            keep = [_f32c(near.detach(), dev), _f32c(far.detach(), dev), self._t_vals(S, dev), _f32c(weights.detach(), dev),
                     None if t_rand is None else _f32c(t_rand, dev), None if u is None else _f32c(u, dev)]
             a = capi.nb_importance_args()
             a.n_rays_total, a.n_samples, a.n_importance = B * n, S, Ni
@@ -563,9 +593,31 @@ class Renderer:
             a.u = keep[5].data_ptr() if keep[5] is not None else None
             a.z_out, a.z_samples = z_all.data_ptr(), z_smp.data_ptr()
             stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_sample_pdf(C.byref(a), C.c_void_p(stream)), "nb_sample_pdf")
+            if routed:
+                capi.check(self.lib.nb_sample_pdf_src(C.byref(a), z_src.data_ptr(), C.c_void_p(stream)), "nb_sample_pdf_src")
+            else:
+                capi.check(self.lib.nb_sample_pdf(C.byref(a), C.c_void_p(stream)), "nb_sample_pdf")
             self.launches += 1
+        if routed:
+            # z_all + (c - c.detach()): the value stays the kernel's bit for bit, the gradient reaches the coarse depths
+            src = z_src.long()
+            zc = self._coarse_z(near, far, S, t_rand, dev).gather(-1, src.clamp(min=0))
+            zc = torch.where(src >= 0, zc, torch.zeros_like(zc))
+            z_all = z_all + (zc - zc.detach())
         return z_all, z_smp
+
+    def _coarse_z(self, near, far, S, t_rand, dev):
+        """The coarse pass's depths as differentiable torch ops of near / far (if_clight_renderer.py:13-23; the kernels derive
+        the same values in z_sample): (B,n,S)."""
+        near, far = near.to(device=dev, dtype=torch.float32), far.to(device=dev, dtype=torch.float32)
+        t_vals = self._t_vals(S, dev)
+        z = near[..., None] * (1. - t_vals) + far[..., None] * t_vals
+        if t_rand is not None:
+            mids = .5 * (z[..., 1:] + z[..., :-1])
+            upper = torch.cat([mids, z[..., -1:]], -1)
+            lower = torch.cat([z[..., :1], mids], -1)
+            z = lower + (upper - lower) * t_rand.to(device=dev, dtype=torch.float32)
+        return z
 
     def render_rays_hierarchical(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, u=None):
         """Coarse pass (cfg.N_samples) -> importance samples from its weights -> fine pass over the merged depths with the SAME

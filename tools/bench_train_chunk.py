@@ -5,9 +5,10 @@ both passes.  Prints one JSON line (rays/s for fwd+bwd).
 With --frame-grads the same process alternates steps without and with gradients for the frame transform
 (sp_input['R'] / ['Th'] requiring grad, as pose refinement does) and reports both step times; --ray-grads does the same
 with ray_o / ray_d requiring grad (camera refinement), --map-grads with a loss that also reads disp_map, disp0 and the fine
-weights (an entropy regulariser on the ray weights and a disparity term, as distortion / smoothness losses do).
+weights (an entropy regulariser on the ray weights and a disparity term, as distortion / smoothness losses do),
+--depth-grads with near, far and sp_input['bounds'] requiring grad (the box-intersection near / far of refined cameras).
 Usage: python tools/bench_train_chunk.py [n_importance=128] [iters=30] [--frame-grads] [--ray-grads] [--map-grads]
-                                         [--precision tc_tf32x3|fp32]"""
+                                         [--depth-grads] [--precision tc_tf32x3|fp32]"""
 import json
 import os
 import sys
@@ -23,6 +24,7 @@ def main():
     frame_grads = "--frame-grads" in args
     ray_grads = "--ray-grads" in args
     map_grads = "--map-grads" in args
+    depth_grads = "--depth-grads" in args
     precision = "tc_tf32x3"
     if "--precision" in args:
         precision = args[args.index("--precision") + 1]
@@ -50,6 +52,9 @@ def main():
     pose = dict(batch, R=batch["R"].clone().requires_grad_(True), Th=batch["Th"].clone().requires_grad_(True))
     sp_pose = ren.prepare_sp_input(pose)
     cam = dict(batch, ray_o=batch["ray_o"].clone().requires_grad_(True), ray_d=batch["ray_d"].clone().requires_grad_(True))
+    depth = dict(batch, near=batch["near"].clone().requires_grad_(True), far=batch["far"].clone().requires_grad_(True),
+                 bounds=batch["bounds"].clone().requires_grad_(True))
+    sp_depth = ren.prepare_sp_input(depth)
     target = torch.rand((1, 1024, 3), device="cuda")
 
     def step(mode):
@@ -57,8 +62,9 @@ def main():
             p.grad = None
         for v in vols:
             v.grad = None
-        s, b = {"plain": (sp, batch), "frame": (sp_pose, pose), "rays": (sp, cam), "maps": (sp, batch)}[mode]
+        s, b = {"plain": (sp, batch), "frame": (sp_pose, pose), "rays": (sp, cam), "maps": (sp, batch), "depths": (sp_depth, depth)}[mode]
         b["R"].grad = b["Th"].grad = b["ray_o"].grad = b["ray_d"].grad = None
+        b["near"].grad = b["far"].grad = b["bounds"].grad = None
         out = ren.get_pixel_value(b["ray_o"], b["ray_d"], b["near"], b["far"], vols, s, b)
         loss = ((out["rgb_map"] - target) ** 2).mean()
         if "rgb0" in out:
@@ -70,7 +76,8 @@ def main():
                 loss = loss + 1e-3 * torch.where(out[a] > 0, out[d], torch.zeros_like(out[d])).mean()
         loss.backward()
 
-    modes = ("plain",) + (("frame",) if frame_grads else ()) + (("rays",) if ray_grads else ()) + (("maps",) if map_grads else ())
+    modes = ("plain",) + (("frame",) if frame_grads else ()) + (("rays",) if ray_grads else ()) + (("maps",) if map_grads else ()) + \
+        (("depths",) if depth_grads else ())
     for _ in range(5):
         for m in modes:
             step(m)
@@ -101,6 +108,11 @@ def main():
     if map_grads:
         res["ms_per_step_map_grads"] = ms["maps"]
         res["map_grads_overhead_ms"] = ms["maps"] - ms["plain"]
+    if depth_grads:
+        res["ms_per_step_depth_grads"] = ms["depths"]
+        res["depth_grads_overhead_ms"] = ms["depths"] - ms["plain"]
+        res["d_near_norm"], res["d_far_norm"] = float(depth["near"].grad.norm()), float(depth["far"].grad.norm())
+        res["d_bounds_norm"] = float(depth["bounds"].grad.norm())
     print(json.dumps(res))
 
 
