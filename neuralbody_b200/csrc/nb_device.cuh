@@ -227,13 +227,14 @@ __device__ __forceinline__ void frame_grad_terms(const FrameXf& f, float wx, flo
     }
 }
 
-// Per-frame sums of the 12 frame-transform gradients (dR 9, dTh 3) across one warp's calls: lane k < 12 holds element k of
-// the running frame's sum and adds it to the caller's dR / dTh (either may be null) with one atomic when the frame changes.
+// Per-frame sums of N values across one warp's calls: lane k < N holds element k of the running frame's sum and hands it to
+// the caller's flush, which adds it to its destination with one atomic, when the frame changes (and once at the end).
 // Callers that visit frames in order (sample lists are frame-major) therefore issue one atomic per warp, frame and element.
 struct FrameGradAcc {
     int frame = -1;
     float v = 0.f;
 };
+// the 12 terms of frame_grad_terms -> dR (B,3,3) / dTh (B,3), either may be null
 __device__ __forceinline__ void frame_grad_flush(FrameGradAcc& a, float* __restrict__ dR, float* __restrict__ dTh, int lane) {
     if (a.frame >= 0 && a.v != 0.f) {
         if (lane < 9 && dR) atomicAdd(dR + (size_t)a.frame * 9 + lane, a.v);
@@ -241,9 +242,15 @@ __device__ __forceinline__ void frame_grad_flush(FrameGradAcc& a, float* __restr
     }
     a.v = 0.f;
 }
+// d loss / d(canonical point) -> -d_bounds[frame, 0, :] (get_grid_coords subtracts bounds[:, 0] from the canonical point;
+// row 1 is never read)
+__device__ __forceinline__ void bounds_grad_flush(FrameGradAcc& a, float* __restrict__ d_bounds, int lane) {
+    if (a.frame >= 0 && a.v != 0.f && lane < 3) atomicAdd(d_bounds + (size_t)a.frame * 6 + lane, -a.v);
+    a.v = 0.f;
+}
 // Whole warp: each lane contributes t for frame b (b < 0: nothing).
-__device__ __forceinline__ void frame_grad_add(FrameGradAcc& a, int b, const float (&t)[12], float* __restrict__ dR,
-                                               float* __restrict__ dTh, int lane) {
+template <int N, typename Flush>
+__device__ __forceinline__ void frame_sum_add(FrameGradAcc& a, int b, const float (&t)[N], int lane, Flush&& flush) {
     constexpr int kNone = 0x7fffffff;
     int f = b < 0 ? kNone : b;
     for (;;) {
@@ -251,40 +258,13 @@ __device__ __forceinline__ void frame_grad_add(FrameGradAcc& a, int b, const flo
         if (fm == kNone) break;
         float mine = 0.f;
 #pragma unroll
-        for (int k = 0; k < 12; ++k) {
+        for (int k = 0; k < N; ++k) {
             float s = f == fm ? t[k] : 0.f;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
             if (lane == k) mine = s;
         }
-        if (fm != a.frame) { frame_grad_flush(a, dR, dTh, lane); a.frame = fm; }
-        a.v += mine;
-        if (f == fm) f = kNone;
-    }
-}
-
-// Whole warp: per-frame sums of each lane's d loss / d(canonical point) dc for frame b (b < 0: nothing), subtracted from
-// d_bounds[frame, 0, :] (get_grid_coords subtracts bounds[:, 0] from the canonical point; row 1 is never read) with one
-// atomic per frame change, like frame_grad_add.  Lanes 0..2 hold the running sums.
-__device__ __forceinline__ void bounds_grad_flush(FrameGradAcc& a, float* __restrict__ d_bounds, int lane) {
-    if (a.frame >= 0 && a.v != 0.f && lane < 3) atomicAdd(d_bounds + (size_t)a.frame * 6 + lane, -a.v);
-    a.v = 0.f;
-}
-__device__ __forceinline__ void bounds_grad_add(FrameGradAcc& a, int b, const float (&dc)[3], float* __restrict__ d_bounds, int lane) {
-    constexpr int kNone = 0x7fffffff;
-    int f = b < 0 ? kNone : b;
-    for (;;) {
-        const int fm = __reduce_min_sync(0xffffffffu, f);
-        if (fm == kNone) break;
-        float mine = 0.f;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            float s = f == fm ? dc[k] : 0.f;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-            if (lane == k) mine = s;
-        }
-        if (fm != a.frame) { bounds_grad_flush(a, d_bounds, lane); a.frame = fm; }
+        if (fm != a.frame) { flush(a); a.frame = fm; }
         a.v += mine;
         if (f == fm) f = kNone;
     }
@@ -391,6 +371,24 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// Whole warp, per-ray sums: each lane contributes v to its ray ri (~0u: none); the lanes of one ray are summed first and
+// lane 0 hands element k of the sum to put(ray, k, sum).  A warp holds consecutive samples, so that is one atomic per ray and
+// element, and a ray inside one warp gets its sum in a single call.
+template <int N, typename Put>
+__device__ __forceinline__ void ray_sum_add(unsigned int ri, const float (&v)[N], int lane, Put&& put) {
+    for (;;) {
+        const unsigned int rm = __reduce_min_sync(0xffffffffu, ri);
+        if (rm == ~0u) break;
+        const bool mine = ri == rm;
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+            const float s = warp_sum(mine ? v[k] : 0.f);
+            if (lane == 0) put(rm, k, s);
+        }
+        if (mine) ri = ~0u;
+    }
 }
 
 __device__ __forceinline__ RayOut composite_ray(const float4* __restrict__ raw, const float* __restrict__ z, int S,

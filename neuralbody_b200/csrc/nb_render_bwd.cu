@@ -25,17 +25,12 @@ struct BwdParams {
     RenderParams f;                 // the forward call's parameters (rays, transforms, packed weights)
     const float* save;              // (B,n,S,kSaveDim)
     const float* raw;               // (B,n,S,4)
-    const float *d_rgb, *d_depth, *d_acc;   // any may be null
-    const float *d_disp, *d_weights;        // (B,n) / (B,n,S); either may be null
+    GradRequest req;                // the map cotangents and the input gradients (accumulated into)
     float* ws;                      // (B*n*S, kGradDim) scratch
     nb_decoder_weights w;           // raw decoder tensors
     float* d_vol[4];                // NCDHW fp32, caller-zeroed, accumulated into
-    float *d_R, *d_Th;              // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
     float* d_raw_out;               // composite backward writes d(rgb logits, sigma) of sample i at d_raw_out + i * d_raw_stride
     int d_raw_stride;
-    float *d_ray_o, *d_ray_d;       // (B,n,3) ray gradients, accumulated into; either may be null
-    DepthGrads d_z;                 // d near / d far (B,n), d z (B,n,S), accumulated into; any may be null
-    float* d_bounds;                // (B,2,3): row 0 accumulated into; may be null
 };
 
 constexpr int kBwdMaxSamples = 256;     // coarse + importance samples of a fine pass (64 + 128) fit
@@ -79,19 +74,20 @@ __device__ __forceinline__ void ray_bwd_recurrences(const BwdParams& Q, size_t r
     const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
     const float* zu = P.z_user ? P.z_user + ri * S : nullptr;
     const float4* raw = reinterpret_cast<const float4*>(Q.raw) + ri * S;
+    const MapCotangents& d = Q.req.maps;
     dC[0] = dC[1] = dC[2] = 0.f;
-    if (Q.d_rgb) { dC[0] = Q.d_rgb[ri * 3]; dC[1] = Q.d_rgb[ri * 3 + 1]; dC[2] = Q.d_rgb[ri * 3 + 2]; }
-    float dD = Q.d_depth ? Q.d_depth[ri] : 0.f;
-    float dA = Q.d_acc ? Q.d_acc[ri] : 0.f;
+    if (d.rgb) { dC[0] = d.rgb[ri * 3]; dC[1] = d.rgb[ri * 3 + 1]; dC[2] = d.rgb[ri * 3 + 2]; }
+    float dD = d.depth ? d.depth[ri] : 0.f;
+    float dA = d.acc ? d.acc[ri] : 0.f;
     if (P.white_bkgd) dA -= dC[0] + dC[1] + dC[2];            // rgb_map += 1 - acc_map
     for (int s = lane; s < S; s += 32) sm.z[s] = z_sample(near, far, P.t_vals, s, S, tr, zu);
     __syncwarp();
-    if (Q.d_disp) {
+    if (d.disp) {
         const RayOut o = composite_ray(raw, sm.z, S, nrm, nullptr, lane);
-        disparity_bwd(o.depth, o.acc, Q.d_disp[ri], dD, dA);
+        disparity_bwd(o.depth, o.acc, d.disp[ri], dD, dA);
     }
     if (dD_out) *dD_out = dD;
-    const float* dW = Q.d_weights ? Q.d_weights + ri * S : nullptr;
+    const float* dW = d.weights ? d.weights + ri * S : nullptr;
     for (int s = lane; s < S; s += 32) {
         const float4 rw = raw[s];
         const float z = sm.z[s];
@@ -152,8 +148,8 @@ __global__ void __launch_bounds__(CB_WARPS * 32) composite_bwd_kernel(const BwdP
 // composite_bwd_kernel (ray_bwd_recurrences).
 // DEPTH (nb_render_bwd_inputs): also d z_i = r_i . d + dD w_i + |d| (c_{i-1} - c_i), with r_i the record's d loss / d(world
 // point), dD the depth cotangent after the disp fold and c_i = dL/d dists_i = dalpha_i relu(sigma_i) e_i (c_{S-1} = c_{-1} = 0:
-// the last dist is 1e10 |d|, independent of z).  It is added to Q.d_z.z and, with z_sample's coefficients, summed into
-// Q.d_z.near / .far.  A skipped sample has r = 0, w = 0 and relu(sigma) = 0, so skipping stays exact.
+// the last dist is 1e10 |d|, independent of z).  It is added to Q.req.depths.z and, with z_sample's coefficients, summed
+// into .near / .far.  A skipped sample has r = 0, w = 0 and relu(sigma) = 0, so skipping stays exact.
 template <bool DEPTH>
 __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams Q, const float* __restrict__ rec, int rec_stride) {
     __shared__ RaySmem s_ray[CB_WARPS];
@@ -188,13 +184,14 @@ __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams
     if constexpr (DEPTH) {
         __syncwarp();
         const float* tr = P.t_rand ? P.t_rand + ri * S : nullptr;
+        const DepthGrads& dzo = Q.req.depths;
         float dnear = 0.f, dfar = 0.f;
         for (int s = lane; s < S; s += 32) {
             const float* r = rec + (ri * S + s) * rec_stride;
             const float w = sm.alpha[s] * sm.T[s];
             const float dzs = fmaf(r[2], dz, fmaf(r[1], dy, r[0] * dx)) + dD * w + nrm * ((s > 0 ? sm.f[s - 1] : 0.f) - sm.f[s]);
-            if (Q.d_z.z) Q.d_z.z[ri * S + s] += dzs;
-            if (Q.d_z.near || Q.d_z.far) {
+            if (dzo.z) dzo.z[ri * S + s] += dzs;
+            if (dzo.near || dzo.far) {
                 float cn, cf;
                 z_sample_coefs(P.t_vals, s, S, tr, cn, cf);
                 dnear = fmaf(cn, dzs, dnear);
@@ -203,22 +200,22 @@ __global__ void __launch_bounds__(CB_WARPS * 32) ray_grad_kernel(const BwdParams
         }
         dnear = warp_sum(dnear);
         dfar = warp_sum(dfar);
-        if (lane == 0 && Q.d_z.near) Q.d_z.near[ri] += dnear;
-        if (lane == 0 && Q.d_z.far) Q.d_z.far[ri] += dfar;
+        if (lane == 0 && dzo.near) dzo.near[ri] += dnear;
+        if (lane == 0 && dzo.far) dzo.far[ri] += dfar;
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { go[k] = warp_sum(go[k]); gd[k] = warp_sum(gd[k]); du[k] = warp_sum(du[k]); }
     dn = warp_sum(dn);
     if (lane == 0) {
-        if (Q.d_ray_o) {
+        if (Q.req.d_ray_o) {
 #pragma unroll
-            for (int k = 0; k < 3; ++k) Q.d_ray_o[ri * 3 + k] += go[k];
+            for (int k = 0; k < 3; ++k) Q.req.d_ray_o[ri * 3 + k] += go[k];
         }
-        if (Q.d_ray_d) {
+        if (Q.req.d_ray_d) {
             const float u[3] = {__fdiv_rn(dx, nrm), __fdiv_rn(dy, nrm), __fdiv_rn(dz, nrm)};
             const float udu = fmaf(u[2], du[2], fmaf(u[1], du[1], u[0] * du[0]));
 #pragma unroll
-            for (int k = 0; k < 3; ++k) Q.d_ray_d[ri * 3 + k] += gd[k] + fmaf(-u[k], udu, du[k]) / nrm + u[k] * dn;
+            for (int k = 0; k < 3; ++k) Q.req.d_ray_d[ri * 3 + k] += gd[k] + fmaf(-u[k], udu, du[k]) / nrm + u[k] * dn;
         }
     }
 }
@@ -302,52 +299,11 @@ __device__ __forceinline__ void gemm_tile(const float* __restrict__ in, float* _
     __syncthreads();
 }
 
-// Whole warp, ray gradients: adds each lane's d loss / d(world point) g to its ray ri (~0u: none) -- d ray_o += g,
-// d ray_d += z g.  The lanes of one ray are summed first: one atomic per ray and element (a warp holds consecutive points).
-__device__ __forceinline__ void ray_pos_add(unsigned int ri, float z, const float (&g)[3], float* __restrict__ d_ray_o,
-                                            float* __restrict__ d_ray_d, int lane) {
-    for (;;) {
-        const unsigned int rm = __reduce_min_sync(0xffffffffu, ri);
-        if (rm == ~0u) break;
-        const bool mine = ri == rm;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            const float so = warp_sum(mine ? g[k] : 0.f), sd = warp_sum(mine ? z * g[k] : 0.f);
-            if (lane == 0 && d_ray_o) atomicAdd(d_ray_o + (size_t)rm * 3 + k, so);
-            if (lane == 0 && d_ray_d) atomicAdd(d_ray_d + (size_t)rm * 3 + k, sd);
-        }
-        if (mine) ri = ~0u;
-    }
-}
-
-// Whole warp, depth gradients: lane's sample s of ray ri (~0u: none) takes v = its grid part of d loss / d z.  Adds v to d z
-// (one writer per sample) and, for the ray, sum cn v / sum cf v to d near / d far with one atomic per ray and element.
-__device__ __forceinline__ void ray_depth_add(const BwdParams& Q, unsigned int ri, int s, float v, int lane) {
-    const RenderParams& P = Q.f;
-    const int S = P.n_samples;
-    if (ri != ~0u && Q.d_z.z) Q.d_z.z[(size_t)ri * S + s] += v;
-    if (!Q.d_z.near && !Q.d_z.far) return;
-    float cn = 0.f, cf = 0.f;
-    if (ri != ~0u) {
-        z_sample_coefs(P.t_vals, s, S, P.t_rand ? P.t_rand + (size_t)ri * S : nullptr, cn, cf);
-        cn *= v; cf *= v;
-    }
-    for (;;) {
-        const unsigned int rm = __reduce_min_sync(0xffffffffu, ri);
-        if (rm == ~0u) break;
-        const bool mine = ri == rm;
-        const float sn = warp_sum(mine ? cn : 0.f), sf = warp_sum(mine ? cf : 0.f);
-        if (lane == 0 && Q.d_z.near) atomicAdd(Q.d_z.near + rm, sn);
-        if (lane == 0 && Q.d_z.far) atomicAdd(Q.d_z.far + rm, sf);
-        if (mine) ri = ~0u;
-    }
-}
-
-// RAYS: also the grid part of the ray gradients (nb_render_bwd_rays), from the same d loss / d(canonical point) as dR / dTh.
-// INPUTS (with RAYS; nb_render_bwd_inputs): each of the ray, depth and bounds parts only when asked for -- the grid part of
-// d z (ray_depth_add: the records of this path hold d_h1pre until the weight gradients have read them, so it is added
-// straight into the outputs like the ray part) and d bounds[:, 0] = -sum d loss / d(canonical point) per frame.
-template <bool RAYS, bool INPUTS = false>
+// Also the input gradients of the request that depend on the sample position, each only when asked for: dR / dTh, d bounds
+// [:, 0] = -sum d loss / d(canonical point) per frame, and the grid parts of the ray gradients (d ray_o += g, d ray_d += z g
+// with g = d loss / d(world point)) and of d z (g . ray_d; through z_sample's coefficients into d near / d far).  The records
+// of this path hold d_h1pre until the weight gradients have read them, so the ray and depth parts go straight into the
+// outputs: d z has one writer per sample, the rest is summed per ray and frame in warp 0 (ray_sum_add, frame_sum_add).
 __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q) {
     extern __shared__ __align__(16) float smem[];
     float* X = smem;                    // [64][356]
@@ -358,9 +314,10 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
     const size_t npts = (size_t)P.batch * P.n_rays * S;
     const int tid = threadIdx.x;
     const float* wf = P.wf32;
-    const bool frame_grads = RAYS || Q.d_R || Q.d_Th;   // any gradient with respect to the sample position
+    const GradRequest& q = Q.req;
+    const bool frame_grads = q.sample_pos();
     FrameGradAcc acc;                   // warp 0: running per-frame sums of dR / dTh
-    FrameGradAcc acc_bounds;            // warp 0, INPUTS: of d bounds[:, 0]
+    FrameGradAcc acc_bounds;            // warp 0: of d bounds[:, 0]
     for (size_t tile = blockIdx.x; tile * TP < npts; tile += gridDim.x) {
         const size_t p0 = tile * TP;
         auto gp = [&](int p) { return p0 + p; };
@@ -462,37 +419,48 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
                     const float* y = Y + (32 * h + tid) * 16;
                     const int b = __float_as_int(y[15]);
                     float t[12] = {};
-                    float dcan[3] = {0.f, 0.f, 0.f};    // INPUTS: d loss / d(canonical point)
+                    float dcan[3] = {0.f, 0.f, 0.f};    // d loss / d(canonical point)
                     if (b >= 0) {
                         FrameXf fx;
 #pragma unroll
                         for (int j = 0; j < 9; ++j) load_frame_xf(P, b, fx, j);
                         // levels summed in order; grid x / y / z pair with the dhw axes 2 / 1 / 0
-                        const float dcx = ((y[0] + y[3]) + y[6]) + y[9], dcy = ((y[1] + y[4]) + y[7]) + y[10],
-                                    dcz = ((y[2] + y[5]) + y[8]) + y[11];
-                        frame_grad_terms(fx, y[12], y[13], y[14], dcx * grid_to_can_scale(fx, 2), dcy * grid_to_can_scale(fx, 1),
-                                         dcz * grid_to_can_scale(fx, 0), t);
-                        if constexpr (INPUTS) {
-                            dcan[0] = dcx * grid_to_can_scale(fx, 2); dcan[1] = dcy * grid_to_can_scale(fx, 1);
-                            dcan[2] = dcz * grid_to_can_scale(fx, 0);
-                        }
+                        dcan[0] = (((y[0] + y[3]) + y[6]) + y[9]) * grid_to_can_scale(fx, 2);
+                        dcan[1] = (((y[1] + y[4]) + y[7]) + y[10]) * grid_to_can_scale(fx, 1);
+                        dcan[2] = (((y[2] + y[5]) + y[8]) + y[11]) * grid_to_can_scale(fx, 0);
+                        frame_grad_terms(fx, y[12], y[13], y[14], dcan[0], dcan[1], dcan[2], t);
                     }
-                    if (!RAYS || Q.d_R || Q.d_Th) frame_grad_add(acc, b, t, Q.d_R, Q.d_Th, tid);
-                    if constexpr (RAYS) {   // d loss / d(world point) through the grid: R dc = -(the dTh term)
+                    if (q.d_R || q.d_Th) frame_sum_add(acc, b, t, tid, [&](FrameGradAcc& x) { frame_grad_flush(x, q.d_R, q.d_Th, tid); });
+                    if (q.d_bounds) frame_sum_add(acc_bounds, b, dcan, tid, [&](FrameGradAcc& x) { bounds_grad_flush(x, q.d_bounds, tid); });
+                    if (q.records()) {   // d loss / d(world point) through the grid: R dc = -(the dTh term)
                         const size_t g = gp(32 * h + tid);
                         const size_t ri = g / S;
+                        const int s = (int)(g % S);
+                        const unsigned int key = b < 0 ? ~0u : (unsigned int)ri;
                         const float gw[3] = {-t[9], -t[10], -t[11]};
-                        const float z = b < 0 ? 0.f : z_sample(P.near[ri], P.far[ri], P.t_vals, (int)(g % S), S,
-                                                               P.t_rand ? P.t_rand + ri * S : nullptr, P.z_user ? P.z_user + ri * S : nullptr);
-                        if constexpr (!INPUTS) {
-                            ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
-                        } else {
-                            if (Q.d_ray_o || Q.d_ray_d) ray_pos_add(b < 0 ? ~0u : (unsigned int)ri, z, gw, Q.d_ray_o, Q.d_ray_d, tid);
-                            if (Q.d_z.any()) {
-                                const float v = b < 0 ? 0.f : fmaf(gw[2], P.ray_d[ri * 3 + 2], fmaf(gw[1], P.ray_d[ri * 3 + 1], gw[0] * P.ray_d[ri * 3]));
-                                ray_depth_add(Q, b < 0 ? ~0u : (unsigned int)ri, (int)(g % S), v, tid);
+                        if (q.d_ray_o || q.d_ray_d) {
+                            const float z = b < 0 ? 0.f : z_sample(P.near[ri], P.far[ri], P.t_vals, s, S, P.t_rand ? P.t_rand + ri * S : nullptr,
+                                                                   P.z_user ? P.z_user + ri * S : nullptr);
+                            const float v[6] = {gw[0], gw[1], gw[2], z * gw[0], z * gw[1], z * gw[2]};
+                            ray_sum_add(key, v, tid, [&](unsigned int r, int k, float sum) {
+                                float* dst = k < 3 ? q.d_ray_o : q.d_ray_d;
+                                if (dst) atomicAdd(dst + (size_t)r * 3 + k % 3, sum);
+                            });
+                        }
+                        if (q.depths.any()) {   // the grid part of d z_i: one writer per sample, then per ray into d near / d far
+                            const float v = b < 0 ? 0.f : fmaf(gw[2], P.ray_d[ri * 3 + 2], fmaf(gw[1], P.ray_d[ri * 3 + 1], gw[0] * P.ray_d[ri * 3]));
+                            if (b >= 0 && q.depths.z) q.depths.z[g] += v;
+                            if (q.depths.near || q.depths.far) {
+                                float c[2] = {0.f, 0.f};
+                                if (b >= 0) {
+                                    z_sample_coefs(P.t_vals, s, S, P.t_rand ? P.t_rand + ri * S : nullptr, c[0], c[1]);
+                                    c[0] *= v; c[1] *= v;
+                                }
+                                ray_sum_add(key, c, tid, [&](unsigned int r, int k, float sum) {
+                                    float* dst = k ? q.depths.far : q.depths.near;
+                                    if (dst) atomicAdd(dst + r, sum);
+                                });
                             }
-                            if (Q.d_bounds) bounds_grad_add(acc_bounds, b, dcan, Q.d_bounds, tid);
                         }
                     }
                 }
@@ -500,8 +468,8 @@ __global__ void __launch_bounds__(NT, 1) decoder_dgrad_kernel(const BwdParams Q)
         }
         __syncthreads();
     }
-    if (frame_grads && tid < 32) frame_grad_flush(acc, Q.d_R, Q.d_Th, tid);
-    if constexpr (INPUTS) if (Q.d_bounds && tid < 32) bounds_grad_flush(acc_bounds, Q.d_bounds, tid);
+    if (tid < 32) frame_grad_flush(acc, q.d_R, q.d_Th, tid);
+    if (q.d_bounds && tid < 32) bounds_grad_flush(acc_bounds, q.d_bounds, tid);
 }
 
 // ------------------------------------------------------------------------------------------ 3. weight gradients
@@ -679,24 +647,22 @@ __global__ void unfold_stage3(const Unfold U) {     // d view_fc[:, :256], d lat
 
 }  // namespace bwd
 
-void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCotangents& d, float* d_raw_out, int d_raw_stride,
+void launch_composite_bwd(const RenderParams& p, const float* raw, const GradRequest& req, float* d_raw_out, int d_raw_stride,
                           cudaStream_t stream) {
     bwd::BwdParams Q{};
-    Q.f = p; Q.raw = raw; Q.d_rgb = d.rgb; Q.d_depth = d.depth; Q.d_acc = d.acc; Q.d_disp = d.disp; Q.d_weights = d.weights;
+    Q.f = p; Q.raw = raw; Q.req = req;
     Q.d_raw_out = d_raw_out; Q.d_raw_stride = d_raw_stride;
     const size_t nrays = (size_t)p.batch * p.n_rays;
     bwd::composite_bwd_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, stream>>>(Q);
 }
 
-void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
-                     float* d_ray_o, float* d_ray_d, const DepthGrads& dz, cudaStream_t stream) {
+void launch_ray_grad(const RenderParams& p, const float* raw, const GradRequest& req, const float* rec, int rec_stride,
+                     cudaStream_t stream) {
     bwd::BwdParams Q{};
-    Q.f = p; Q.raw = raw; Q.d_rgb = d.rgb; Q.d_depth = d.depth; Q.d_acc = d.acc; Q.d_disp = d.disp; Q.d_weights = d.weights;
-    Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
-    Q.d_z = dz;
+    Q.f = p; Q.raw = raw; Q.req = req;
     const size_t nrays = (size_t)p.batch * p.n_rays;
     const unsigned grid = (unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS);
-    if (dz.any()) bwd::ray_grad_kernel<true><<<grid, bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
+    if (req.depths.any()) bwd::ray_grad_kernel<true><<<grid, bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
     else bwd::ray_grad_kernel<false><<<grid, bwd::CB_WARPS * 32, 0, stream>>>(Q, rec, rec_stride);
 }
 
@@ -767,8 +733,8 @@ extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_
     }
     const nb_render_input_grads none{};
     if (!in) in = &none;
-    float *d_R = in->d_R, *d_Th = in->d_Th, *d_ray_o = in->d_ray_o, *d_ray_d = in->d_ray_d;
-    const DepthGrads d_depths{in->d_near, in->d_far, in->d_z_vals};
+    const GradRequest req{{a->d_rgb_map, a->d_depth_map, a->d_acc_map, d_disp_map, d_weights}, in->d_R, in->d_Th, in->d_ray_o,
+                          in->d_ray_d, {in->d_near, in->d_far, in->d_z_vals}, in->d_bounds};
     const nb_render_args* f = a->fwd;
     if (f->z_vals && (in->d_near || in->d_far)) {
         set_error("nb_render_bwd: d_near / d_far need a forward that derived its depths from near / far (z_vals was given: "
@@ -783,12 +749,10 @@ extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_
     if (f->precision == NB_PRECISION_TC_TF32X3) {
         if (a->workspace_bytes < train_bwd_workspace_bytes(p, f->n_rays, f->n_samples)) { set_error("nb_render_bwd: workspace too small (see nb_render_bwd_workspace_bytes_for)"); return NB_ERR_BAD_ARG; }
         trn::TrainBwd t;
-        t.save = a->save; t.raw = a->raw;
-        t.d_maps = {a->d_rgb_map, a->d_depth_map, a->d_acc_map, d_disp_map, d_weights};
+        t.save = a->save; t.raw = a->raw; t.req = req;
         t.weights = a->weights; t.grads = a->grads; t.workspace = (float*)a->workspace;
         for (int l = 0; l < 4; ++l) t.d_vol[l] = a->d_volumes[l];
-        t.d_R = d_R; t.d_Th = d_Th; t.d_ray_o = d_ray_o; t.d_ray_d = d_ray_d; t.volume_dtype = f->volume_dtype;
-        t.d_depths = d_depths; t.d_bounds = in->d_bounds;
+        t.volume_dtype = f->volume_dtype;
         return launch_train_bwd(p, t, (cudaStream_t)stream);
     }
     if (f->precision != NB_PRECISION_FP32 || f->volume_dtype != NB_DTYPE_F32) {
@@ -801,37 +765,22 @@ extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_
     }
     bwd::BwdParams Q{};
     Q.f = p;
-    Q.save = a->save; Q.raw = a->raw;
-    const MapCotangents d_maps{a->d_rgb_map, a->d_depth_map, a->d_acc_map, d_disp_map, d_weights};
-    Q.d_rgb = d_maps.rgb; Q.d_depth = d_maps.depth; Q.d_acc = d_maps.acc; Q.d_disp = d_maps.disp; Q.d_weights = d_maps.weights;
+    Q.save = a->save; Q.raw = a->raw; Q.req = req;
     Q.ws = (float*)a->workspace;
-    Q.d_raw_out = Q.ws + kGradRaw; Q.d_raw_stride = kGradDim;
     Q.w = *a->weights;
     for (int l = 0; l < 4; ++l) Q.d_vol[l] = a->d_volumes[l];
-    Q.d_R = d_R; Q.d_Th = d_Th;
-    Q.d_ray_o = d_ray_o; Q.d_ray_d = d_ray_d;
-    Q.d_z = d_depths; Q.d_bounds = in->d_bounds;
-    const bool ray_grads = d_ray_o || d_ray_d, depth_grads = d_depths.any(), inputs = depth_grads || in->d_bounds;
     cudaStream_t s = (cudaStream_t)stream;
     const size_t nrays = (size_t)f->batch * f->n_rays, npts = nrays * f->n_samples;
     if (npts == 0) return NB_OK;
     const nb_decoder_weights& g = *a->grads;
 
-    bwd::composite_bwd_kernel<<<(unsigned)((nrays + bwd::CB_WARPS - 1) / bwd::CB_WARPS), bwd::CB_WARPS * 32, 0, s>>>(Q);
+    launch_composite_bwd(p, a->raw, req, Q.ws + kGradRaw, kGradDim, s);
 
     const size_t smem = ((size_t)bwd::TP * bwd::LDX + (size_t)bwd::TP * bwd::LDY + (size_t)bwd::KC * kFeat) * 4;
     const size_t ntiles = (npts + bwd::TP - 1) / bwd::TP;
     const unsigned dgrad_grid = (unsigned)(ntiles < kGridSMs ? ntiles : kGridSMs);
-    if (inputs) {      // + whichever of the grid parts of the ray, depth and bounds gradients was asked for
-        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        bwd::decoder_dgrad_kernel<true, true><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
-    } else if (ray_grads) {   // + the grid part of the ray gradients, added straight into d_ray_o / d_ray_d
-        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        bwd::decoder_dgrad_kernel<true><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
-    } else {
-        cudaFuncSetAttribute(bwd::decoder_dgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        bwd::decoder_dgrad_kernel<false><<<dgrad_grid, bwd::NT, smem, s>>>(Q);
-    }
+    cudaFuncSetAttribute(bwd::decoder_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    bwd::decoder_dgrad_kernel<<<dgrad_grid, bwd::NT, smem, s>>>(Q);
 
     // scratch after the per-point region
     float* extra = Q.ws + npts * kGradDim;
@@ -868,12 +817,12 @@ extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_
 
     st = launch_unfold(*a->weights, g, dWcx, dbc, T, dT, u, du, s);
     if (st != NB_OK) return st;
-    if (ray_grads || depth_grads) {   // the encodings' part per point into the d_h1pre columns (read by the weight / bias gradients above), then per ray
+    if (req.records()) {   // the encodings' part per point into the d_h1pre columns (read by the weight / bias gradients above), then per ray
         float* rec = Q.ws + kGradH1;
         bwd::pe_grad_kernel<<<(unsigned)((npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS < (size_t)kGridSMs * 16
                                              ? (npts + bwd::PG_WARPS - 1) / bwd::PG_WARPS : (size_t)kGridSMs * 16),
                               bwd::PG_WARPS * 32, 0, s>>>(Q, rec, kGradDim);
-        launch_ray_grad(p, a->raw, d_maps, rec, kGradDim, d_ray_o, d_ray_d, d_depths, s);
+        launch_ray_grad(p, a->raw, req, rec, kGradDim, s);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("nb_render_bwd: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

@@ -14,11 +14,11 @@
 //             head_kernel        rgb_fc, raw records; then composite_kernel (shared with the inference path)
 //   backward  composite_bwd_kernel (nb_render_bwd.cu) -> bwd_head_kernel -> 4 x gemm (dgrad, relu masks in the epilogue)
 //             -> scatter_kernel (trilinear backward, 16-byte vector atomics into a channels-last gradient blob, then one
-//             transposing add into the NCDHW gradients autograd expects) ; frame_grad_kernel (only when the frame
-//             transform's gradients are asked for) ; 4 x gemm (wgrad, split over the list, fp32 atomics)
-//             ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu) ; only when the rays'
-//             gradients are asked for: gemm (the encodings' input gradient), frame_grad_kernel<VT, true> (per-sample
-//             records, and dR / dTh in place of the earlier frame pass), ray_grad_kernel (nb_render_bwd.cu).
+//             transposing add into the NCDHW gradients autograd expects) ; 4 x gemm (wgrad, split over the list, fp32
+//             atomics) ; column sums for the biases ; the un-fold of the colour layer (nb_render_bwd.cu) ; only when a
+//             gradient with respect to the sample position is asked for: frame_grad_kernel (dR / dTh, d bounds) and, for
+//             the ray and depth gradients, gemm (the encodings' input gradient) before it (per-sample records) and
+//             ray_grad_kernel (nb_render_bwd.cu) after it.
 //
 // gemm_tf32x3_kernel: C[128 x <=256 tile] = epilogue(A B^T), fp32 in HBM on both sides.  Operands are split on the way into
 // shared memory into hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi, and three wgmma tf32 passes
@@ -452,26 +452,28 @@ __global__ void __launch_bounds__(256) scatter_kernel(const __grid_constant__ Re
 // scatter_kernel; each (entry, quad) adds sum_c dF_c d f_c / d i, scaled to d / d(canonical point), into its entry's shared
 // slot; warp 0 then turns the 32 entries into dR / dTh terms and sums them per frame (one atomic per CTA, frame and element:
 // the list is frame-major and each CTA walks it in order).  Reads the packed blob the forward gathered from.
-// RAYS (nb_render_bwd_rays): also each entry's ray-gradient record rec + id * kRayRec = [d loss / d(world point) 3 |
-// d loss / d(view direction) 3]: the grid part R dc plus the two encodings' parts, from dPE (count x kPECols, the colour
-// layer's input gradient in columns kXyzCol..) and the sin / cos the forward saved in H2X.  dR / dTh may both be null then.
+// WIDE (ray, depth or bounds gradients asked for; dR / dTh may both be null then), each part only when its pointer is given:
+//   rec: each entry's ray-gradient record rec + id * kRayRec = [d loss / d(world point) 3 | d loss / d(view direction) 3]:
+//        the grid part R dc plus the two encodings' parts, from dPE (count x kPECols, the colour layer's input gradient in
+//        columns kXyzCol..) and the sin / cos the forward saved in H2X;
+//   d_bounds: d_bounds[b, 0, :] -= the per-frame sum of d loss / d(canonical point), the quantity whose image under R is the
+//        dTh term, taken before R is applied.
+// The frame-only variant takes 63 registers and runs 4 CTAs per SM; WIDE asks for at least 2, so that ptxas does not squeeze
+// it into 64 registers and spill.
 constexpr int kPECols = kH2X - kXyzCol;     // [PE(xyz) 63 | 0 | PE(view) 27 | 0 x 5]
 constexpr int kRayRec = 8;
-// BOUNDS (nb_render_bwd_inputs): also d_bounds[b, 0, :] -= the per-frame sum of d loss / d(canonical point), the quantity
-// whose image under R is the dTh term, taken before R is applied.  dR / dTh may both be null then.
-// (RAYS: at least 2 CTAs per SM, so ptxas does not squeeze it into 64 registers and spill; 0 = no minimum, as before)
-template <typename VT, bool RAYS, bool BOUNDS = false>
-__global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
+template <typename VT, bool WIDE>
+__global__ void __launch_bounds__(256, WIDE ? 2 : 0) frame_grad_kernel(const __grid_constant__ RenderParams P, SaveMap sv, const float* __restrict__ DF,
                                                          float* __restrict__ dR, float* __restrict__ dTh, const float* __restrict__ dPE,
-                                                         float* __restrict__ rec, float* __restrict__ d_bounds = nullptr) {
+                                                         float* __restrict__ rec, float* __restrict__ d_bounds) {
     __shared__ float gc[GP][3], dc[GP][3];
     __shared__ int fr[GP];
-    __shared__ float pe[RAYS ? 2 : 1][GP][3];   // RAYS: [PE(xyz) | PE(view)][entry][axis]
+    __shared__ float pe[WIDE ? 2 : 1][GP][3];   // WIDE: [PE(xyz) | PE(view)][entry][axis]
     const unsigned int count = *sv.count;
     const unsigned int spf = (unsigned int)P.n_rays * P.n_samples;
     const int tid = threadIdx.x;
     FrameGradAcc acc;
-    FrameGradAcc acc_bounds;                    // BOUNDS: warp 0's running per-frame sums of d bounds[:, 0]
+    FrameGradAcc acc_bounds;                    // WIDE: warp 0's running per-frame sums of d bounds[:, 0]
     for (unsigned int e0 = blockIdx.x * GP; e0 < count; e0 += gridDim.x * GP) {
         if (tid < GP) {
             fr[tid] = -1;
@@ -503,22 +505,20 @@ __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __g
             atomicAdd(&dc[p][1], d.y * (0.5f * (float)(P.lvl_H[lvl] - 1)));
             atomicAdd(&dc[p][2], d.z * (0.5f * (float)(P.lvl_D[lvl] - 1)));
         }
-        if constexpr (RAYS) {   // (encoding, entry, axis) items
-            if (tid < 2 * GP * 3) {
-                const int v = tid / (GP * 3), p = tid % (GP * 3) / 3, ax = tid % 3;
-                float r = 0.f;
-                if (e0 + p < count) {
-                    const float* d = dPE + (size_t)(e0 + p) * kPECols + (v ? kViewCol - kXyzCol : 0);
-                    const float* enc = sv.H2X + (size_t)(e0 + p) * kH2X + (v ? kViewCol : kXyzCol);
-                    r = v ? positional_embed_bwd<4>(d, enc, ax) : positional_embed_bwd<10>(d, enc, ax);
-                }
-                pe[v][p][ax] = r;
+        if (WIDE && rec && tid < 2 * GP * 3) {   // (encoding, entry, axis) items
+            const int v = tid / (GP * 3), p = tid % (GP * 3) / 3, ax = tid % 3;
+            float r = 0.f;
+            if (e0 + p < count) {
+                const float* d = dPE + (size_t)(e0 + p) * kPECols + (v ? kViewCol - kXyzCol : 0);
+                const float* enc = sv.H2X + (size_t)(e0 + p) * kH2X + (v ? kViewCol : kXyzCol);
+                r = v ? positional_embed_bwd<4>(d, enc, ax) : positional_embed_bwd<10>(d, enc, ax);
             }
+            pe[v][p][ax] = r;
         }
         __syncthreads();
         if (tid < 32) {
             float t[12] = {};
-            float dcan[3] = {0.f, 0.f, 0.f};    // BOUNDS: d loss / d(canonical point)
+            float dcan[3] = {0.f, 0.f, 0.f};    // WIDE: d loss / d(canonical point)
             const int b = fr[tid];
             if (b >= 0) {
                 const float4 en = sv.list[e0 + tid];
@@ -528,23 +528,23 @@ __global__ void __launch_bounds__(256, RAYS ? 2 : 0) frame_grad_kernel(const __g
                 // grid x / y / z pair with the dhw axes 2 / 1 / 0
                 frame_grad_terms(fx, en.x, en.y, en.z, dc[tid][0] * grid_to_can_scale(fx, 2), dc[tid][1] * grid_to_can_scale(fx, 1),
                                  dc[tid][2] * grid_to_can_scale(fx, 0), t);
-                if constexpr (BOUNDS) {
+                if constexpr (WIDE) {
                     dcan[0] = dc[tid][0] * grid_to_can_scale(fx, 2); dcan[1] = dc[tid][1] * grid_to_can_scale(fx, 1);
                     dcan[2] = dc[tid][2] * grid_to_can_scale(fx, 0);
                 }
-                if constexpr (RAYS) {   // the grid part R dc is -(the dTh term)
+                if (WIDE && rec) {   // the grid part R dc is -(the dTh term)
                     float* r = rec + (size_t)(__float_as_uint(en.w) & kListIdMask) * kRayRec;
 #pragma unroll
                     for (int k = 0; k < 3; ++k) { r[k] = pe[0][tid][k] - t[9 + k]; r[3 + k] = pe[1][tid][k]; }
                 }
             }
-            if (!(RAYS || BOUNDS) || dR || dTh) frame_grad_add(acc, b, t, dR, dTh, tid);
-            if constexpr (BOUNDS) bounds_grad_add(acc_bounds, b, dcan, d_bounds, tid);
+            if (!WIDE || dR || dTh) frame_sum_add(acc, b, t, tid, [&](FrameGradAcc& x) { frame_grad_flush(x, dR, dTh, tid); });
+            if (WIDE && d_bounds) frame_sum_add(acc_bounds, b, dcan, tid, [&](FrameGradAcc& x) { bounds_grad_flush(x, d_bounds, tid); });
         }
         __syncthreads();
     }
     if (tid < 32) frame_grad_flush(acc, dR, dTh, tid);
-    if constexpr (BOUNDS) if (tid < 32) bounds_grad_flush(acc_bounds, d_bounds, tid);
+    if (WIDE && d_bounds && tid < 32) bounds_grad_flush(acc_bounds, d_bounds, tid);
 }
 
 // d_vol[b][c][v] += blob[b][v][c] for one level: 32 voxels x 32 channels through shared memory
@@ -718,7 +718,8 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     cudaMemsetAsync(dwcol, 0, ((size_t)kWS * kH2X + ((size_t)p.batch * kWS + 63) / 64 * 64) * 4, stream);
 
     // 1. d(outputs) -> d(raw) per sample (dense), 2. the colour layer's output gradient over the list
-    launch_composite_bwd(p, t.raw, t.d_maps, reinterpret_cast<float*>(d_raw), 4, stream);
+    const GradRequest& q = t.req;
+    launch_composite_bwd(p, t.raw, q, reinterpret_cast<float*>(d_raw), 4, stream);
     bwd_head_kernel<<<kGridSMs * 2, 256, 0, stream>>>(p.wf32, sv, d_raw, G3, G_(g.rgb_w), G_(g.rgb_b));
     // 3. dgrad chain (relu masks = the saved activations)
     GemmArgs a{};
@@ -730,10 +731,7 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     a.a = G1; a.b = w.fc1_w; a.c = G0; a.mask = sv.H0;
     if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
-    const bool frame_grads = t.d_R || t.d_Th || t.d_bounds;
-    // any depth gradient needs the per-sample records of the ray gradients (d z_i takes d loss / d(world point) along ray_d)
-    const bool ray_grads = t.d_ray_o || t.d_ray_d || t.d_depths.any();
-    if (t.d_vol[0] || frame_grads || ray_grads) {
+    if (t.d_vol[0] || q.sample_pos()) {
         a.a = G0; a.b = w.fc0_w; a.ldb = kFeat; a.N = kFeat; a.c = DF; a.ldc = kFeat; a.mask = nullptr;
         if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
     }
@@ -746,17 +744,6 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
             const size_t nvox = (size_t)p.lvl_D[l] * p.lvl_H[l] * p.lvl_W[l];
             dim3 grid((unsigned)((nvox + 31) / 32), (p.lvl_C[l] + 31) / 32, p.batch);
             unpack_grad_kernel<<<grid, 256, 0, stream>>>(dblob + gb.off[l], t.d_vol[l], p.lvl_C[l], nvox, p.batch);
-        }
-    }
-    if (frame_grads && !ray_grads) {   // 4b. the frame transform's gradients, from the same DF (with ray gradients: step 8)
-        const bool f32 = t.volume_dtype == NB_DTYPE_F32;
-        if (t.d_bounds) {
-            if (f32) frame_grad_kernel<float, false, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr, t.d_bounds);
-            else frame_grad_kernel<__half, false, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr, t.d_bounds);
-        } else if (f32) {
-            frame_grad_kernel<float, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
-        } else {
-            frame_grad_kernel<__half, false><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, nullptr, nullptr);
         }
     }
     // 5. weight gradients: dW[out][in] += G^T X, split over the list
@@ -783,24 +770,23 @@ int launch_train_bwd(const RenderParams& p, const TrainBwd& t, cudaStream_t stre
     finish_color_kernel<<<(nfin + 255) / 256, 256, 0, stream>>>(dwcol, dbias3, p.batch, dWcx, dbc, G_(g.view_w), G_(g.alpha_w), G_(g.alpha_b));
     st = launch_unfold(w, g, dWcx, dbc, T, dT, u, du, stream);
     if (st != NB_OK) return st;
-    if (ray_grads) {
-        // 8. ray gradients (+ dR / dTh when asked for), in G2 / G1, which steps 5 and 6 were the last to read: the encodings'
-        // input gradient dPE = G3 Wcol[:, 256:352]^T, then the per-entry records by sample id (skipped samples: 0), then per ray
-        float* dPE = G2;
-        float* rec = G1;
-        a.a = G3; a.lda = kWS; a.b = sv.wcol + kXyzCol; a.ldb = kH2X; a.N = kPECols; a.K = kWS; a.c = dPE; a.ldc = kPECols; a.mask = nullptr;
-        if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
-        cudaMemsetAsync(rec, 0, pmax * kRayRec * 4, stream);
-        const bool f32 = t.volume_dtype == NB_DTYPE_F32;
-        if (t.d_bounds) {
-            if (f32) frame_grad_kernel<float, true, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec, t.d_bounds);
-            else frame_grad_kernel<__half, true, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec, t.d_bounds);
-        } else if (f32) {
-            frame_grad_kernel<float, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
-        } else {
-            frame_grad_kernel<__half, true><<<grid_pts, 256, 0, stream>>>(p, sv, DF, t.d_R, t.d_Th, dPE, rec);
+    if (q.sample_pos()) {
+        // 8. the frame pass over DF, which steps 5-7 do not touch.  Ray and depth gradients first need the per-entry records
+        // (skipped samples: 0) in G2 / G1, which steps 5 and 6 were the last to read: the encodings' input gradient
+        // dPE = G3 Wcol[:, 256:352]^T, then the records by sample id, then per ray
+        float* dPE = nullptr;
+        float* rec = nullptr;
+        if (q.records()) {
+            dPE = G2; rec = G1;
+            a.a = G3; a.lda = kWS; a.b = sv.wcol + kXyzCol; a.ldb = kH2X; a.N = kPECols; a.K = kWS; a.c = dPE; a.ldc = kPECols; a.mask = nullptr;
+            if ((st = launch_gemm(a, true, false, (int)pmax, 1, stream)) != NB_OK) return st;
+            cudaMemsetAsync(rec, 0, pmax * kRayRec * 4, stream);
         }
-        launch_ray_grad(p, t.raw, t.d_maps, rec, kRayRec, t.d_ray_o, t.d_ray_d, t.d_depths, stream);
+        const bool f32 = t.volume_dtype == NB_DTYPE_F32, wide = q.records() || q.d_bounds;
+        auto* frame_pass = wide ? (f32 ? frame_grad_kernel<float, true> : frame_grad_kernel<__half, true>)
+                                : (f32 ? frame_grad_kernel<float, false> : frame_grad_kernel<__half, false>);
+        frame_pass<<<grid_pts, 256, 0, stream>>>(p, sv, DF, q.d_R, q.d_Th, dPE, rec, q.d_bounds);
+        if (q.records()) launch_ray_grad(p, t.raw, q, rec, kRayRec, stream);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("train bwd launch failed: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }

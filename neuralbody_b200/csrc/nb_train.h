@@ -15,6 +15,22 @@ struct DepthGrads {
     __host__ __device__ bool any() const { return near || far || z; }
 };
 
+// what one backward call was asked for: the map cotangents it was given and the input gradients it accumulates into
+// (device; any pointer may be null)
+struct GradRequest {
+    MapCotangents maps;
+    float *d_R, *d_Th;               // (B,3,3) / (B,3) frame transform
+    float *d_ray_o, *d_ray_d;        // (B,n,3) rays
+    DepthGrads depths;
+    float* d_bounds;                 // (B,2,3): row 0
+    // any per-frame gradient (the frame pass sums them per frame)
+    __host__ __device__ bool frame() const { return d_R || d_Th || d_bounds; }
+    // per-sample ray records: d z_i takes d loss / d(world point) along ray_d, so the depths need them too
+    __host__ __device__ bool records() const { return d_ray_o || d_ray_d || depths.any(); }
+    // any gradient with respect to the sample position
+    __host__ __device__ bool sample_pos() const { return frame() || records(); }
+};
+
 namespace trn {
 
 constexpr int kH2X = 352;                   // colour-layer input record: [h2 256 | PE(xyz) 63 | 0 | PE(viewdir) 27 | 0 x 5]
@@ -53,13 +69,9 @@ struct GradBlob { size_t off[4], bstride[4], floats; };   // channels-last volum
 
 struct TrainBwd {
     const float* save; const float* raw;
-    MapCotangents d_maps;
+    GradRequest req;
     const nb_decoder_weights* weights; const nb_decoder_weights* grads;
     float* d_vol[4];
-    float *d_R, *d_Th;               // (B,3,3) / (B,3) frame-transform gradients, accumulated into; either may be null
-    float *d_ray_o, *d_ray_d;        // (B,n,3) ray gradients, accumulated into; either may be null
-    DepthGrads d_depths;             // near / far / sample-depth gradients, accumulated into; any may be null
-    float* d_bounds;                 // (B,2,3): row 0 accumulated into; may be null
     int volume_dtype;               // of the forward's volume blob (the frame-gradient pass reads it)
     float* workspace;
 };
@@ -75,14 +87,13 @@ int launch_train_bwd(const RenderParams& p, const trn::TrainBwd& t, cudaStream_t
 // shared pieces living in other translation units
 void launch_classify(const RenderParams& p, cudaStream_t stream);    // nb_render_tc_list.cu (p.frame, lists, raw_ws set by the caller)
 void launch_composite(const RenderParams& p, cudaStream_t stream);   // nb_render_tc_list.cu
-void launch_composite_bwd(const RenderParams& p, const float* raw, const MapCotangents& d, float* d_raw_out, int d_raw_stride,
+void launch_composite_bwd(const RenderParams& p, const float* raw, const GradRequest& req, float* d_raw_out, int d_raw_stride,
                           cudaStream_t stream);                                        // nb_render_bwd.cu
 // per ray: the per-sample records rec + i * rec_stride = [d / d(world point) 3 | d / d(view direction) 3] plus the compositing
-// term -> d_ray_o / d_ray_d (accumulated into; either may be null); with any depth gradient asked for, also d z per sample
-// (the records' world-point part along ray_d, the depth map and the dists) -> dz.z and, through z_sample, dz.near / dz.far
-//                                                                                                                  nb_render_bwd.cu
-void launch_ray_grad(const RenderParams& p, const float* raw, const MapCotangents& d, const float* rec, int rec_stride,
-                     float* d_ray_o, float* d_ray_d, const DepthGrads& dz, cudaStream_t stream);
+// term -> req.d_ray_o / d_ray_d; with any depth gradient asked for, also d z per sample (the records' world-point part along
+// ray_d, the depth map and the dists) -> req.depths.z and, through z_sample, .near / .far                      nb_render_bwd.cu
+void launch_ray_grad(const RenderParams& p, const float* raw, const GradRequest& req, const float* rec, int rec_stride,
+                     cudaStream_t stream);
 int launch_unfold(const nb_decoder_weights& w, const nb_decoder_weights& g, const float* dWcx, const float* dbc, float* T, float* dT,
                   float* u, float* du, cudaStream_t stream);                          // nb_render_bwd.cu
 

@@ -23,6 +23,13 @@ _PRECISIONS = {"fp32": capi.NB_PRECISION_FP32, "tc_fp16": capi.NB_PRECISION_TC_F
 _DECODER_FIELDS = tuple(f[0] for f in capi.nb_decoder_weights._fields_[:17])
 
 
+def _input_grad_slots(B, n, S):
+    """The eight input-gradient slots after the volumes and the decoder tensors, in _FusedRender.apply order (R, Th, ray_o,
+    ray_d, near, far, bounds, z_vals): the nb_render_input_grads field each is accumulated through, and its fp32 shape."""
+    return (("d_R", (B, 3, 3)), ("d_Th", (B, 3)), ("d_ray_o", (B, n, 3)), ("d_ray_d", (B, n, 3)),
+            ("d_near", (B, n)), ("d_far", (B, n)), ("d_bounds", (B, 2, 3)), ("d_z_vals", (B, n, S)))
+
+
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
@@ -33,7 +40,7 @@ def _f32c(t, device):
 
 class _FusedRender(torch.autograd.Function):
     """Autograd boundary of the training path (BASELINE config 3): forward = nb_render_fwd with the exact
-    kernel + activation record, backward = nb_render_bwd_maps.  Differentiable outputs: all five maps, rgb_map,
+    kernel + activation record, backward = nb_render_bwd_inputs.  Differentiable outputs: all five maps, rgb_map,
     disp_map, acc_map, depth_map and weights, as upstream's raw2outputs (nerf_net_utils.py:37-45); an output the loss
     does not read costs nothing (its cotangent stays None and the kernels get NULL).  disp_map follows upstream's NaN
     rule: on a ray with acc_map == 0 its gradient is NaN, which reaches ray_d only (see nb_render_bwd_maps).
@@ -236,15 +243,13 @@ class Renderer:
         B, n = int(ray_o.shape[0]), int(ray_o.shape[1])
         S = int(cfg.N_samples) if z_vals is None else int(z_vals.shape[-1])   # z_vals: caller-supplied depths (fine pass, f-4)
         params = self.net.decoder_tensors()
-        frame = [sp_input['R'], sp_input['Th']]
-        # near, far, bounds, z_vals: the depth inputs (near / far are not read when the caller gives the depths)
-        depths = [near if z_vals is None else None, far if z_vals is None else None, sp_input['bounds'], z_vals]
-        depths = [t if torch.is_tensor(t) else None for t in depths]
+        # the inputs of _input_grad_slots (near / far are not read when the caller gives the depths)
+        inputs = [sp_input['R'], sp_input['Th'], ray_o, ray_d, near if z_vals is None else None,
+                  far if z_vals is None else None, sp_input['bounds'], z_vals]
+        inputs = [t if torch.is_tensor(t) else None for t in inputs]
         needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
                                                   any(v.requires_grad for v in feature_volume) or
-                                                  any(torch.is_tensor(t) and t.requires_grad for t in frame) or
-                                                  ray_o.requires_grad or ray_d.requires_grad or
-                                                  any(t is not None and t.requires_grad for t in depths))
+                                                  any(t is not None and t.requires_grad for t in inputs))
         precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
@@ -259,8 +264,7 @@ class Renderer:
             "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": self._volume_dtype(precision),
             "ray_o": _f32c(ray_o.detach(), dev), "ray_d": _f32c(ray_d.detach(), dev),
             "near": _f32c(near.detach(), dev), "far": _f32c(far.detach(), dev),
-            "ray_like": [(t.shape, t.dtype, t.device) for t in (ray_o, ray_d)],
-            "depth_like": [None if t is None else (t.shape, t.dtype, t.device) for t in depths],
+            "input_like": [None if t is None else (t.shape, t.dtype, t.device) for t in inputs],
             "sp_input": sp_input, "t_rand": None if t_rand is None else _f32c(t_rand, dev), "white_bkgd": bool(cfg.white_bkgd),
             "z_vals": None if z_vals is None else _f32c(z_vals.detach(), dev),
             "feature_volume": list(feature_volume), "want_raw": want_raw or needs_grad, "user_raw": bool(want_raw), "out": out, "trace": trace,
@@ -280,8 +284,7 @@ class Renderer:
         if call["t_rand"] is not None:
             assert tuple(call["t_rand"].shape) == (B, n, S)
         if needs_grad:
-            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *frame, ray_o, ray_d,
-                                                                *depths)
+            rgb, disp, acc, depth, weights = _FusedRender.apply(self, call, *feature_volume, *params, *inputs)
             ret = {'rgb_map': rgb, 'disp_map': disp, 'acc_map': acc, 'weights': weights, 'depth_map': depth}
             if want_raw:
                 ret['raw'] = call["raw"]
@@ -416,9 +419,9 @@ class Renderer:
         return out
 
     def _launch_bwd(self, call, d_rgb, d_depth, d_acc, needs, d_disp=None, d_weights=None):
-        """nb_render_bwd_maps, or nb_render_bwd_inputs when a depth input needs a gradient: gradients for (volumes...,
-        decoder tensors..., R, Th, ray_o, ray_d, near, far, bounds, z_vals) in the order of _FusedRender.apply, from the
-        cotangents of the five maps (None: the loss does not read that map)."""
+        """nb_render_bwd_inputs: gradients for (volumes..., decoder tensors..., R, Th, ray_o, ray_d, near, far, bounds,
+        z_vals) in the order of _FusedRender.apply, from the cotangents of the five maps (None: the loss does not read that
+        map)."""
         dev, B, n, S = call["dev"], call["B"], call["n"], call["S"]
         if call.get("save") is None:
             raise RuntimeError("the activation record of this render call was already consumed by a backward pass "
@@ -451,44 +454,27 @@ class Renderer:
             for l in range(capi.NB_NUM_LEVELS):
                 ba.d_volumes[l] = gvols[l].data_ptr() if want_vol else None
             ba.workspace, ba.workspace_bytes = ws.data_ptr(), nbytes
+            # fp32 accumulators, only for the inputs autograd asks about (pose and camera refinement, depths, box)
             k0 = len(vols) + len(params)
-            # frame transform (pose refinement): fp32 (B,3,3) / (B,3) accumulators, only for the inputs autograd asks about
-            want_R, want_Th = needs[k0], needs[k0 + 1]
-            dR = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev) if want_R else None
-            dTh = torch.zeros((B, 3), dtype=torch.float32, device=dev) if want_Th else None
-            # rays (camera refinement): fp32 (B,n,3) accumulators, likewise
-            drays = [torch.zeros((B, n, 3), dtype=torch.float32, device=dev) if want else None for want in needs[k0 + 2:k0 + 4]]
-            # near, far (B,n), bounds (B,2,3), z_vals (B,n,S)
-            shapes = ((B, n), (B, n), (B, 2, 3), (B, n, S))
-            ddepths = [torch.zeros(sh, dtype=torch.float32, device=dev) if want else None
-                       for sh, want in zip(shapes, needs[k0 + 4:k0 + 8])]
+            ig = capi.nb_render_input_grads()
+            dins = []
+            for (name, shape), want in zip(_input_grad_slots(B, n, S), needs[k0:]):
+                d = torch.zeros(shape, dtype=torch.float32, device=dev) if want else None
+                setattr(ig, name, d.data_ptr() if d is not None else None)
+                dins.append(d)
             stream = torch.cuda.current_stream(dev).cuda_stream
-            if any(d is not None for d in ddepths):
-                ig = capi.nb_render_input_grads()
-                for name, t in zip(("d_R", "d_Th", "d_ray_o", "d_ray_d", "d_near", "d_far", "d_bounds", "d_z_vals"),
-                                   [dR, dTh] + drays + ddepths):
-                    setattr(ig, name, t.data_ptr() if t is not None else None)
-                capi.check(self.lib.nb_render_bwd_inputs(C.byref(ba), _ptr(d_disp), _ptr(d_weights), C.byref(ig),
-                                                         C.c_void_p(stream)), "nb_render_bwd_inputs")
-            else:
-                capi.check(self.lib.nb_render_bwd_maps(C.byref(ba), _ptr(d_disp), _ptr(d_weights), _ptr(dR), _ptr(dTh),
-                                                       _ptr(drays[0]), _ptr(drays[1]), C.c_void_p(stream)), "nb_render_bwd_maps")
+            capi.check(self.lib.nb_render_bwd_inputs(C.byref(ba), _ptr(d_disp), _ptr(d_weights), C.byref(ig),
+                                                     C.c_void_p(stream)), "nb_render_bwd_inputs")
             # stream-ordered reuse: the next forward / backward on this stream runs after the kernels just enqueued
             self._pool_give("bwd_ws", ws)
             self._pool_give("save", call.pop("save"))
             if not call.get("user_raw"):
                 r = call.pop("raw")
                 self._pool_give("raw", r._base if r._base is not None else r)
-        R, Th = call["sp_input"]['R'], call["sp_input"]['Th']
-        if dR is not None:     # the caller's shape, dtype and device ((B,1,3) or (B,3) for Th)
-            dR = dR.to(device=R.device, dtype=R.dtype).view(R.shape)
-        if dTh is not None:
-            dTh = dTh.to(device=Th.device, dtype=Th.dtype).view(Th.shape)
-        drays = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])   # the caller's shape, dtype and device
-                 for d, like in zip(drays, call["ray_like"])]
-        ddepths = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])
-                   for d, like in zip(ddepths, call["depth_like"])]
-        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + [dR, dTh] + drays + ddepths
+        # the caller's shape, dtype and device (Th: (B,1,3) or (B,3))
+        dins = [None if d is None else d.to(device=like[2], dtype=like[1]).view(like[0])
+                for d, like in zip(dins, call["input_like"])]
+        grads = list(gvols) + [gp.view_as(t) for gp, t in zip(gparams, params)] + dins
         return [gr if need else None for gr, need in zip(grads, needs)]
 
     def _weights_struct(self, tensors, latent_index, device):

@@ -396,9 +396,9 @@ def test_depth_kernels_only_when_asked(case, train_precision):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("train_precision", ["tc_tf32x3", "fp32"])
-def test_no_depth_inputs_same_as_maps_entry(case, train_precision):
-    """Without near / far / bounds requiring grad the binding calls nb_render_bwd_maps; on the same forward record,
-    nb_render_bwd_inputs with the four depth pointers NULL gives the same ray gradients (bit for bit on fp32)."""
+def test_no_depth_inputs_null_and_same_as_maps_entry(case, train_precision):
+    """Without near / far / bounds requiring grad the binding calls nb_render_bwd_inputs with the four depth pointers NULL;
+    on the same forward record, that gives the ray gradients of nb_render_bwd_maps (bit for bit on fp32)."""
     from neuralbody_b200 import capi
     scene, t_rand, G, _ = case
     net, ren, vols, batch = _setup(scene, train_precision, rays=True, near_far=False, bounds=False)
@@ -409,24 +409,26 @@ def test_no_depth_inputs_same_as_maps_entry(case, train_precision):
         def __getattr__(self, name):
             return getattr(lib, name)
 
-        def nb_render_bwd_inputs(self, *a):
-            seen["inputs"] = True
-            return lib.nb_render_bwd_inputs(*a)
+        def nb_render_bwd_maps(self, *a):
+            seen["maps"] = True
+            return lib.nb_render_bwd_maps(*a)
 
-        def nb_render_bwd_maps(self, ba_ref, d_disp, d_weights, dR, dTh, do, dd, stream):
+        def nb_render_bwd_inputs(self, ba_ref, d_disp, d_weights, ig_ref, stream):
+            ig = ig_ref._obj
+            seen["depth_ptrs"] = [ig.d_near, ig.d_far, ig.d_bounds, ig.d_z_vals]
             B, n = batch["ray_o"].shape[:2]
             twin = {k: torch.zeros((B, n, 3), dtype=torch.float32, device="cuda") for k in ("ray_o", "ray_d")}
             ba = capi.nb_render_bwd_args.from_buffer_copy(ba_ref._obj)
-            ig = capi.nb_render_input_grads()
-            ig.d_ray_o, ig.d_ray_d = twin["ray_o"].data_ptr(), twin["ray_d"].data_ptr()
-            assert lib.nb_render_bwd_inputs(ctypes.byref(ba), d_disp, d_weights, ctypes.byref(ig), stream) == 0
+            assert lib.nb_render_bwd_maps(ctypes.byref(ba), d_disp, d_weights, None, None, twin["ray_o"].data_ptr(),
+                                          twin["ray_d"].data_ptr(), stream) == 0
             seen["twin"] = twin
-            return lib.nb_render_bwd_maps(ba_ref, d_disp, d_weights, dR, dTh, do, dd, stream)
+            return lib.nb_render_bwd_inputs(ba_ref, d_disp, d_weights, ig_ref, stream)
     ren.lib = Spy()
     out = _render(ren, vols, batch, t_rand)
     _loss(G, "cuda")(out).backward()
     torch.cuda.synchronize()
-    assert "inputs" not in seen and "twin" in seen
+    assert "maps" not in seen and "twin" in seen
+    assert seen["depth_ptrs"] == [None] * 4, seen["depth_ptrs"]
     for k in ("ray_o", "ray_d"):
         if train_precision == "fp32":
             assert torch.equal(batch[k].grad, seen["twin"][k]), k

@@ -137,7 +137,7 @@ def _check(report):
 
 
 class _Spy:
-    """Stands in for Renderer.lib and records what each nb_render_bwd_maps call was given."""
+    """Stands in for Renderer.lib and records what each nb_render_bwd_inputs call was given."""
 
     def __init__(self, lib, twin=None):
         self._lib, self._twin, self.calls = lib, twin, []
@@ -145,13 +145,13 @@ class _Spy:
     def __getattr__(self, name):
         return getattr(self._lib, name)
 
-    def nb_render_bwd_maps(self, ba_ref, d_disp, d_weights, *rest):
+    def nb_render_bwd_inputs(self, ba_ref, d_disp, d_weights, ig_ref, stream):
         ba = ba_ref._obj
         self.calls.append({"d_rgb": ba.d_rgb_map, "d_depth": ba.d_depth_map, "d_acc": ba.d_acc_map,
                            "d_disp": d_disp.value, "d_weights": d_weights.value})
         if self._twin is not None:
-            self._twin(ba, rest)
-        return self._lib.nb_render_bwd_maps(ba_ref, d_disp, d_weights, *rest)
+            self._twin(ba, ig_ref._obj, stream)
+        return self._lib.nb_render_bwd_inputs(ba_ref, d_disp, d_weights, ig_ref, stream)
 
 
 @pytest.mark.gpu
@@ -179,7 +179,7 @@ def test_map_grads_match_oracle(case, train_precision):
 @pytest.mark.gpu
 @pytest.mark.parametrize("train_precision", ["tc_tf32x3", "fp32"])
 @pytest.mark.parametrize("kind", ["weights", "disp"])
-def test_single_map_loss(case, train_precision, kind):
+def test_single_map_loss_inputs_entry(case, train_precision, kind):
     """A loss that reads only weights, or only disp_map: backward runs with the rgb / depth / acc cotangents NULL (and the
     other new one NULL too) and every gradient is within the gate."""
     scene, t_rand, G, Gm, _ = case
@@ -259,7 +259,7 @@ def test_chunked_render_map_grads(case, train_precision):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("train_precision", ["tc_tf32x3", "fp32"])
-def test_no_map_terms_pass_null_and_match_ray_entry(case, train_precision):
+def test_no_map_terms_inputs_entry_matches_ray_entry(case, train_precision):
     """A loss without disp_map or weights: the binding passes NULL for both, and on the same forward record the gradients are
     those of nb_render_bwd_rays.  The spy runs nb_render_bwd_rays first, into its own zeroed buffers, then the binding's
     call: so the record is also shown to be read-only to a backward.  On fp32 the ray gradients are deterministic and are
@@ -274,7 +274,7 @@ def test_no_map_terms_pass_null_and_match_ray_entry(case, train_precision):
     lib = ren.lib
     twin = {}
 
-    def rays_twin(ba, rest):
+    def rays_twin(ba, ig, stream):
         t = capi.nb_render_bwd_args.from_buffer_copy(ba)
         g = capi.nb_decoder_weights.from_buffer_copy(ba.grads.contents)
         twin["params"] = [torch.zeros(p.shape, dtype=torch.float32, device="cuda") for p in net.decoder_tensors()]
@@ -287,10 +287,10 @@ def test_no_map_terms_pass_null_and_match_ray_entry(case, train_precision):
         B, n = batch["ray_o"].shape[:2]
         shapes = {"R": (B, 3, 3), "Th": (B, 3), "ray_o": (B, n, 3), "ray_d": (B, n, 3)}
         ptrs = []
-        for k, p in zip(("R", "Th", "ray_o", "ray_d"), rest[:4]):
-            twin[k] = torch.zeros(shapes[k], dtype=torch.float32, device="cuda") if p.value else None
+        for k in ("R", "Th", "ray_o", "ray_d"):
+            twin[k] = torch.zeros(shapes[k], dtype=torch.float32, device="cuda") if getattr(ig, "d_" + k) else None
             ptrs.append(ctypes.c_void_p(twin[k].data_ptr() if twin[k] is not None else 0))
-        assert lib.nb_render_bwd_rays(ctypes.byref(t), *ptrs, rest[4]) == 0, lib.nb_last_error()
+        assert lib.nb_render_bwd_rays(ctypes.byref(t), *ptrs, stream) == 0, lib.nb_last_error()
     spy = ren.lib = _Spy(lib, rays_twin)
     out = _render(ren, vols, batch, t_rand)
     MC.loss_of(out, {k: v.cuda() for k, v in G.items()}, tuple(t.cuda() for t in Gm), terms=False).backward()
