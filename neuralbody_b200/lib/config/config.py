@@ -106,7 +106,9 @@ def _defaults():
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
                                         # (meets the 1e-3 parity gate) | "tc_fp16" wgmma 1-pass (fastest, ~4e-3 on depth)
-    c.render_volume_dtype = "auto"      # "auto": fp16 volume for tc_fp16, fp32 otherwise
+    c.render_volume_dtype = "auto"      # "auto": fp16 volume for tc_fp16, fp32 otherwise | "fp32" | "fp16".  A training call on
+                                        # the exact kernel (render_train_precision 'fp32') packs fp32 whatever this says: its
+                                        # backward reads the fp32 volume only
     c.render_skip_empty = True          # tensor-core modes: exact empty-sample skipping (bit-identical outputs)
     c.render_return_weights = True      # 'weights' (B,n,S) is unused downstream; may be skipped
     c.render_train_precision = 'tc_tf32x3'   # calls autograd records: 'tc_tf32x3' (wgmma TF32 GEMM chains over the sample list) | 'fp32' (exact FFMA kernels)

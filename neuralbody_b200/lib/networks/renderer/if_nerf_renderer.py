@@ -260,8 +260,10 @@ class Renderer:
             t_rand = None
         elif t_rand is None and float(cfg.perturb) > 0. and self.net.training:
             t_rand = self._draw_t_rand(B, n, S, dev)
+        # the exact kernel's backward reads the fp32 volume only: a call that records activations for it packs that one
+        vdtype = capi.NB_DTYPE_F32 if needs_grad and precision == capi.NB_PRECISION_FP32 else self._volume_dtype(precision)
         call = {
-            "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": self._volume_dtype(precision),
+            "B": B, "n": n, "S": S, "dev": dev, "precision": precision, "vdtype": vdtype,
             "ray_o": _f32c(ray_o.detach(), dev), "ray_d": _f32c(ray_d.detach(), dev),
             "near": _f32c(near.detach(), dev), "far": _f32c(far.detach(), dev),
             "input_like": [None if t is None else (t.shape, t.dtype, t.device) for t in inputs],

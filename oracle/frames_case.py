@@ -45,11 +45,14 @@ def _ray_subset(total, n, W):
     return (torch.arange(n) * total) // n + (total // n) // 2
 
 
-def build(n_samples=N_SAMPLES, n_rays=N_RAYS, variant="distinct", batch=3, frames=None):
+def build(n_samples=N_SAMPLES, n_rays=N_RAYS, variant="distinct", batch=3, frames=None, volume_dtype=None, subnormal=False):
     """(scene, t_rand, G, Gm): `batch` frames (or the frames listed in `frames`) of the distinct case, n_rays rays each,
     jitter t_rand (B,n,S) and the cotangents G (rgb, depth, acc; grad_case.loss_of) and Gm (disp, weights;
     map_grad_case.loss_of), all from seed 77 -- drawn for the full 3-frame batch and sliced, so a sub-batch sees the same
-    numbers as those frames of the full one."""
+    numbers as those frames of the full one.
+    volume_dtype (e.g. torch.float16): every volume is rounded to it (synth.round_volumes; `subnormal` scales level 0 into
+    the fp16 subnormal range first) BEFORE the samples are conditioned, since the rounding moves the decoder's
+    pre-activations and the kink margins must hold on the volumes the kernels read."""
     from oracle import synth
     assert variant in VARIANTS, variant
     ids = list(range(batch)) if frames is None else list(frames)
@@ -70,6 +73,10 @@ def build(n_samples=N_SAMPLES, n_rays=N_RAYS, variant="distinct", batch=3, frame
     scene = {k: torch.cat([p[k] for p in parts], 0).contiguous() for k in FRAME_KEYS}
     scene["volumes"] = [torch.cat([p["volumes"][l] for p in parts], 0).contiguous() for l in range(4)]
     scene["weights"], scene["voxel_size"] = parts[0]["weights"], parts[0]["voxel_size"]
+    if volume_dtype is not None:
+        scene["volumes"] = synth.round_volumes(scene["volumes"], volume_dtype, subnormal)
+    else:
+        assert not subnormal, "the subnormal variant is a rounded case (volume_dtype)"
     empty = {"distinct": (), "middle_empty": (1,), "all_empty": tuple(range(3))}[variant]
     for b in empty:
         # beyond the far side of the padded box the ray only moves away from the body: every sample has zero features

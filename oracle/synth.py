@@ -398,6 +398,28 @@ def make_scene(seed=313, H=512, W=512, scale=1.0, voxel_size=(0.005, 0.005, 0.00
     return scene
 
 
+SUBNORMAL_SCALE = 2.0 ** -20   # relu(N(0,1)) * 2^-20 lies mostly below fp16's smallest normal 2^-14
+
+
+def round_volumes(volumes, dtype=torch.float16, subnormal=False):
+    """The volumes as a `dtype` blob holds them: every value rounded to `dtype` (round to nearest even) and back to float32,
+    so that an fp32 and an fp16 pack of the result contain the same numbers.  subnormal=True first scales level 0 by
+    SUBNORMAL_SCALE, which puts most of its non-zero values in the fp16 subnormal range."""
+    out = []
+    for l, v in enumerate(volumes):
+        if subnormal and l == 0:
+            v = v * SUBNORMAL_SCALE
+        out.append(v.to(dtype).float().contiguous())
+    return out
+
+
+def rounded_scene(scene, dtype=torch.float16, subnormal=False):
+    """A copy of a make_scene scene whose volumes are round_volumes(scene['volumes'], dtype, subnormal)."""
+    sc = dict(scene)
+    sc["volumes"] = round_volumes(scene["volumes"], dtype, subnormal)
+    return sc
+
+
 def make_mask_views(scene, nv=4, H=128, W=128, radius=3, distance=None):
     """Inputs of the masked renderers (lib/networks/renderer/if_clight_renderer_mmsk.py:12-45): `nv` training
     views around the body with their world->camera RT (nv,3,4), intrinsics Ks (nv,3,3) and foreground masks

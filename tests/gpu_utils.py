@@ -63,6 +63,22 @@ def render_product(scene, n_samples=64, perturb=0.0, training=False, white_bkgd=
     return {k: v.detach().cpu() for k, v in out.items()}
 
 
+def backward_kernel_names(loss, settle_s=0.1):
+    """Names of the CUDA kernels and memsets `loss.backward()` enqueues, from torch.profiler.  The profiler keeps only the
+    device activities that start inside its capture window, whose start is a host timestamp taken when the trace starts;
+    the device timestamps are converted to that clock.  A kernel launched right after the start can be stamped just before
+    it and is dropped: on a busy host the first kernels of a backward (its loss-gradient multiplies, the gradient zeroing)
+    were seen missing.  So the backward is launched `settle_s` after the trace started, on an idle device."""
+    import time
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(settle_s)
+        loss.backward()
+        torch.cuda.synchronize()
+    return {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+
+
 def compare(out, gold, atol_main, atol_weights=None, nan_mismatch_frac=0.0, label=""):
     """max-abs comparison of the five outputs.  rgb_map / depth_map / acc_map / weights: absolute;
     disp_map = 1/(depth/acc) is ill-conditioned where acc ~ 0, so it is compared relatively on rays

@@ -369,15 +369,10 @@ def test_camera_refinement_chain(case, train_precision):
 
 
 def _backward_kernel_names(scene, t_rand, G, train_precision, depths):
-    from torch.profiler import ProfilerActivity, profile
+    import gpu_utils as Gu
     net, ren, vols, batch = _setup(scene, train_precision, decoder=True, rays=True, near_far=depths, bounds=depths)
     out = _render(ren, vols, batch, t_rand)
-    loss = _loss(G, "cuda")(out)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        loss.backward()
-        torch.cuda.synchronize()
-    return {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+    return Gu.backward_kernel_names(_loss(G, "cuda")(out))
 
 
 @pytest.mark.gpu

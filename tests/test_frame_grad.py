@@ -154,19 +154,14 @@ def test_hierarchical_frame_grads(case, train_precision):
 
 
 def _backward_kernel_names(scene, t_rand, G, frame):
-    from torch.profiler import ProfilerActivity, profile
+    import gpu_utils as Gu
     net, ren, vols, batch = _setup(scene, "tc_tf32x3", (1, 3), decoder=True)
     if not frame:
         batch["R"].requires_grad_(False)
         batch["Th"].requires_grad_(False)
     sp = ren.prepare_sp_input(batch)
     out = ren.render_rays(batch["ray_o"], batch["ray_d"], batch["near"], batch["far"], vols, sp, t_rand=t_rand.cuda())
-    loss = grad_case.loss_of(out, {k: v.cuda() for k, v in G.items()})
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        loss.backward()
-        torch.cuda.synchronize()
-    return {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+    return Gu.backward_kernel_names(grad_case.loss_of(out, {k: v.cuda() for k, v in G.items()}))
 
 
 @pytest.mark.gpu

@@ -314,15 +314,11 @@ def test_no_map_terms_inputs_entry_matches_ray_entry(case, train_precision):
 
 
 def _backward_kernel_names(scene, t_rand, G, Gm, train_precision, terms):
-    from torch.profiler import ProfilerActivity, profile
+    import gpu_utils as Gu
     net, ren, vols, batch = _setup(scene, train_precision)
     out = _render(ren, vols, batch, t_rand)
-    loss = MC.loss_of(out, {k: v.cuda() for k, v in G.items()}, tuple(t.cuda() for t in Gm), terms=terms)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        loss.backward()
-        torch.cuda.synchronize()
-    return {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+    return Gu.backward_kernel_names(MC.loss_of(out, {k: v.cuda() for k, v in G.items()}, tuple(t.cuda() for t in Gm),
+                                               terms=terms))
 
 
 @pytest.mark.gpu

@@ -223,18 +223,13 @@ def test_mask_views_reject_ray_grads(case):
 
 
 def _backward_kernel_names(scene, t_rand, G, train_precision, rays):
-    from torch.profiler import ProfilerActivity, profile
+    import gpu_utils as Gu
     net, ren, vols, batch = _setup(scene, train_precision, decoder=True)
     if not rays:
         batch["ray_o"].requires_grad_(False)
         batch["ray_d"].requires_grad_(False)
     out = _render(ren, vols, batch, t_rand)
-    loss = grad_case.loss_of(out, {k: v.cuda() for k, v in G.items()})
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        loss.backward()
-        torch.cuda.synchronize()
-    return {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+    return Gu.backward_kernel_names(grad_case.loss_of(out, {k: v.cuda() for k, v in G.items()}))
 
 
 @pytest.mark.gpu
