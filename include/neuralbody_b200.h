@@ -247,6 +247,27 @@ size_t nb_mcubes_workspace_bytes(int nx, int ny, int nz);   /* 0 for dims < 1 */
 int    nb_mcubes_count(const nb_mcubes_args* a, void* stream);
 int    nb_mcubes_emit(const nb_mcubes_args* a, void* stream);   /* after the caller read counts */
 
+/* The mesh dataset's world grid and its mask-view test (lib/datasets/light_stage/multi_view_mesh_dataset.py:117-160,
+ * prepare_inside_pts) on the device.  Grid point (i, j, k) is (x[i], y[j], z[k]); inside is written in the order of
+ * meshgrid(x, y, z, indexing='ij').reshape(-1, 3), k fastest, and the grid itself is never materialised.  Per point, the
+ * views are taken in order: the point is projected as base_utils.project does in fp32 (pts @ R^T + T, then @ K^T, then
+ * xy / z), rounded half to even, converted as numpy's astype(int32) converts (NaN or outside int32 -> INT_MIN) and clipped to
+ * [0, W-1] x [0, H-1]; the mask value there is read, and the point goes on to the next view only while that value is
+ * exactly 1.  inside = the last value read (uint8, as upstream; callers treat it as a bool).  Validation (null pointers,
+ * nv, H, W and grid dims >= 1, at most 2^31 points) happens before anything is enqueued; one launch. */
+typedef struct nb_mesh_inside_args {
+    const float* x;              /* device (nx) world x of the grid planes */
+    const float* y;              /* device (ny) */
+    const float* z;              /* device (nz) */
+    int nx, ny, nz;
+    const unsigned char* msks;   /* device (nv, H, W) uint8 mask views */
+    const float* RT;             /* device (nv,3,4) world->camera, metres */
+    const float* Ks;             /* device (nv,3,3) */
+    int nv, H, W;
+    unsigned char* inside;       /* device (nx, ny, nz) uint8, written */
+} nb_mesh_inside_args;
+int nb_mesh_inside(const nb_mesh_inside_args* a, void* stream);
+
 /* f-2: ray generation on the device.  Replaces the per-view numpy of get_rays (lib/utils/if_nerf/if_nerf_data_utils.py:8-21)
  * and get_near_far (:54-69) as called from image_rays (lib/utils/render_utils.py:120-137): fp64 arithmetic like upstream, fp32
  * results.  Writes ALL H*W pixels (row-major) plus mask_at_box; the caller compacts with the mask (upstream: ray_o[mask_at_box]).

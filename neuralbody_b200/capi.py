@@ -17,7 +17,7 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_render_bwd_maps", "nb_render_bwd_inputs", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
-           "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit"]
+           "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside"]
 
 
 class nb_volume_level(C.Structure):
@@ -68,6 +68,12 @@ class nb_mcubes_args(C.Structure):
     _fields_ = [("grid", C.c_void_p), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int), ("isovalue", C.c_double),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("counts", C.c_void_p),
                 ("vertices", C.c_void_p), ("triangles", C.c_void_p)]
+
+
+class nb_mesh_inside_args(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("z", C.c_void_p), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int),
+                ("msks", C.c_void_p), ("RT", C.c_void_p), ("Ks", C.c_void_p), ("nv", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("inside", C.c_void_p)]
 
 
 class nb_render_bwd_args(C.Structure):
@@ -160,6 +166,8 @@ def load(path=None):
     lib.nb_mcubes_count.argtypes = [C.POINTER(nb_mcubes_args), C.c_void_p]
     lib.nb_mcubes_emit.restype = C.c_int
     lib.nb_mcubes_emit.argtypes = [C.POINTER(nb_mcubes_args), C.c_void_p]
+    lib.nb_mesh_inside.restype = C.c_int
+    lib.nb_mesh_inside.argtypes = [C.POINTER(nb_mesh_inside_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

@@ -279,6 +279,26 @@ __device__ __forceinline__ int mask_pixel(float r, int size) {
     const long long q = (long long)rintf(r);
     return (int)(q < 0 ? 0 : (q > size - 1 ? size - 1 : q));
 }
+// The mesh dataset's rule (multi_view_mesh_dataset.py:131-133): np.round (half to even), then .astype(np.int32), then clip.
+// A NaN or a rounded value outside int32 converts to INT_MIN on x86, which the clip turns into 0 (not size - 1).
+__device__ __forceinline__ int mask_pixel_i32(float r, int size) {
+    const float q = rintf(r);
+    if (!(q < 2147483648.f) || q < 0.f) return 0;
+    const int i = (int)q;
+    return i > size - 1 ? size - 1 : i;
+}
+// The perspective projection of a world point into one mask view (base_utils.project), fp32: pts @ R^T + T, then @ K^T,
+// with RT (3,4) world->camera and K (3,3).  (ix, iy, iz) are the homogeneous pixel coordinates; the callers divide
+// (u = ix / iz, v = iy / iz, __fdiv_rn) and round with their own integer rule.
+__device__ __forceinline__ void project_view(const float* RT, const float* K, float wx, float wy, float wz, float& ix, float& iy,
+                                             float& iz) {
+    const float cx = __fadd_rn(fmaf(wz, RT[2], fmaf(wy, RT[1], __fmul_rn(wx, RT[0]))), RT[3]);
+    const float cy = __fadd_rn(fmaf(wz, RT[6], fmaf(wy, RT[5], __fmul_rn(wx, RT[4]))), RT[7]);
+    const float cz = __fadd_rn(fmaf(wz, RT[10], fmaf(wy, RT[9], __fmul_rn(wx, RT[8]))), RT[11]);
+    ix = fmaf(cz, K[2], fmaf(cy, K[1], __fmul_rn(cx, K[0])));
+    iy = fmaf(cz, K[5], fmaf(cy, K[4], __fmul_rn(cx, K[3])));
+    iz = fmaf(cz, K[8], fmaf(cy, K[7], __fmul_rn(cx, K[6])));
+}
 // The single-view variant (if_clight_renderer_msk.py:17-30) first moves the sample into the world of the snapshot frame:
 // can = (p - Th) @ R;  q = can @ R0^T + Th0.
 __device__ __forceinline__ bool inside_masks(const RenderParams& P, const FrameXf& f, float wx, float wy, float wz) {
@@ -293,15 +313,8 @@ __device__ __forceinline__ bool inside_masks(const RenderParams& P, const FrameX
         wz = __fadd_rn(fmaf(cz, __ldg(R0 + 8), fmaf(cy, __ldg(R0 + 7), __fmul_rn(cx, __ldg(R0 + 6)))), __ldg(P.mask_Th0 + 2));
     }
     for (int v = 0; v < P.mask_nv; ++v) {
-        const float* RT = P.mask_RT + v * 12;
-        const float* K = P.mask_Ks + v * 9;
-        // pts @ R^T + T, then @ K^T
-        const float cx = __fadd_rn(fmaf(wz, RT[2], fmaf(wy, RT[1], __fmul_rn(wx, RT[0]))), RT[3]);
-        const float cy = __fadd_rn(fmaf(wz, RT[6], fmaf(wy, RT[5], __fmul_rn(wx, RT[4]))), RT[7]);
-        const float cz = __fadd_rn(fmaf(wz, RT[10], fmaf(wy, RT[9], __fmul_rn(wx, RT[8]))), RT[11]);
-        const float ix = fmaf(cz, K[2], fmaf(cy, K[1], __fmul_rn(cx, K[0])));
-        const float iy = fmaf(cz, K[5], fmaf(cy, K[4], __fmul_rn(cx, K[3])));
-        const float iz = fmaf(cz, K[8], fmaf(cy, K[7], __fmul_rn(cx, K[6])));
+        float ix, iy, iz;
+        project_view(P.mask_RT + v * 12, P.mask_Ks + v * 9, wx, wy, wz, ix, iy, iz);
         const int u = mask_pixel(__fdiv_rn(ix, iz), P.mask_W), w = mask_pixel(__fdiv_rn(iy, iz), P.mask_H);
         if (!__ldg(P.mask_msks + ((size_t)v * P.mask_H + w) * P.mask_W + u)) return false;
     }

@@ -3,7 +3,10 @@
 grid -> cube -> marching cubes at `cfg.mesh_th`, all on the GPU.
 
 Same contract as upstream's `render(batch)` (:26-56): `batch['pts']` (1,X,Y,Z,3) world grid and `batch['inside']`
-(1,X,Y,Z) uint8 from lib/datasets/light_stage/multi_view_mesh_dataset.py:121-160; the inside points' raw sigma (no relu)
+(1,X,Y,Z) uint8 from lib/datasets/light_stage/multi_view_mesh_dataset.py:121-160.  A batch without them may carry the
+frame's mask views instead (`wbounds` (1,2,3), `RT` (1,nv,3,4), `Ks` (1,nv,3,3), `msks` (1,nv,H,W), as this package's
+drop-in lib/datasets/light_stage/multi_view_mesh_dataset.py returns them): the grid's axes and its mask-view test are then
+built here, the test on the device, with the same result.  The inside points' raw sigma (no relu)
 is scattered into a zero cube, padded by 10 on every side, and returned as `'cube'` (host float64 numpy, upstream's
 shape) with `'mesh'`, whose vertices are in padded index coordinates, as upstream leaves them.  B = 1, as upstream.
 
@@ -13,13 +16,55 @@ and marching cubes is this package's kernel (neuralbody_b200/mcubes.py), not PyM
 interpolated the same way in double, but a watertight triangulation and grid-ordered output.  `'mesh'` is
 `trimesh.Trimesh(vertices, triangles)` when trimesh is importable (upstream's call), else neuralbody_b200.mcubes.Mesh,
 which has what lib/visualizers/if_nerf_mesh.py uses (`.vertices`, `.faces`, `.export(path)` as binary PLY)."""
+import ctypes as C
+
+import numpy as np
 import torch
 
-from neuralbody_b200 import mcubes
+from neuralbody_b200 import capi, mcubes
 from neuralbody_b200.lib.config import get_active_cfg
 from neuralbody_b200.lib.networks.renderer import if_nerf_renderer
 
 PAD = 10   # np.pad(cube, 10) of if_mesh_renderer.py:47
+MASK_KEYS = ('wbounds', 'RT', 'Ks', 'msks')
+
+
+def world_axes(wbounds, voxel_size):
+    """multi_view_mesh_dataset.py:150-156: the x, y and z planes of the world grid (float32, as the grid's `pts`) over the
+    float32 world box wbounds (2,3), spaced cfg.voxel_size.  This is numpy's own arange on the dataset's operands (a
+    float32 bound, python floats), because its values follow numpy's scalar promotion: under NumPy 2 the second element
+    start + step is a float32 sum and the fill step is its float64 difference from start, so a restated formula would
+    not reproduce the dataset's grid."""
+    wb = np.asarray(wbounds, dtype=np.float32)
+    vs = [float(v) for v in voxel_size]
+    return [np.arange(wb[0, a], wb[1, a] + vs[a], vs[a]).astype(np.float32) for a in range(3)]
+
+
+def grid_inside(axes, RT, Ks, msks):
+    """prepare_inside_pts (multi_view_mesh_dataset.py:117-140) on the device, one nb_mesh_inside launch: axes = the grid's
+    x, y and z planes (CUDA fp32 vectors), RT (nv,3,4), Ks (nv,3,3), msks (nv,H,W) CUDA tensors on the same device.
+    -> inside (X,Y,Z) uint8, the last mask value each point read (views in order, on while it reads exactly 1)."""
+    if any(t.device.type != "cuda" for t in (RT, Ks, msks, *axes)):
+        raise RuntimeError("grid_inside needs CUDA tensors: there is no CPU implementation")
+    nv = int(msks.shape[0]) if msks.dim() == 3 else -1
+    if nv < 1 or tuple(RT.shape) != (nv, 3, 4) or tuple(Ks.shape) != (nv, 3, 3) or any(a.dim() != 1 for a in axes):
+        raise ValueError("grid_inside: msks must be (nv,H,W) with nv >= 1, RT (nv,3,4), Ks (nv,3,3) and the axes vectors; got "
+                         "%s, %s, %s" % (tuple(msks.shape), tuple(RT.shape), tuple(Ks.shape)))
+    dev = msks.device
+    with torch.cuda.device(dev):
+        x, y, z = (a.to(device=dev, dtype=torch.float32).contiguous() for a in axes)
+        m = msks.to(torch.uint8).contiguous()
+        rt = RT.to(torch.float32).contiguous()
+        ks = Ks.to(torch.float32).contiguous()
+        inside = torch.empty((len(x), len(y), len(z)), dtype=torch.uint8, device=dev)
+        a = capi.nb_mesh_inside_args()
+        a.x, a.y, a.z = x.data_ptr(), y.data_ptr(), z.data_ptr()
+        a.nx, a.ny, a.nz = inside.shape
+        a.msks, a.RT, a.Ks, a.inside = m.data_ptr(), rt.data_ptr(), ks.data_ptr(), inside.data_ptr()
+        a.nv, a.H, a.W = (int(s) for s in m.shape)
+        lib = capi.load()
+        capi.check(lib.nb_mesh_inside(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "nb_mesh_inside")
+    return inside
 
 
 class Renderer(if_nerf_renderer.Renderer):
@@ -28,11 +73,28 @@ class Renderer(if_nerf_renderer.Renderer):
 
     def density_cube(self, batch):
         """The padded density cube on the device (fp32: it holds the fp32 sigma and zeros, so it is exact as upstream's
-        float64 cube), shape (X + 20, Y + 20, Z + 20)."""
-        for k in ('pts', 'inside'):
-            if k not in batch:
-                raise KeyError("the mesh renderer needs batch['%s'] (lib/datasets/light_stage/multi_view_mesh_dataset.py:"
-                               "150-169: the world grid 'pts' (1,X,Y,Z,3) and its mask-view test 'inside' (1,X,Y,Z))" % k)
+        float64 cube), shape (X + 20, Y + 20, Z + 20).  The grid comes from the batch's `pts` / `inside` when both are
+        there, else from its mask views (`wbounds`, `RT`, `Ks`, `msks`; see `grid_from_masks`)."""
+        if 'pts' in batch and 'inside' in batch:
+            wpts, inside = self.grid_from_points(batch)
+        elif all(k in batch for k in MASK_KEYS):
+            wpts, inside = self.grid_from_masks(batch)
+        else:
+            raise KeyError("the mesh renderer needs either batch['pts'] (1,X,Y,Z,3) and batch['inside'] (1,X,Y,Z) (the world "
+                           "grid and its mask-view test, lib/datasets/light_stage/multi_view_mesh_dataset.py:150-169) or "
+                           "batch['wbounds'] (1,2,3), batch['RT'] (1,nv,3,4), batch['Ks'] (1,nv,3,3) and batch['msks'] "
+                           "(1,nv,H,W) (the frame's mask views, neuralbody_b200/lib/datasets/light_stage/"
+                           "multi_view_mesh_dataset.py); got keys %s" % sorted(batch))
+        sp_input = self.prepare_sp_input(batch)
+        feature_volume = self.net.encode_sparse_voxels(sp_input)
+        with torch.no_grad():
+            alpha = self.net.calculate_density(wpts, feature_volume, sp_input)     # one nb_decode_density launch
+            cube = torch.zeros(tuple(s + 2 * PAD for s in inside.shape), dtype=torch.float32, device=wpts.device)
+            cube[PAD:-PAD, PAD:-PAD, PAD:-PAD][inside] = alpha[0, :, 0]
+        return cube
+
+    def grid_from_points(self, batch):
+        """Upstream's contract: -> (the inside points (1,n,3), inside (X,Y,Z) bool) from batch['pts'] / batch['inside']."""
         pts, inside = batch['pts'], batch['inside']
         if pts.device.type != "cuda" or inside.device.type != "cuda":
             raise RuntimeError("the mesh renderer needs CUDA tensors: there is no CPU implementation")
@@ -40,14 +102,27 @@ class Renderer(if_nerf_renderer.Renderer):
             raise ValueError("batch['pts'] must be (1,X,Y,Z,3) and batch['inside'] (1,X,Y,Z) (B = 1, as upstream); got %s and %s"
                              % (tuple(pts.shape), tuple(inside.shape)))
         inside = inside[0].bool()
-        wpts = pts[0][inside][None]
-        sp_input = self.prepare_sp_input(batch)
-        feature_volume = self.net.encode_sparse_voxels(sp_input)
-        with torch.no_grad():
-            alpha = self.net.calculate_density(wpts, feature_volume, sp_input)     # one nb_decode_density launch
-            cube = torch.zeros(tuple(s + 2 * PAD for s in inside.shape), dtype=torch.float32, device=pts.device)
-            cube[PAD:-PAD, PAD:-PAD, PAD:-PAD][inside] = alpha[0, :, 0]
-        return cube
+        return pts[0][inside][None], inside
+
+    def grid_from_masks(self, batch):
+        """The same (inside points, inside) from the frame's mask views, without the (X,Y,Z,3) grid: the axes on the host
+        (`world_axes`), the mask-view test of prepare_inside_pts on the device (nb_mesh_inside, one launch), and the inside
+        points gathered from the axes at inside.nonzero() -- the values and the order of pts[0][inside]."""
+        wb, RT, Ks, msks = (batch[k] for k in MASK_KEYS)
+        if RT.device.type != "cuda" or Ks.device.type != "cuda" or msks.device.type != "cuda":
+            raise RuntimeError("the mesh renderer needs CUDA tensors: there is no CPU implementation")
+        nv = int(msks.shape[1]) if msks.dim() == 4 else -1
+        if (msks.dim() != 4 or msks.shape[0] != 1 or nv < 1 or tuple(RT.shape) != (1, nv, 3, 4)
+                or tuple(Ks.shape) != (1, nv, 3, 3) or tuple(wb.shape) != (1, 2, 3)):
+            raise ValueError("batch['msks'] must be (1,nv,H,W) with nv >= 1, batch['RT'] (1,nv,3,4), batch['Ks'] (1,nv,3,3) and "
+                             "batch['wbounds'] (1,2,3) (B = 1, as upstream); got %s, %s, %s and %s"
+                             % (tuple(msks.shape), tuple(RT.shape), tuple(Ks.shape), tuple(wb.shape)))
+        axes = [torch.from_numpy(a).to(msks.device) for a in world_axes(wb[0].detach().cpu().numpy(),
+                                                                         get_active_cfg().voxel_size)]
+        inside = grid_inside(axes, RT[0], Ks[0], msks[0]).bool()
+        ijk = inside.nonzero()
+        wpts = torch.stack([axes[0][ijk[:, 0]], axes[1][ijk[:, 1]], axes[2][ijk[:, 2]]], dim=1)
+        return wpts[None], inside
 
     def render(self, batch):
         cfg = get_active_cfg()

@@ -8,7 +8,14 @@ fp32 and tc_fp16x3 step by step in one process and reports the density ms of bot
 reports the points listed for the decoder and skipped (stats[1]) and the algorithmic rate on the evaluated points only:
 fc_0 (minus the layer-0 K-steps the tile's class skipped, as bench.py counts them for rays) + fc_1 + fc_2 + alpha_fc.
 
-Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab]
+--from-masks compares, in one process and alternating frame by frame, the two ways the renderer gets its grid: (a) the
+upstream data path, the world grid and its mask-view test on this host (mesh_case.mesh_grid + mesh_inside, numpy, as the
+reference's mesh dataset builds them), the copy of `pts` / `inside` to the device and the render; (b) the copy of the
+mask views and cameras to the device and the render, which builds the grid's axes on the host and its test on the device
+(nb_mesh_inside).  4 synthetic 1024 x 1024 mask views; medians per frame of each step, the nb_mesh_inside kernel time
+from CUDA events over back-to-back launches, and whether the two cubes are identical.
+
+Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab | --from-masks]
 (upstream's default mesh_th = 50 lies above the synthetic body's sigma, p95 ~ 30, and would give an empty mesh)"""
 import argparse
 import json
@@ -54,7 +61,11 @@ def main():
     ap.add_argument("--mesh-th", type=float, default=10.0, help="isovalue (cfg.mesh_th)")
     ap.add_argument("--density-precision", choices=("fp32", "tc_fp16x3", "tc_fp16"), default="fp32")
     ap.add_argument("--ab", action="store_true", help="alternate fp32 and tc_fp16x3 density steps in one process")
+    ap.add_argument("--from-masks", action="store_true",
+                    help="compare the host-built grid / inside (upstream's data path) with the device-built one")
     args = ap.parse_args()
+    if args.from_masks:
+        return from_masks(args)
     arms = ("fp32", "tc_fp16x3") if args.ab else (args.density_precision,)
     if not torch.cuda.is_available():
         raise SystemExit("bench_mesh needs a CUDA device")
@@ -180,6 +191,129 @@ def main():
         "marching_cubes": {"bytes_as_written": mc_bytes, "gbs": mc_gbs, "fraction_of_hbm_datasheet": mc_gbs / (HBM_TBS_DATASHEET * 1e3),
                            "note": "includes the one host sync between count and emit and the launch gaps"},
         "density_precision": arm, "density_arms": density,
+        "card": card_info(dev),
+    }
+    print(json.dumps(line))
+
+
+def from_masks(args):
+    """--from-masks: arm (a) upstream's data path (host grid + host inside + H2D of pts / inside + render), arm (b) H2D of
+    the mask views and cameras + render from them; one JSON line."""
+    import ctypes as C
+    import time
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_mesh needs a CUDA device")
+    from oracle import mesh_case, synth
+    from neuralbody_b200 import capi
+    from neuralbody_b200.lib.config import cfg
+    from neuralbody_b200.lib.networks.make_network import make_network, load_source
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scene = synth.make_scene(**mesh_case.CASES["mesh_full"][0])
+    masks = synth.make_mask_views(scene, nv=4, H=1024, W=1024, radius=12)
+    Ks, Rs, Ts, msks = mesh_case._views(masks)
+    cfg.num_train_frame = int(scene["weights"]["latent.weight"].shape[0])
+    cfg.voxel_size = list(scene["voxel_size"])
+    cfg.mesh_th = float(args.mesh_th)
+    cfg.density_precision = args.density_precision
+    net = make_network(cfg)
+    net.load_state_dict(scene["weights"], strict=False)
+    net = net.to(dev).eval()
+    net.set_feature_volume([v.to(dev) for v in scene["volumes"]])
+    path = os.path.join(ROOT, "neuralbody_b200", "lib", "networks", "renderer", "if_mesh_renderer.py")
+    mod = load_source("neuralbody_b200.lib.networks.renderer.if_mesh_renderer", path)
+    ren = mod.Renderer(net)
+    frame = {k: scene[k].to(dev) for k in ("coord", "out_sh", "bounds", "R", "Th", "latent_index")}
+    cb = scene["can_bounds"][0].numpy()
+
+    def sync_ms(t0):
+        torch.cuda.synchronize(dev)
+        return (time.perf_counter() - t0) * 1e3
+
+    def arm_host():
+        t = time.perf_counter()
+        pts = mesh_case.mesh_grid(cb, scene["voxel_size"])
+        t_grid = (time.perf_counter() - t) * 1e3
+        t = time.perf_counter()
+        inside = mesh_case.mesh_inside(pts, Ks, Rs, Ts, msks)
+        t_inside = (time.perf_counter() - t) * 1e3
+        t = time.perf_counter()
+        b = dict(frame, pts=torch.from_numpy(pts)[None].to(dev), inside=torch.from_numpy(inside)[None].to(dev))
+        t_h2d = sync_ms(t)
+        t = time.perf_counter()
+        with torch.no_grad():
+            out = ren.render(b)
+        t_render = sync_ms(t)
+        return {"grid_host_ms": t_grid, "inside_host_ms": t_inside, "h2d_ms": t_h2d, "render_ms": t_render,
+                "h2d_bytes": pts.nbytes + inside.nbytes}, out, int(inside.astype(bool).sum())
+
+    def arm_device():
+        t = time.perf_counter()
+        b = dict(frame, wbounds=scene["can_bounds"].to(dev), RT=masks["RT"].to(dev), Ks=masks["Ks"].to(dev),
+                 msks=masks["msks"].to(dev))
+        t_h2d = sync_ms(t)
+        t = time.perf_counter()
+        with torch.no_grad():
+            wpts, _ = ren.grid_from_masks(b)
+        t_grid = sync_ms(t)
+        t = time.perf_counter()
+        with torch.no_grad():
+            out = ren.render(b)
+        t_render = sync_ms(t)
+        nbytes = sum(int(b[k].numel() * b[k].element_size()) for k in mod.MASK_KEYS)
+        return {"h2d_ms": t_h2d, "grid_from_masks_ms": t_grid, "render_ms": t_render, "h2d_bytes": nbytes}, out, int(wpts.shape[1])
+
+    for _ in range(args.warmup):
+        arm_host(); arm_device()
+    rows = {"a_host_grid": [], "b_device_grid": []}
+    for _ in range(args.steps):
+        ra, out_a, n_a = arm_host()
+        rb, out_b, n_b = arm_device()
+        rows["a_host_grid"].append(ra)
+        rows["b_device_grid"].append(rb)
+    med = {arm: {k: float(np.median([r[k] for r in rs])) for k in rs[0]} for arm, rs in rows.items()}
+    med["a_host_grid"]["frame_ms"] = sum(med["a_host_grid"][k] for k in ("grid_host_ms", "inside_host_ms", "h2d_ms", "render_ms"))
+    med["b_device_grid"]["frame_ms"] = sum(med["b_device_grid"][k] for k in ("h2d_ms", "render_ms"))
+
+    # nb_mesh_inside alone: back-to-back launches between two CUDA events
+    axes = [torch.from_numpy(a).to(dev) for a in mod.world_axes(cb, scene["voxel_size"])]
+    m, rt = masks["msks"][0].to(dev).contiguous(), masks["RT"][0].to(dev).contiguous()
+    ks = masks["Ks"][0].to(dev).contiguous()
+    inside = torch.empty(tuple(len(a) for a in axes), dtype=torch.uint8, device=dev)
+    a = capi.nb_mesh_inside_args()
+    a.x, a.y, a.z = (t.data_ptr() for t in axes)
+    a.nx, a.ny, a.nz = inside.shape
+    a.msks, a.RT, a.Ks, a.inside = m.data_ptr(), rt.data_ptr(), ks.data_ptr(), inside.data_ptr()
+    a.nv, a.H, a.W = (int(s) for s in m.shape)
+    lib, stream = capi.load(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    launches = 200
+    for _ in range(20):
+        capi.check(lib.nb_mesh_inside(C.byref(a), stream), "nb_mesh_inside")
+    kernel_ms = []
+    for _ in range(5):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(launches):
+            lib.nb_mesh_inside(C.byref(a), stream)
+        e1.record()
+        torch.cuda.synchronize(dev)
+        kernel_ms.append(e0.elapsed_time(e1) / launches)
+    n_pts = inside.numel()
+    line = {
+        "metric": "mesh_frame_ms_from_masks", "value": med["b_device_grid"]["frame_ms"], "unit": "ms", "higher_is_better": False,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "data": "synthetic",
+        "config": {"workload": "mesh renderer on the full-size synth-313 frame: 5 mm world grid %s (%d points), 4 synthetic "
+                               "1024x1024 mask views, density %s, mesh_th = %g; render = the whole Renderer.render call "
+                               "(cube copy to the host included)" % (tuple(inside.shape), n_pts, args.density_precision,
+                                                                     cfg.mesh_th)},
+        "inside_points": {"a": n_a, "b": n_b},
+        "cubes_identical": bool(out_a["cube"].shape == out_b["cube"].shape and np.array_equal(out_a["cube"], out_b["cube"])),
+        "meshes_identical": bool(np.array_equal(np.asarray(out_a["mesh"].faces), np.asarray(out_b["mesh"].faces)) and
+                                 np.array_equal(np.asarray(out_a["mesh"].vertices), np.asarray(out_b["mesh"].vertices))),
+        "median_ms": med, "speedup_frame": med["a_host_grid"]["frame_ms"] / med["b_device_grid"]["frame_ms"],
+        "nb_mesh_inside_kernel_ms": {"median": float(np.median(kernel_ms)), "all": kernel_ms, "launches_per_sample": launches,
+                                     "gpoints_per_s": n_pts / (float(np.median(kernel_ms)) * 1e-3) / 1e9},
+        "host_cpus": os.cpu_count(), "numpy": np.__version__,
         "card": card_info(dev),
     }
     print(json.dumps(line))
