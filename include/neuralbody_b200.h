@@ -267,6 +267,13 @@ typedef struct nb_mesh_inside_args {
     unsigned char* inside;       /* device (nx, ny, nz) uint8, written */
 } nb_mesh_inside_args;
 int nb_mesh_inside(const nb_mesh_inside_args* a, void* stream);
+/* The same test with a float64 camera (lib/datasets/light_stage/monocular_mesh_dataset.py:35-48, whose K, R and T are
+ * float64, so numpy projects the float32 grid in float64): RT (nv,3,4) and Ks (nv,3,3) are device doubles passed here, and
+ * a->RT / a->Ks must be NULL; everything else is read from `a` as nb_mesh_inside reads it.  Per point and view: the grid
+ * point widened to double, pts @ R^T + T, then @ K^T, then xy / z, in double with the product and sum order of the fp32
+ * chain; rounded half to even, converted as numpy's astype(int32) converts a float64 (NaN or outside int32 -> INT_MIN),
+ * clipped.  The view loop and `inside` are nb_mesh_inside's.  Validated as nb_mesh_inside, before anything is enqueued. */
+int nb_mesh_inside_f64(const nb_mesh_inside_args* a, const double* RT, const double* Ks, void* stream);
 
 /* f-2: ray generation on the device.  Replaces the per-view numpy of get_rays (lib/utils/if_nerf/if_nerf_data_utils.py:8-21)
  * and get_near_far (:54-69) as called from image_rays (lib/utils/render_utils.py:120-137): fp64 arithmetic like upstream, fp32

@@ -17,7 +17,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_render_bwd_maps", "nb_render_bwd_inputs", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
-           "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside"]
+           "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
+           "nb_mesh_inside_f64"]
 
 
 class nb_volume_level(C.Structure):
@@ -168,6 +169,8 @@ def load(path=None):
     lib.nb_mcubes_emit.argtypes = [C.POINTER(nb_mcubes_args), C.c_void_p]
     lib.nb_mesh_inside.restype = C.c_int
     lib.nb_mesh_inside.argtypes = [C.POINTER(nb_mesh_inside_args), C.c_void_p]
+    lib.nb_mesh_inside_f64.restype = C.c_int
+    lib.nb_mesh_inside_f64.argtypes = [C.POINTER(nb_mesh_inside_args), C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

@@ -299,6 +299,27 @@ __device__ __forceinline__ void project_view(const float* RT, const float* K, fl
     iy = fmaf(cz, K[5], fmaf(cy, K[4], __fmul_rn(cx, K[3])));
     iz = fmaf(cz, K[8], fmaf(cy, K[7], __fmul_rn(cx, K[6])));
 }
+// The same two steps for a float64 camera (the monocular mesh dataset's, monocular_mesh_dataset.py:35-48): numpy promotes
+// the float32 grid point to float64, so the point is widened exactly and the chain above runs in double, in the same
+// product and sum order.
+__device__ __forceinline__ int mask_pixel_i32(double r, int size) {
+    const double q = rint(r);
+    if (!(q < 2147483648.0) || q < 0.0) return 0;
+    const int i = (int)q;
+    return i > size - 1 ? size - 1 : i;
+}
+__device__ __forceinline__ void project_view(const double* RT, const double* K, float px, float py, float pz, double& ix,
+                                             double& iy, double& iz) {
+    const double wx = px, wy = py, wz = pz;
+    const double cx = __dadd_rn(fma(wz, RT[2], fma(wy, RT[1], __dmul_rn(wx, RT[0]))), RT[3]);
+    const double cy = __dadd_rn(fma(wz, RT[6], fma(wy, RT[5], __dmul_rn(wx, RT[4]))), RT[7]);
+    const double cz = __dadd_rn(fma(wz, RT[10], fma(wy, RT[9], __dmul_rn(wx, RT[8]))), RT[11]);
+    ix = fma(cz, K[2], fma(cy, K[1], __dmul_rn(cx, K[0])));
+    iy = fma(cz, K[5], fma(cy, K[4], __dmul_rn(cx, K[3])));
+    iz = fma(cz, K[8], fma(cy, K[7], __dmul_rn(cx, K[6])));
+}
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 // The single-view variant (if_clight_renderer_msk.py:17-30) first moves the sample into the world of the snapshot frame:
 // can = (p - Th) @ R;  q = can @ R0^T + Th0.
 __device__ __forceinline__ bool inside_masks(const RenderParams& P, const FrameXf& f, float wx, float wy, float wz) {

@@ -7,12 +7,12 @@
 // nb_mcubes_emit (after the caller read the totals and allocated): the same threads write their vertices and
 // triangles at those offsets.  No atomics: the output order is the grid order, so the mesh is deterministic.
 //
-// nb_mesh_inside (the mesh dataset's prepare_inside_pts): one thread per world-grid point, k fastest; the point is built from
-// the three axis arrays and projected into the mask views with the masked renderers' projection (nb_device.cuh).
+// nb_mesh_inside (the multi-view mesh dataset's prepare_inside_pts, float32 camera): mesh_inside_kernel<float> of
+// nb_mesh_inside.cuh.
 #include <cub/device/device_scan.cuh>
 #include <thrust/iterator/transform_iterator.h>
 
-#include "nb_device.cuh"
+#include "nb_mesh_inside.cuh"
 
 #define NB_MC_TABLE_QUALIFIER static __constant__
 #include "nb_mc_table.h"
@@ -154,33 +154,6 @@ int mc_check(const nb_mcubes_args* a, const char* who, McGrid* g, McLayout* L) {
     return NB_OK;
 }
 
-constexpr int kInsideThreads = 256;
-
-struct InsideGrid {
-    const float *x, *y, *z;
-    unsigned ny, nz, n;         // n <= 2^31, so a point index fits in 32 bits
-    const unsigned char* msks;
-    const float *RT, *Ks;
-    int nv, H, W;
-    unsigned char* inside;
-};
-
-__global__ void __launch_bounds__(kInsideThreads) mesh_inside_kernel(const __grid_constant__ InsideGrid g) {
-    const unsigned p = blockIdx.x * kInsideThreads + threadIdx.x;
-    if (p >= g.n) return;
-    const unsigned nyz = g.ny * g.nz;
-    const unsigned i = p / nyz, r = p - i * nyz, j = r / g.nz, k = r - j * g.nz;
-    const float wx = __ldg(g.x + i), wy = __ldg(g.y + j), wz = __ldg(g.z + k);
-    unsigned char val = 1;
-    for (int v = 0; v < g.nv && val == 1; ++v) {
-        float ix, iy, iz;
-        project_view(g.RT + v * 12, g.Ks + v * 9, wx, wy, wz, ix, iy, iz);
-        const int u = mask_pixel_i32(__fdiv_rn(ix, iz), g.W), w = mask_pixel_i32(__fdiv_rn(iy, iz), g.H);
-        val = __ldg(g.msks + ((size_t)v * g.H + w) * g.W + u);
-    }
-    g.inside[p] = val;
-}
-
 }  // namespace
 }  // namespace nb
 
@@ -241,29 +214,7 @@ int nb_mesh_inside(const nb_mesh_inside_args* a, void* stream) {
         set_error("nb_mesh_inside: null argument");
         return NB_ERR_BAD_ARG;
     }
-    if (a->nv < 1 || a->H < 1 || a->W < 1) {
-        set_error("nb_mesh_inside: nv, H and W must be >= 1 (got nv = %d, %d x %d)", a->nv, a->H, a->W);
-        return NB_ERR_BAD_ARG;
-    }
-    if (a->nx < 1 || a->ny < 1 || a->nz < 1) {
-        set_error("nb_mesh_inside: grid dims must be >= 1 (got %d x %d x %d)", a->nx, a->ny, a->nz);
-        return NB_ERR_BAD_ARG;
-    }
-    const long long n = (long long)a->nx * a->ny * a->nz;
-    if (n > (1LL << 31)) {
-        set_error("nb_mesh_inside: a %d x %d x %d grid has more than 2^31 points", a->nx, a->ny, a->nz);
-        return NB_ERR_UNSUPPORTED;
-    }
-    InsideGrid g;
-    g.x = a->x; g.y = a->y; g.z = a->z;
-    g.ny = (unsigned)a->ny; g.nz = (unsigned)a->nz; g.n = (unsigned)n;
-    g.msks = a->msks; g.RT = a->RT; g.Ks = a->Ks;
-    g.nv = a->nv; g.H = a->H; g.W = a->W;
-    g.inside = a->inside;
-    mesh_inside_kernel<<<(unsigned)((n + kInsideThreads - 1) / kInsideThreads), kInsideThreads, 0, (cudaStream_t)stream>>>(g);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("nb_mesh_inside: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    return NB_OK;
+    return mesh_inside_launch<float>("nb_mesh_inside", a, a->RT, a->Ks, stream);
 }
 
 }  // extern "C"

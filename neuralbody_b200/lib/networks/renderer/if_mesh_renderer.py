@@ -5,8 +5,9 @@ grid -> cube -> marching cubes at `cfg.mesh_th`, all on the GPU.
 Same contract as upstream's `render(batch)` (:26-56): `batch['pts']` (1,X,Y,Z,3) world grid and `batch['inside']`
 (1,X,Y,Z) uint8 from lib/datasets/light_stage/multi_view_mesh_dataset.py:121-160.  A batch without them may carry the
 frame's mask views instead (`wbounds` (1,2,3), `RT` (1,nv,3,4), `Ks` (1,nv,3,3), `msks` (1,nv,H,W), as this package's
-drop-in lib/datasets/light_stage/multi_view_mesh_dataset.py returns them): the grid's axes and its mask-view test are then
-built here, the test on the device, with the same result.  The inside points' raw sigma (no relu)
+drop-ins lib/datasets/light_stage/multi_view_mesh_dataset.py (float32 camera) and monocular_mesh_dataset.py (nv = 1,
+float64 camera) return them): the grid's axes and its mask-view test are then built here, the test on the device in the
+camera's precision, with the same result.  The inside points' raw sigma (no relu)
 is scattered into a zero cube, padded by 10 on every side, and returned as `'cube'` (host float64 numpy, upstream's
 shape) with `'mesh'`, whose vertices are in padded index coordinates, as upstream leaves them.  B = 1, as upstream.
 
@@ -40,30 +41,51 @@ def world_axes(wbounds, voxel_size):
     return [np.arange(wb[0, a], wb[1, a] + vs[a], vs[a]).astype(np.float32) for a in range(3)]
 
 
+def camera_is_f64(RT, Ks):
+    """True for a float64 camera (both RT and Ks float64: the monocular mesh dataset's, projected in double by
+    nb_mesh_inside_f64), False otherwise (projected in fp32 by nb_mesh_inside, the multi-view dataset's float32 camera).
+    A camera with only one of the two in float64 is a ValueError: numpy would project it with a chain neither kernel
+    reproduces."""
+    f64 = (RT.dtype == torch.float64, Ks.dtype == torch.float64)
+    if f64[0] != f64[1]:
+        raise ValueError("the mask views' RT and Ks must both be float64 (projected in double) or neither; got %s and %s"
+                         % (RT.dtype, Ks.dtype))
+    return f64[0]
+
+
 def grid_inside(axes, RT, Ks, msks):
-    """prepare_inside_pts (multi_view_mesh_dataset.py:117-140) on the device, one nb_mesh_inside launch: axes = the grid's
-    x, y and z planes (CUDA fp32 vectors), RT (nv,3,4), Ks (nv,3,3), msks (nv,H,W) CUDA tensors on the same device.
-    -> inside (X,Y,Z) uint8, the last mask value each point read (views in order, on while it reads exactly 1)."""
+    """prepare_inside_pts (multi_view_mesh_dataset.py:117-140, monocular_mesh_dataset.py:35-48) on the device, one launch:
+    axes = the grid's x, y and z planes (CUDA fp32 vectors), RT (nv,3,4), Ks (nv,3,3), msks (nv,H,W) CUDA tensors on the
+    same device.  A float64 camera is projected in double (nb_mesh_inside_f64), any other in fp32 (nb_mesh_inside); see
+    `camera_is_f64`.  -> inside (X,Y,Z) uint8, the last mask value each point read (views in order, on while it reads
+    exactly 1)."""
     if any(t.device.type != "cuda" for t in (RT, Ks, msks, *axes)):
         raise RuntimeError("grid_inside needs CUDA tensors: there is no CPU implementation")
     nv = int(msks.shape[0]) if msks.dim() == 3 else -1
     if nv < 1 or tuple(RT.shape) != (nv, 3, 4) or tuple(Ks.shape) != (nv, 3, 3) or any(a.dim() != 1 for a in axes):
         raise ValueError("grid_inside: msks must be (nv,H,W) with nv >= 1, RT (nv,3,4), Ks (nv,3,3) and the axes vectors; got "
                          "%s, %s, %s" % (tuple(msks.shape), tuple(RT.shape), tuple(Ks.shape)))
+    f64 = camera_is_f64(RT, Ks)
+    cam_dtype = torch.float64 if f64 else torch.float32
     dev = msks.device
     with torch.cuda.device(dev):
         x, y, z = (a.to(device=dev, dtype=torch.float32).contiguous() for a in axes)
         m = msks.to(torch.uint8).contiguous()
-        rt = RT.to(torch.float32).contiguous()
-        ks = Ks.to(torch.float32).contiguous()
+        rt = RT.to(cam_dtype).contiguous()
+        ks = Ks.to(cam_dtype).contiguous()
         inside = torch.empty((len(x), len(y), len(z)), dtype=torch.uint8, device=dev)
         a = capi.nb_mesh_inside_args()
         a.x, a.y, a.z = x.data_ptr(), y.data_ptr(), z.data_ptr()
         a.nx, a.ny, a.nz = inside.shape
-        a.msks, a.RT, a.Ks, a.inside = m.data_ptr(), rt.data_ptr(), ks.data_ptr(), inside.data_ptr()
+        a.msks, a.inside = m.data_ptr(), inside.data_ptr()
         a.nv, a.H, a.W = (int(s) for s in m.shape)
         lib = capi.load()
-        capi.check(lib.nb_mesh_inside(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "nb_mesh_inside")
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        if f64:
+            capi.check(lib.nb_mesh_inside_f64(C.byref(a), rt.data_ptr(), ks.data_ptr(), stream), "nb_mesh_inside_f64")
+        else:
+            a.RT, a.Ks = rt.data_ptr(), ks.data_ptr()
+            capi.check(lib.nb_mesh_inside(C.byref(a), stream), "nb_mesh_inside")
     return inside
 
 
@@ -107,8 +129,10 @@ class Renderer(if_nerf_renderer.Renderer):
     def grid_from_masks(self, batch):
         """The same (inside points, inside) from the frame's mask views, without the (X,Y,Z,3) grid: the axes on the host
         (`world_axes`), the mask-view test of prepare_inside_pts on the device (nb_mesh_inside, one launch), and the inside
-        points gathered from the axes at inside.nonzero() -- the values and the order of pts[0][inside]."""
+        points gathered from the axes at inside.nonzero() -- the values and the order of pts[0][inside].  The camera's dtype
+        picks the projection: float64 RT / Ks (the monocular dataset's) are projected in double, float32 ones in fp32."""
         wb, RT, Ks, msks = (batch[k] for k in MASK_KEYS)
+        camera_is_f64(RT, Ks)
         if RT.device.type != "cuda" or Ks.device.type != "cuda" or msks.device.type != "cuda":
             raise RuntimeError("the mesh renderer needs CUDA tensors: there is no CPU implementation")
         nv = int(msks.shape[1]) if msks.dim() == 4 else -1

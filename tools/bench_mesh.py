@@ -13,9 +13,12 @@ upstream data path, the world grid and its mask-view test on this host (mesh_cas
 reference's mesh dataset builds them), the copy of `pts` / `inside` to the device and the render; (b) the copy of the
 mask views and cameras to the device and the render, which builds the grid's axes on the host and its test on the device
 (nb_mesh_inside).  4 synthetic 1024 x 1024 mask views; medians per frame of each step, the nb_mesh_inside kernel time
-from CUDA events over back-to-back launches, and whether the two cubes are identical.
+from CUDA events over back-to-back launches, and whether the two cubes are identical.  With --monocular the frame is the
+People-Snapshot one instead (tools/mesh_mono_case.py, the monocular mesh dataset's bounds): one 540 x 540 mask view (a 1080 x
+1080 frame at ratio 0.5) with the dataset's float64 camera, so (a) projects the grid in float64 numpy and (b) runs
+nb_mesh_inside_f64.
 
-Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab | --from-masks]
+Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab | --from-masks [--monocular]]
 (upstream's default mesh_th = 50 lies above the synthetic body's sigma, p95 ~ 30, and would give an empty mesh)"""
 import argparse
 import json
@@ -63,7 +66,11 @@ def main():
     ap.add_argument("--ab", action="store_true", help="alternate fp32 and tc_fp16x3 density steps in one process")
     ap.add_argument("--from-masks", action="store_true",
                     help="compare the host-built grid / inside (upstream's data path) with the device-built one")
+    ap.add_argument("--monocular", action="store_true",
+                    help="with --from-masks: the People-Snapshot frame (one view, float64 camera) instead of the 4-view one")
     args = ap.parse_args()
+    if args.monocular and not args.from_masks:
+        ap.error("--monocular goes with --from-masks")
     if args.from_masks:
         return from_masks(args)
     arms = ("fp32", "tc_fp16x3") if args.ab else (args.density_precision,)
@@ -209,9 +216,21 @@ def from_masks(args):
     from neuralbody_b200.lib.networks.make_network import make_network, load_source
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    scene = synth.make_scene(**mesh_case.CASES["mesh_full"][0])
-    masks = synth.make_mask_views(scene, nv=4, H=1024, W=1024, radius=12)
-    Ks, Rs, Ts, msks = mesh_case._views(masks)
+    if args.monocular:
+        from tools import mesh_mono_case as MM
+        scene, pkl, _, _ = MM.build_case("mono_full")
+        K = MM.get_camera(pkl)["K"].copy()
+        K[:2] = K[:2] * MM.RATIO                                     # the dataset's K after its resize, float64
+        msk = MM.silhouette(scene, K, 540, 540, 2)
+        Ks, Rs, Ts, msks = K[None], np.eye(3)[None], np.zeros((1, 3, 1)), msk[None]
+        masks = {"RT": torch.from_numpy(np.concatenate([Rs, Ts], axis=2))[None], "Ks": torch.from_numpy(Ks)[None],
+                 "msks": torch.from_numpy(msks)[None]}
+        host_inside = lambda pts: MM.mesh_inside_f64(pts, K, Rs[0], Ts[0], msk)    # noqa: E731
+    else:
+        scene = synth.make_scene(**mesh_case.CASES["mesh_full"][0])
+        masks = synth.make_mask_views(scene, nv=4, H=1024, W=1024, radius=12)
+        Ks, Rs, Ts, msks = mesh_case._views(masks)
+        host_inside = lambda pts: mesh_case.mesh_inside(pts, Ks, Rs, Ts, msks)    # noqa: E731
     cfg.num_train_frame = int(scene["weights"]["latent.weight"].shape[0])
     cfg.voxel_size = list(scene["voxel_size"])
     cfg.mesh_th = float(args.mesh_th)
@@ -235,7 +254,7 @@ def from_masks(args):
         pts = mesh_case.mesh_grid(cb, scene["voxel_size"])
         t_grid = (time.perf_counter() - t) * 1e3
         t = time.perf_counter()
-        inside = mesh_case.mesh_inside(pts, Ks, Rs, Ts, msks)
+        inside = host_inside(pts)
         t_inside = (time.perf_counter() - t) * 1e3
         t = time.perf_counter()
         b = dict(frame, pts=torch.from_numpy(pts)[None].to(dev), inside=torch.from_numpy(inside)[None].to(dev))
@@ -283,18 +302,25 @@ def from_masks(args):
     a = capi.nb_mesh_inside_args()
     a.x, a.y, a.z = (t.data_ptr() for t in axes)
     a.nx, a.ny, a.nz = inside.shape
-    a.msks, a.RT, a.Ks, a.inside = m.data_ptr(), rt.data_ptr(), ks.data_ptr(), inside.data_ptr()
+    a.msks, a.inside = m.data_ptr(), inside.data_ptr()
     a.nv, a.H, a.W = (int(s) for s in m.shape)
     lib, stream = capi.load(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if args.monocular:
+        entry = "nb_mesh_inside_f64"
+        launch = lambda: lib.nb_mesh_inside_f64(C.byref(a), rt.data_ptr(), ks.data_ptr(), stream)    # noqa: E731
+    else:
+        entry = "nb_mesh_inside"
+        a.RT, a.Ks = rt.data_ptr(), ks.data_ptr()
+        launch = lambda: lib.nb_mesh_inside(C.byref(a), stream)    # noqa: E731
     launches = 200
     for _ in range(20):
-        capi.check(lib.nb_mesh_inside(C.byref(a), stream), "nb_mesh_inside")
+        capi.check(launch(), entry)
     kernel_ms = []
     for _ in range(5):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(launches):
-            lib.nb_mesh_inside(C.byref(a), stream)
+            launch()
         e1.record()
         torch.cuda.synchronize(dev)
         kernel_ms.append(e0.elapsed_time(e1) / launches)
@@ -302,15 +328,17 @@ def from_masks(args):
     line = {
         "metric": "mesh_frame_ms_from_masks", "value": med["b_device_grid"]["frame_ms"], "unit": "ms", "higher_is_better": False,
         "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "data": "synthetic",
-        "config": {"workload": "mesh renderer on the full-size synth-313 frame: 5 mm world grid %s (%d points), 4 synthetic "
-                               "1024x1024 mask views, density %s, mesh_th = %g; render = the whole Renderer.render call "
-                               "(cube copy to the host included)" % (tuple(inside.shape), n_pts, args.density_precision,
-                                                                     cfg.mesh_th)},
+        "config": {"workload": "mesh renderer on the full-size synth-313 frame: 5 mm world grid %s (%d points), %s, "
+                               "density %s, mesh_th = %g; render = the whole Renderer.render call (cube copy to the host "
+                               "included)" % (tuple(inside.shape), n_pts, "one synthetic 540x540 People-Snapshot mask view, "
+                                              "float64 camera" if args.monocular else "4 synthetic 1024x1024 mask views",
+                                              args.density_precision, cfg.mesh_th)},
         "inside_points": {"a": n_a, "b": n_b},
         "cubes_identical": bool(out_a["cube"].shape == out_b["cube"].shape and np.array_equal(out_a["cube"], out_b["cube"])),
         "meshes_identical": bool(np.array_equal(np.asarray(out_a["mesh"].faces), np.asarray(out_b["mesh"].faces)) and
                                  np.array_equal(np.asarray(out_a["mesh"].vertices), np.asarray(out_b["mesh"].vertices))),
         "median_ms": med, "speedup_frame": med["a_host_grid"]["frame_ms"] / med["b_device_grid"]["frame_ms"],
+        "kernel": entry,
         "nb_mesh_inside_kernel_ms": {"median": float(np.median(kernel_ms)), "all": kernel_ms, "launches_per_sample": launches,
                                      "gpoints_per_s": n_pts / (float(np.median(kernel_ms)) * 1e-3) / 1e9},
         "host_cpus": os.cpu_count(), "numpy": np.__version__,
