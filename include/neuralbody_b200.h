@@ -299,6 +299,38 @@ int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, in
                         float* ray_o /* device (n_local,3) */, float* ray_d, float* near, float* far,
                         unsigned char* mask_at_box /* device (n_local) */, void* stream);
 
+/* The demo datasets' per-view rays (render_utils.image_rays, lib/utils/render_utils.py:120-137, as called by
+ * multi_view_demo_dataset.py:151, multi_view_perform_dataset.py:148 and monocular_demo_dataset.py:113) on the device, bit for
+ * bit: get_rays (if_nerf_data_utils.py:8-21) in the camera's scalar type with the product and sum order numpy's BLAS uses
+ * for upstream's two np.dot calls over the pixels, `.astype(np.float32)`, then get_near_far (:54-69) in float32 and the
+ * `ray_o[mask_at_box]` compaction in row-major pixel order.  The per-view host operands are upstream's own: K_inv =
+ * np.linalg.inv(K) and the camera centre o = -np.dot(R.T, T), both in the camera's dtype (their rounding belongs to the host
+ * LAPACK / BLAS, so the caller computes them as upstream does); R (3,3) and T (3) row-major; all four are HOST memory, read
+ * during the call.  The box is upstream's float32 can_bounds.
+ * Writes mask_at_box (H*W) and the first n entries of ray_o / ray_d (n,3) and near / far (n), n = the number of pixels whose
+ * ray enters the box, and n itself to `count` (device int32).  The caller reads count once (the one host synchronisation:
+ * upstream's n varies per view).  Validation (null pointers, H, W >= 1, H*W < 2^31, workspace size) happens before anything is
+ * enqueued; three launches (the box test, a CUB scan, the compacting write). */
+typedef struct nb_image_rays_args {
+    int H, W;
+    float bounds[6];             /* can_bounds (2,3): world box min, max */
+    void* workspace;             /* device scratch of nb_image_rays_workspace_bytes(H, W) bytes */
+    size_t workspace_bytes;
+    float* ray_o;                /* device, room for H*W rays (n,3) */
+    float* ray_d;                /* device, room for H*W rays (n,3), not normalised */
+    float* near;                 /* device, room for H*W (n) */
+    float* far;                  /* device, room for H*W (n) */
+    unsigned char* mask_at_box;  /* device (H*W) 0 / 1 */
+    int* count;                  /* device int32: n */
+} nb_image_rays_args;
+size_t nb_image_rays_workspace_bytes(int H, int W);   /* 0 for an invalid size */
+/* float32 camera (monocular_demo_dataset.py:109-112: RT and K cast to float32) */
+int nb_image_rays(const nb_image_rays_args* a, const float K_inv[9], const float R[9], const float T[3], const float o[3],
+                  void* stream);
+/* float64 camera (the multi-view demo / perform sets: gen_path's render_w2c and the annotation's K) */
+int nb_image_rays_f64(const nb_image_rays_args* a, const double K_inv[9], const double R[9], const double T[3],
+                      const double o[3], void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

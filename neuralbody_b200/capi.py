@@ -18,7 +18,7 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
-           "nb_mesh_inside_f64"]
+           "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64"]
 
 
 class nb_volume_level(C.Structure):
@@ -75,6 +75,12 @@ class nb_mesh_inside_args(C.Structure):
     _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("z", C.c_void_p), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int),
                 ("msks", C.c_void_p), ("RT", C.c_void_p), ("Ks", C.c_void_p), ("nv", C.c_int), ("H", C.c_int), ("W", C.c_int),
                 ("inside", C.c_void_p)]
+
+
+class nb_image_rays_args(C.Structure):
+    _fields_ = [("H", C.c_int), ("W", C.c_int), ("bounds", C.c_float * 6), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t), ("ray_o", C.c_void_p), ("ray_d", C.c_void_p), ("near", C.c_void_p),
+                ("far", C.c_void_p), ("mask_at_box", C.c_void_p), ("count", C.c_void_p)]
 
 
 class nb_render_bwd_args(C.Structure):
@@ -171,6 +177,12 @@ def load(path=None):
     lib.nb_mesh_inside.argtypes = [C.POINTER(nb_mesh_inside_args), C.c_void_p]
     lib.nb_mesh_inside_f64.restype = C.c_int
     lib.nb_mesh_inside_f64.argtypes = [C.POINTER(nb_mesh_inside_args), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.nb_image_rays_workspace_bytes.restype = C.c_size_t
+    lib.nb_image_rays_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    lib.nb_image_rays.restype = C.c_int
+    lib.nb_image_rays.argtypes = [C.POINTER(nb_image_rays_args)] + [C.POINTER(C.c_float)] * 4 + [C.c_void_p]
+    lib.nb_image_rays_f64.restype = C.c_int
+    lib.nb_image_rays_f64.argtypes = [C.POINTER(nb_image_rays_args)] + [C.POINTER(C.c_double)] * 4 + [C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

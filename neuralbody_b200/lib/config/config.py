@@ -101,6 +101,7 @@ def _defaults():
     c.ratio = 0.5
     c.num_train_frame = 60
     c.begin_ith_frame = 0               # the dataset's first frame (config.py:22)
+    c.ith_frame = 0                     # the frame the multi-view demo renders from every view (config.py:25)
     c.voxel_size = [0.005, 0.005, 0.005]
     c.big_box = False
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)

@@ -630,15 +630,46 @@ class Renderer:
         fine['z_std'] = torch.std(z_smp, dim=-1, unbiased=False)
         return fine
 
+    # ------------------------------------------------------------------ the demo datasets' camera
+    def camera_rays(self, batch):
+        """The rays of a batch that carries the render camera instead of them (this package's multi_view_demo_dataset,
+        multi_view_perform_dataset and monocular_demo_dataset drop-ins: `cam_RT`, `cam_K`, `can_bounds`), generated on the
+        device as upstream's render_utils.image_rays generates them on the host, bit for bit (neuralbody_b200.rays.
+        camera_image_rays; a float64 camera runs nb_image_rays_f64, a float32 one nb_image_rays, a mixed one is a
+        ValueError).  The camera is read from batch['meta'] when it is there: upstream's visualize loop (run.py) moves every
+        key but 'meta' to the GPU, and the drop-ins put a copy of the camera there, so reading it costs no device copy and
+        the view's one host synchronisation is reading n.  Without it the camera keys are copied to the host in one
+        transfer.  Sets batch['mask_at_box'] (1, H*W) bool on the device, which upstream's visualizers read; returns
+        ray_o, ray_d (1,n,3), near, far (1,n)."""
+        from neuralbody_b200 import rays
+        cfg = get_active_cfg()
+        keys = ('cam_RT', 'cam_K', 'can_bounds')
+        meta = batch.get('meta')
+        src = meta if isinstance(meta, dict) and all(k in meta for k in keys) else batch
+        if any(src[k].shape[0] != 1 for k in keys):
+            raise ValueError("a camera batch renders one view (batch size 1, as upstream's demo loaders)")
+        H, W = cfg.H * cfg.ratio, cfg.W * cfg.ratio
+        if H != int(H) or W != int(W):
+            raise ValueError("cfg.H * cfg.ratio and cfg.W * cfg.ratio must be whole pixels (got %s x %s)" % (H, W))
+        dev = batch['coord'].device if batch['coord'].device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+        ray_o, ray_d, near, far, mask = rays.camera_image_rays(src['cam_RT'][0], src['cam_K'][0], src['can_bounds'][0],
+                                                               int(H), int(W), device=dev)
+        batch['mask_at_box'] = mask[None]
+        return ray_o[None], ray_d[None], near[None], far[None]
+
     # ------------------------------------------------------------------ a1
     def render(self, batch):
         """if_clight_renderer.py:94-122.  `cfg.chunk` rays per launch (0 = everything in one
         launch; upstream hard-codes 2048 to bound activation memory, which the fused kernel
-        never materialises)."""
-        ray_o = batch['ray_o']
-        ray_d = batch['ray_d']
-        near = batch['near']
-        far = batch['far']
+        never materialises).  A batch without `ray_o` but with the render camera (`cam_RT`, `cam_K`, `can_bounds`) gets
+        its rays from `camera_rays`."""
+        if 'ray_o' not in batch and 'cam_RT' in batch:
+            ray_o, ray_d, near, far = self.camera_rays(batch)
+        else:
+            ray_o = batch['ray_o']
+            ray_d = batch['ray_d']
+            near = batch['near']
+            far = batch['far']
 
         sp_input = self.prepare_sp_input(batch)
         feature_volume = self.net.encode_sparse_voxels(sp_input)

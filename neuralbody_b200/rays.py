@@ -55,6 +55,72 @@ class ShardedRays:
         return self
 
 
+def _host(*xs):
+    """numpy copies of numpy arrays / tensors.  The device tensors among them come over in ONE copy (widened to float64,
+    which holds float32 values exactly, and narrowed back), so a camera left on the GPU costs one host synchronisation."""
+    dev = [x for x in xs if torch.is_tensor(x) and x.device.type != "cpu"]
+    flat = torch.cat([x.detach().reshape(-1).to(torch.float64) for x in dev]).cpu().numpy() if dev else None
+    out, at = [], 0
+    for x in xs:
+        if torch.is_tensor(x) and x.device.type != "cpu":
+            n = x.numel()
+            out.append(flat[at:at + n].reshape(tuple(x.shape)).astype(str(x.dtype).replace("torch.", "")))
+            at += n
+        else:
+            out.append(x.detach().numpy() if torch.is_tensor(x) else np.asarray(x))
+    return out
+
+
+def camera_image_rays(RT, K, bounds, H, W, device="cuda:0"):
+    """render_utils.image_rays (render_utils.py:120-137) bit for bit, on the device (nb_image_rays / nb_image_rays_f64).
+    RT (3,4) or (4,4) world->camera and K (3,3), both float32 or both float64 as the dataset holds them (numpy arrays or
+    tensors); bounds (2,3) the float32 can_bounds; H, W the image size.  -> ray_o, ray_d (n,3), near, far (n,) float32 and
+    mask_at_box (H*W,) bool, torch tensors on `device`, in row-major pixel order.  inv(K) and the camera centre
+    -np.dot(R.T, T) are computed here with upstream's own numpy expressions, so the camera is needed on the host: a camera
+    given on the host costs one host synchronisation (reading n), one given as device tensors two (one copy of all of it
+    to the host, then n)."""
+    RT, K, bounds = _host(RT, K, bounds)
+    if RT.dtype != K.dtype or RT.dtype not in (np.float32, np.float64):
+        raise ValueError("the camera must be all float32 or all float64 (got RT %s, K %s)" % (RT.dtype, K.dtype))
+    if RT.shape not in ((3, 4), (4, 4)) or K.shape != (3, 3):
+        raise ValueError("RT must be (3,4) or (4,4) and K (3,3) (got %s and %s)" % (RT.shape, K.shape))
+    if bounds.dtype != np.float32 or bounds.shape != (2, 3):
+        raise ValueError("bounds must be the float32 (2,3) can_bounds (got %s %s)" % (bounds.dtype, bounds.shape))
+    lib = capi.load()
+    H, W = int(H), int(W)
+    nbytes = lib.nb_image_rays_workspace_bytes(H, W)
+    if nbytes == 0:
+        raise ValueError("bad image size %d x %d" % (H, W))
+    f64 = RT.dtype == np.float64
+    ct = C.c_double if f64 else C.c_float
+    R, T = RT[:3, :3], RT[:3, 3]
+    host = [np.ascontiguousarray(x, dtype=RT.dtype).reshape(-1)
+            for x in (np.linalg.inv(K), R, T, -np.dot(R.T, T).ravel())]   # get_rays :10 and :16, as upstream evaluates them
+    ptrs = [x.ctypes.data_as(C.POINTER(ct)) for x in host]
+    dev = torch.device(device)
+    n = H * W
+    with torch.cuda.device(dev):
+        ray_o = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        ray_d = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        near = torch.empty((n,), dtype=torch.float32, device=dev)
+        far = torch.empty((n,), dtype=torch.float32, device=dev)
+        mask = torch.empty((n,), dtype=torch.uint8, device=dev)
+        count = torch.empty((1,), dtype=torch.int32, device=dev)
+        ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        a = capi.nb_image_rays_args()
+        a.H, a.W = H, W
+        for i, v in enumerate(bounds.reshape(-1)):
+            a.bounds[i] = float(v)
+        a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
+        a.ray_o, a.ray_d, a.near, a.far = ray_o.data_ptr(), ray_d.data_ptr(), near.data_ptr(), far.data_ptr()
+        a.mask_at_box, a.count = mask.data_ptr(), count.data_ptr()
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        fn, name = (lib.nb_image_rays_f64, "nb_image_rays_f64") if f64 else (lib.nb_image_rays, "nb_image_rays")
+        capi.check(fn(C.byref(a), *ptrs, stream), name)
+        m = int(count.item())
+        return ray_o[:m], ray_d[:m], near[:m], far[:m], mask.bool()
+
+
 def image_rays(RT, K, bounds, H, W, device="cuda:0"):
     """RT (3,4) or (4,4) world->camera, K (3,3), bounds (2,3) world box -> ray_o, ray_d (n,3), near, far (n,), mask_at_box
     (H*W,) bool, all torch tensors on `device`; n = mask_at_box.sum() (order = row-major pixel order, as upstream)."""
