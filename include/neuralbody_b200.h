@@ -322,6 +322,11 @@ typedef struct nb_image_rays_args {
     float* far;                  /* device, room for H*W (n) */
     unsigned char* mask_at_box;  /* device (H*W) 0 / 1 */
     int* count;                  /* device int32: n */
+    const float* image;          /* device (H*W,3) or NULL: the view's image, whose box-hit pixels go to rgb (the training
+                                    datasets' test split, if_nerf_data_utils.py:139-145) */
+    float* rgb;                  /* device, room for H*W (n,3); set with image */
+    int k_f32;                   /* nb_image_rays_f64 only, nonzero: K is float32 (K_inv's values are float32's and
+                                    xy1 @ inv(K).T runs in float32, as for People-Snapshot's get_camera R and T) */
 } nb_image_rays_args;
 size_t nb_image_rays_workspace_bytes(int H, int W);   /* 0 for an invalid size */
 /* float32 camera (monocular_demo_dataset.py:109-112: RT and K cast to float32) */
@@ -330,6 +335,64 @@ int nb_image_rays(const nb_image_rays_args* a, const float K_inv[9], const float
 /* float64 camera (the multi-view demo / perform sets: gen_path's render_w2c and the annotation's K) */
 int nb_image_rays_f64(const nb_image_rays_args* a, const double K_inv[9], const double R[9], const double T[3],
                       const double o[3], void* stream);
+
+/* The training datasets' ray sampler (if_nerf_data_utils.sample_ray_h36m :153-219 for ZJU-MoCap's multi_view_dataset,
+ * sample_ray :72-137 for People-Snapshot's monocular_dataset, split 'train') on the device.  Per batch item b the caller
+ * hands the processed image and a class map built on the host from upstream's own masks; the call draws n_rays pixels in
+ * upstream's rounds and writes, for each, the ray, near, far and colour upstream's item carries:
+ *   - lists: the pixels of each class in row-major order (np.argwhere's), compacted by a CUB scan;
+ *   - rounds (one CTA per item): m = n_rays - sampled, n_body = int(m * body_ratio), n_face = int(m * face_ratio) (in
+ *     double, as Python), n_rand = m - n_body - n_face; candidates body, face (omitted when the face list is empty), bound,
+ *     in that order; the ones whose ray enters the box are appended in that order, until n_rays are sampled;
+ *   - a candidate's ray: get_rays (:8-21) at the pixel with the roundings of nb_image_rays, K_inv in K's dtype and R, T, o
+ *     in float64; get_near_far (:54-69) in float64 on the float64 ray and the promoted float32 can_bounds; ray_o, ray_d,
+ *     near and far rounded to float32 once; rgb gathered from the image.
+ * Randomness: `draws` != NULL replays upstream's np.random.randint results (tests): item b's draws are
+ * draws[draw_offset[b] .. draw_offset[b+1]), each round's body, face and bound draws in turn.  draws == NULL draws each
+ * index from Philox4x32-10 keyed by `key` (counter: the item, the round and the candidate), mapped to [0, len) by the
+ * 64-bit multiply-high.
+ * status[b] (device int32): NB_TRAIN_RAYS_OK, or an error: upstream would loop forever (NB_TRAIN_RAYS_ROUNDS: no n_rays
+ * after NB_TRAIN_RAYS_MAX_ROUNDS rounds), or would raise in randint (NB_TRAIN_RAYS_EMPTY: draws from an empty list), or
+ * the replayed draws do not fit the lists (NB_TRAIN_RAYS_REPLAY).  The slots of an item whose status is not OK are
+ * unspecified.  Validation (null pointers, sizes, ratios, kinds, workspace) happens before anything is enqueued; four
+ * kinds of launch (three scans, the list scatter, the sampler); nothing synchronises with the host. */
+#define NB_SCALAR_F32 0
+#define NB_SCALAR_F64 1
+#define NB_TRAIN_CAM_DOUBLES 30        /* per item: K_inv[9] | R[9] | T[3] | o[3] | can_bounds[6], row-major, as double */
+#define NB_TRAIN_CLASS_BODY 1          /* class map bits */
+#define NB_TRAIN_CLASS_FACE 2
+#define NB_TRAIN_CLASS_BOUND 4
+#define NB_TRAIN_RAYS_OK 0
+#define NB_TRAIN_RAYS_ROUNDS 1
+#define NB_TRAIN_RAYS_EMPTY 2
+#define NB_TRAIN_RAYS_REPLAY 3
+#define NB_TRAIN_RAYS_MAX_ROUNDS 64
+typedef struct nb_train_rays_args {
+    int B, H, W;
+    int n_rays;                      /* N_rand, >= 1 */
+    double body_ratio, face_ratio;   /* >= 0, body_ratio + face_ratio <= 1 */
+    int k_kind;                      /* NB_SCALAR_*: K's dtype (People-Snapshot: float32; ZJU-MoCap: float64) */
+    int rt_kind;                     /* R's and T's dtype: NB_SCALAR_F64 (both training datasets) */
+    const unsigned char* class_map;  /* device (B,H,W): NB_TRAIN_CLASS_* bits */
+    const float* image;              /* device (B,H,W,3) */
+    const double* cams;              /* device (B, NB_TRAIN_CAM_DOUBLES): K_inv = np.linalg.inv(K) and o = -np.dot(R.T, T)
+                                        as upstream computes them, each value exact in its kind */
+    const long long* draws;          /* device, or NULL for Philox */
+    const long long* draw_offset;    /* device (B+1), with draws */
+    unsigned long long key[2];       /* Philox key, without draws */
+    void* workspace;                 /* device scratch of nb_train_rays_workspace_bytes(B, H, W) bytes */
+    size_t workspace_bytes;
+    float* ray_o;                    /* device (B, n_rays, 3) */
+    float* ray_d;                    /* device (B, n_rays, 3) */
+    float* near;                     /* device (B, n_rays) */
+    float* far;                      /* device (B, n_rays) */
+    float* rgb;                      /* device (B, n_rays, 3) */
+    int* coord;                      /* device (B, n_rays) row-major pixel index of each slot, or NULL */
+    int* rounds;                     /* device (B) rounds run, or NULL */
+    int* status;                     /* device (B) */
+} nb_train_rays_args;
+size_t nb_train_rays_workspace_bytes(int B, int H, int W);   /* 0 for an invalid size */
+int nb_train_rays(const nb_train_rays_args* a, void* stream);
 
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for

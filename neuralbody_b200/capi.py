@@ -18,7 +18,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
-           "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64"]
+           "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
+           "nb_train_rays_workspace_bytes", "nb_train_rays"]
 
 
 class nb_volume_level(C.Structure):
@@ -77,10 +78,27 @@ class nb_mesh_inside_args(C.Structure):
                 ("inside", C.c_void_p)]
 
 
+NB_SCALAR_F32, NB_SCALAR_F64 = 0, 1
+NB_TRAIN_CAM_DOUBLES = 30
+NB_TRAIN_CLASS_BODY, NB_TRAIN_CLASS_FACE, NB_TRAIN_CLASS_BOUND = 1, 2, 4
+NB_TRAIN_RAYS_OK, NB_TRAIN_RAYS_ROUNDS, NB_TRAIN_RAYS_EMPTY, NB_TRAIN_RAYS_REPLAY = 0, 1, 2, 3
+NB_TRAIN_RAYS_MAX_ROUNDS = 64
+
+
+class nb_train_rays_args(C.Structure):
+    _fields_ = [("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("n_rays", C.c_int), ("body_ratio", C.c_double),
+                ("face_ratio", C.c_double), ("k_kind", C.c_int), ("rt_kind", C.c_int), ("class_map", C.c_void_p),
+                ("image", C.c_void_p), ("cams", C.c_void_p), ("draws", C.c_void_p), ("draw_offset", C.c_void_p),
+                ("key", C.c_ulonglong * 2), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+                ("ray_o", C.c_void_p), ("ray_d", C.c_void_p), ("near", C.c_void_p), ("far", C.c_void_p), ("rgb", C.c_void_p),
+                ("coord", C.c_void_p), ("rounds", C.c_void_p), ("status", C.c_void_p)]
+
+
 class nb_image_rays_args(C.Structure):
     _fields_ = [("H", C.c_int), ("W", C.c_int), ("bounds", C.c_float * 6), ("workspace", C.c_void_p),
                 ("workspace_bytes", C.c_size_t), ("ray_o", C.c_void_p), ("ray_d", C.c_void_p), ("near", C.c_void_p),
-                ("far", C.c_void_p), ("mask_at_box", C.c_void_p), ("count", C.c_void_p)]
+                ("far", C.c_void_p), ("mask_at_box", C.c_void_p), ("count", C.c_void_p), ("image", C.c_void_p),
+                ("rgb", C.c_void_p), ("k_f32", C.c_int)]
 
 
 class nb_render_bwd_args(C.Structure):
@@ -183,6 +201,10 @@ def load(path=None):
     lib.nb_image_rays.argtypes = [C.POINTER(nb_image_rays_args)] + [C.POINTER(C.c_float)] * 4 + [C.c_void_p]
     lib.nb_image_rays_f64.restype = C.c_int
     lib.nb_image_rays_f64.argtypes = [C.POINTER(nb_image_rays_args)] + [C.POINTER(C.c_double)] * 4 + [C.c_void_p]
+    lib.nb_train_rays_workspace_bytes.restype = C.c_size_t
+    lib.nb_train_rays_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    lib.nb_train_rays.restype = C.c_int
+    lib.nb_train_rays.argtypes = [C.POINTER(nb_train_rays_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

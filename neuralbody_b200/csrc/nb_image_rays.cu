@@ -16,7 +16,11 @@ size_t nb_image_rays_workspace_bytes(int H, int W) {
 
 int nb_image_rays(const nb_image_rays_args* a, const float K_inv[9], const float R[9], const float T[3], const float o[3],
                   void* stream) {
-    return image_rays_launch<float>("nb_image_rays", a, K_inv, R, T, o, stream);
+    if (a && a->k_f32) {
+        set_error("nb_image_rays: k_f32 is for nb_image_rays_f64 (a float32 K with a float64 R and T)");
+        return NB_ERR_BAD_ARG;
+    }
+    return image_rays_launch<float, float>("nb_image_rays", a, K_inv, R, T, o, stream);
 }
 
 }  // extern "C"

@@ -104,6 +104,9 @@ def _defaults():
     c.ith_frame = 0                     # the frame the multi-view demo renders from every view (config.py:25)
     c.voxel_size = [0.005, 0.005, 0.005]
     c.big_box = False
+    c.mask_bkgd = True                  # the training datasets' background (config.py:31)
+    c.body_sample_ratio = 0.5           # sample_ray's class split (config.py:128-129)
+    c.face_sample_ratio = 0.
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path

@@ -645,6 +645,8 @@ class Renderer:
         cfg = get_active_cfg()
         keys = ('cam_RT', 'cam_K', 'can_bounds')
         meta = batch.get('meta')
+        if isinstance(meta, dict) and 'train_cam' in meta and 'img' in batch:   # the training datasets' test split
+            return self._dataset_view_rays(batch, meta)
         src = meta if isinstance(meta, dict) and all(k in meta for k in keys) else batch
         if any(src[k].shape[0] != 1 for k in keys):
             raise ValueError("a camera batch renders one view (batch size 1, as upstream's demo loaders)")
@@ -657,13 +659,72 @@ class Renderer:
         batch['mask_at_box'] = mask[None]
         return ray_o[None], ray_d[None], near[None], far[None]
 
+    def _dataset_view_rays(self, batch, meta):
+        """camera_rays for the training datasets' test split (multi_view_dataset / monocular_dataset drop-ins): `img`
+        (1,H,W,3) and meta['train_cam'] / ['train_k_kind'] -> upstream's sample_ray(_h36m) test-split rays, bit for bit
+        (rays.dataset_image_rays); also sets batch['rgb'] (1,n,3) and batch['mask_at_box'] (1,H*W) on the device."""
+        from neuralbody_b200 import rays
+        img = batch['img']
+        if img.shape[0] != 1:
+            raise ValueError("a test-split batch renders one view (batch size 1, as upstream's test loader)")
+        dev = img.device if img.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+        H, W = int(img.shape[1]), int(img.shape[2])
+        ray_o, ray_d, near, far, mask, rgb = rays.dataset_image_rays(torch.as_tensor(meta['train_cam'])[0].numpy(),
+                                                                     int(torch.as_tensor(meta['train_k_kind']).reshape(-1)[0]),
+                                                                     H, W, img[0].to(dev), device=dev)
+        batch['mask_at_box'] = mask[None]
+        batch['rgb'] = rgb[None]
+        return ray_o[None], ray_d[None], near[None], far[None]
+
+    # ------------------------------------------------------------------ the training datasets' sampled rays
+    def train_rays(self, batch, draws=None):
+        """The rays of a training batch that carries the image instead of them (this package's multi_view_dataset and
+        monocular_dataset drop-ins, split 'train': `img` (B,H,W,3) float32, `ray_class` (B,H,W) uint8 and, in batch['meta']
+        on the host, `train_cam` (B, NB_TRAIN_CAM_DOUBLES), `train_k_kind`, `N_rand`, `body_sample_ratio` and
+        `face_sample_ratio`).  Draws N_rand pixels per item on the device as upstream's sample_ray_h36m / sample_ray do on
+        the host (neuralbody_b200.rays.train_rays; `draws`: upstream's recorded np.random.randint results, for tests) and
+        writes upstream's keys into the batch: ray_o, ray_d, rgb (B,N_rand,3), near, far (B,N_rand) float32 and an all-True
+        mask_at_box (B,N_rand) bool, on the image's device.  Nothing synchronises with the host: the sampler's status is
+        checked by the next render() after its prepare_sp_input, or by `check_train_rays()`.  A loop that refines cameras
+        calls this first and then edits the rays; they are constants, as upstream's are."""
+        from neuralbody_b200 import rays
+        meta = batch['meta']
+        img, cmap = batch['img'], batch['ray_class']
+        if img.device.type != "cuda":
+            dev = torch.device("cuda", torch.cuda.current_device())
+            img, cmap = img.to(dev, non_blocking=True), cmap.to(dev, non_blocking=True)
+        same = {}
+        for k in ('train_k_kind', 'N_rand', 'body_sample_ratio', 'face_sample_ratio'):
+            vals = set(torch.as_tensor(meta[k]).reshape(-1).tolist())
+            if len(vals) != 1:
+                raise ValueError("a training batch's items must share %s (got %s)" % (k, sorted(vals)))
+            same[k] = vals.pop()
+        res = rays.train_rays(img, cmap, torch.as_tensor(meta['train_cam']).numpy(), int(same['train_k_kind']),
+                              int(same['N_rand']), float(same['body_sample_ratio']), float(same['face_sample_ratio']),
+                              draws=draws)
+        batch.update({'ray_o': res.ray_o, 'ray_d': res.ray_d, 'near': res.near, 'far': res.far, 'rgb': res.rgb,
+                      'mask_at_box': torch.ones(tuple(res.near.shape), dtype=torch.bool, device=res.near.device)})
+        self._train_rays_pending = res
+        return res
+
+    def check_train_rays(self):
+        """Raise RuntimeError when the last train_rays call failed (a view whose bound pixels' rays all miss the box, where
+        upstream loops forever)."""
+        res = self.__dict__.pop("_train_rays_pending", None)
+        if res is not None:
+            res.check()
+
     # ------------------------------------------------------------------ a1
     def render(self, batch):
         """if_clight_renderer.py:94-122.  `cfg.chunk` rays per launch (0 = everything in one
         launch; upstream hard-codes 2048 to bound activation memory, which the fused kernel
         never materialises).  A batch without `ray_o` but with the render camera (`cam_RT`, `cam_K`, `can_bounds`) gets
-        its rays from `camera_rays`."""
-        if 'ray_o' not in batch and 'cam_RT' in batch:
+        its rays from `camera_rays`; a training batch without `ray_o` but with the image (`img`, `ray_class`) gets them from
+        `train_rays`, issued before prepare_sp_input's host synchronisation and checked after it; a test-split batch of
+        those datasets (`img` without `ray_class`) gets the whole view's rays and colours from `camera_rays`."""
+        if 'ray_o' not in batch and 'ray_class' in batch:
+            self.train_rays(batch)
+        if 'ray_o' not in batch and ('cam_RT' in batch or 'img' in batch):
             ray_o, ray_d, near, far = self.camera_rays(batch)
         else:
             ray_o = batch['ray_o']
@@ -672,6 +733,7 @@ class Renderer:
             far = batch['far']
 
         sp_input = self.prepare_sp_input(batch)
+        self.check_train_rays()   # after the .tolist() above waited for the stream: no second synchronisation
         feature_volume = self.net.encode_sparse_voxels(sp_input)
 
         n_pixel = ray_o.shape[1]
