@@ -6,7 +6,8 @@ fp16, lo = fp16(value - hi) -- and the tensor cores accumulate A_hi W_hi + A_lo 
 colour layer (latent_xyzc.py:106-121, folded as nb_layout.h describes) as ONE fp16 rounded to nearest; alpha_fc and rgb_fc are
 fp32 dot products.  This module emulates exactly those roundings around the oracle's own feature gather and compositing, on the
 full-size `full_313` golden case (the scene on which the 1-pass mode misses the gate), and pins the two facts the kernel's
-precision scheme rests on:
+precision scheme rests on (the emulation itself lives in oracle/tc_decoder_model.py, which tests/test_decoder_rows_gpu.py
+also holds the kernel to row by row):
 
   * the 3-pass scheme with a 1-pass colour layer stays well inside the north star's 1e-3 gate on every map;
   * one fp16 rounding per density-path operand (the 1-pass `tc_fp16` mode) does NOT: its depth error is several times larger,
@@ -19,75 +20,17 @@ import torch
 
 from conftest import golden_case
 from oracle import neuralbody_oracle as O
-
-
-def _f16_rn(x):
-    return x.to(torch.float16).to(torch.float32)
-
-
-def _f16_rz(x):
-    """fp32 -> fp16 truncation (cvt.rz): for values in fp16's normal range the fp32 bit pattern with 13 mantissa bits cleared."""
-    bits = x.contiguous().view(torch.int32) & torch.tensor(-8192, dtype=torch.int32)      # 0xFFFFE000
-    return bits.view(torch.float32)
-
-
-def _split(x):
-    hi = _f16_rz(x)
-    return hi, _f16_rn(x - hi)
-
-
-def _mm(a, w):
-    """(P,K) x (N,K)^T with an accumulator at least as wide as the tensor core's fp32."""
-    return (a.double() @ w.double().t()).float()
-
-
-def _layer(a, w, b, passes):
-    """relu-less dense layer with the decoder's operand roundings: 3 = (hi, lo) pairs without the lo x lo term, 1 = fp16 only."""
-    if passes == 3:
-        a_hi, a_lo = _split(a)
-        w_hi, w_lo = _f16_rn(w), None
-        w_lo = _f16_rn(w - w_hi)
-        b_hi = _f16_rn(b)
-        b_lo = _f16_rn(b - b_hi)
-        return _mm(a_hi, w_hi) + _mm(a_lo, w_hi) + _mm(a_hi, w_lo) + (b_hi + b_lo)
-    return _mm(_f16_rn(a), _f16_rn(w)) + _f16_rn(b)
-
-
-def _folded_colour_layer(w, latent_index):
-    """nb_layout.h: view_fc[:, :256] o latent_fc o (feature_fc (+) latent[idx]) -> Wc (128 x 256), bc (128), exactly, in fp64."""
-    d = {k: v.double() for k, v in w.items()}
-    Wv = d["view_fc.weight"][:, :, 0]
-    Lf = d["latent_fc.weight"][:, :, 0]
-    Ff = d["feature_fc.weight"][:, :, 0]
-    Wv_h = Wv[:, :256]
-    T = Wv_h @ Lf[:, :256]
-    Wc = T @ Ff
-    lat = d["latent.weight"][latent_index].reshape(-1)
-    bc = T @ d["feature_fc.bias"] + Wv_h @ (Lf[:, 256:] @ lat + d["latent_fc.bias"]) + d["view_fc.bias"]
-    return Wc.float(), Wv[:, 256:].float(), bc.float()     # Wv[:, 256:] multiplies [PE(view) 27 | PE(xyz) 63] (latent_xyzc.py:117-119)
+from oracle import tc_decoder_model as M
 
 
 def _decode(scene, wpts, viewdir, density_passes):
-    """(P,3) world points / view directions of ONE frame -> raw (P,4) with the decoder's roundings."""
-    w = scene["weights"]
+    """(P,3) world points / view directions of ONE frame -> raw (P,4) with the decoder's roundings, on the oracle's gather."""
     sp = O.prepare_sp_input(scene)
     ppts = O.pts_to_can_pts(wpts[None], sp["R"], sp["Th"])
     grid = O.get_grid_coords(ppts, sp["bounds"], sp["out_sh"], scene["voxel_size"])
     f = O.interpolate_features(grid, scene["volumes"])[0].t().contiguous()            # (P,352) fp32, as the producers gather it
-    h = f
-    for name in ("fc_0", "fc_1", "fc_2"):
-        h = torch.relu(_layer(h, w[name + ".weight"][:, :, 0], w[name + ".bias"], density_passes))
-    sigma = (h.double() @ w["alpha_fc.weight"][0, :, 0].double() + w["alpha_fc.bias"].double()).float()   # fp32 dot product in the epilogue
-    Wc, Wpe, bc = _folded_colour_layer(w, int(scene["latent_index"].reshape(-1)[0]))
     pe = torch.cat([O.positional_embed(viewdir, 4), O.positional_embed(wpts, 10)], -1)  # order of latent_xyzc.py:117-119
-    if density_passes == 3:
-        bc_hi = _f16_rn(bc)
-        bias = bc_hi + _f16_rn(bc - bc_hi)                                              # [1 | 1] x [hi(bc) | lo(bc)]
-    else:
-        bias = _f16_rn(bc)
-    col = torch.relu(_mm(_f16_rn(h), _f16_rn(Wc)) + _mm(_f16_rn(pe), _f16_rn(Wpe)) + bias)   # 1-pass layer, h2 rounded to nearest
-    rgb = (col.double() @ w["rgb_fc.weight"][:, :, 0].double().t() + w["rgb_fc.bias"].double()).float()
-    return torch.cat([rgb, sigma[:, None]], -1)
+    return M.decode_rows(scene["weights"], int(scene["latent_index"].reshape(-1)[0]), f, pe=pe, passes=density_passes)
 
 
 def _render(scene, n_samples, density_passes):
@@ -109,7 +52,7 @@ def test_split_is_exact_and_13_bits_survive():
     """hi + lo reproduces an fp32 value to ~2^-22 relative (hi keeps 11 bits by truncation, lo the next 11)."""
     g = torch.Generator().manual_seed(5)
     x = (torch.rand(4096, generator=g) * 8 - 4)
-    hi, lo = _split(x)
+    hi, lo = M.split_act(x)
     assert torch.equal(hi, hi.to(torch.float16).to(torch.float32))                     # hi is representable in fp16
     assert float((hi.abs() <= x.abs()).float().min()) == 1.0                           # truncation, not rounding
     rel = ((hi + lo - x).abs() / x.abs().clamp_min(1e-3)).max()
