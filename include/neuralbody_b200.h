@@ -394,6 +394,44 @@ typedef struct nb_train_rays_args {
 size_t nb_train_rays_workspace_bytes(int B, int H, int W);   /* 0 for an invalid size */
 int nb_train_rays(const nb_train_rays_args* a, void* stream);
 
+/* The training datasets' image steps after decoding (multi_view_dataset.py:121-145, monocular_dataset.py:74-103 upstream)
+ * on the device, for B items of one size, bit for bit with OpenCV's:
+ *   - cv2.undistort(img_u8 / 255 as float32, K, D) and cv2.undistort(msk_u8, K, D): the map of initUndistortRectifyMap in
+ *     float64 (stripes of max(1, 4096 / W0) rows, each with its own inverse of the camera matrix; the per-column sums along
+ *     each row), rounded to 1/32 px, then the bilinear remap with BORDER_CONSTANT 0 (float weights for the image, 15-bit
+ *     fixed-point ones for the mask);
+ *   - the resize to (H, W): a copy, or an exact 2x reduction (INTER_AREA's fast path for the image: the 2x2 cell summed
+ *     row-major, times 0.25f; INTER_NEAREST for the mask: source pixel (2y, 2x));
+ *   - the background: where the processed mask is 0, the image is 0 (NB_ITEM_BKGD_BLACK) or 1 (NB_ITEM_BKGD_WHITE);
+ *   - optionally the sampler's class map (NB_TRAIN_CLASS_* bits) from the processed mask m and the bound mask bm,
+ *     with mb = (uint8)(m * bm): NB_ITEM_CLASS_H36M (sample_ray_h36m): body mb == 1, face mb == 13, bound bm == 1 and
+ *     mb != 100; NB_ITEM_CLASS_SNAPSHOT (sample_ray): body mb != 0, face mb == 13, bound bm == 1.
+ * Validation (null pointers, sizes, the geometry, n_dist, the enums) happens before anything is enqueued; one launch; no
+ * workspace; nothing synchronises with the host. */
+#define NB_ITEM_CAM_DOUBLES 17         /* per item: K[9] row-major | k1 k2 p1 p2 k3 k4 k5 k6 (the first n_dist are read) */
+#define NB_ITEM_MAX_W 4096
+#define NB_ITEM_BKGD_NONE 0
+#define NB_ITEM_BKGD_BLACK 1
+#define NB_ITEM_BKGD_WHITE 2
+#define NB_ITEM_CLASS_NONE 0
+#define NB_ITEM_CLASS_H36M 1
+#define NB_ITEM_CLASS_SNAPSHOT 2
+typedef struct nb_item_images_args {
+    int B, H0, W0;                   /* the decoded source size, W0 <= NB_ITEM_MAX_W */
+    int H, W;                        /* the output size: (H0, W0), or exactly (H0 / 2, W0 / 2) */
+    int n_dist;                      /* the distortion model's coefficient count: 4, 5 or 8 */
+    int bkgd;                        /* NB_ITEM_BKGD_* */
+    int class_rule;                  /* NB_ITEM_CLASS_* */
+    const unsigned char* img_u8;     /* device (B,H0,W0,3) */
+    const unsigned char* msk_u8;     /* device (B,H0,W0) */
+    const double* cams;              /* device (B, NB_ITEM_CAM_DOUBLES): K and D at the source size, as float64 */
+    const unsigned char* bound;      /* device (B,H,W) bound mask with a class rule, else NULL */
+    float* img;                      /* device (B,H,W,3) */
+    unsigned char* msk;              /* device (B,H,W) */
+    unsigned char* class_map;        /* device (B,H,W) with a class rule, else NULL */
+} nb_item_images_args;
+int nb_item_images(const nb_item_images_args* a, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

@@ -19,7 +19,7 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
-           "nb_train_rays_workspace_bytes", "nb_train_rays"]
+           "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images"]
 
 
 class nb_volume_level(C.Structure):
@@ -92,6 +92,19 @@ class nb_train_rays_args(C.Structure):
                 ("key", C.c_ulonglong * 2), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
                 ("ray_o", C.c_void_p), ("ray_d", C.c_void_p), ("near", C.c_void_p), ("far", C.c_void_p), ("rgb", C.c_void_p),
                 ("coord", C.c_void_p), ("rounds", C.c_void_p), ("status", C.c_void_p)]
+
+
+NB_ITEM_CAM_DOUBLES = 17
+NB_ITEM_MAX_W = 4096
+NB_ITEM_BKGD_NONE, NB_ITEM_BKGD_BLACK, NB_ITEM_BKGD_WHITE = 0, 1, 2
+NB_ITEM_CLASS_NONE, NB_ITEM_CLASS_H36M, NB_ITEM_CLASS_SNAPSHOT = 0, 1, 2
+
+
+class nb_item_images_args(C.Structure):
+    _fields_ = [("B", C.c_int), ("H0", C.c_int), ("W0", C.c_int), ("H", C.c_int), ("W", C.c_int), ("n_dist", C.c_int),
+                ("bkgd", C.c_int), ("class_rule", C.c_int), ("img_u8", C.c_void_p), ("msk_u8", C.c_void_p),
+                ("cams", C.c_void_p), ("bound", C.c_void_p), ("img", C.c_void_p), ("msk", C.c_void_p),
+                ("class_map", C.c_void_p)]
 
 
 class nb_image_rays_args(C.Structure):
@@ -205,6 +218,8 @@ def load(path=None):
     lib.nb_train_rays_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.nb_train_rays.restype = C.c_int
     lib.nb_train_rays.argtypes = [C.POINTER(nb_train_rays_args), C.c_void_p]
+    lib.nb_item_images.restype = C.c_int
+    lib.nb_item_images.argtypes = [C.POINTER(nb_item_images_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

@@ -107,6 +107,9 @@ def _defaults():
     c.mask_bkgd = True                  # the training datasets' background (config.py:31)
     c.body_sample_ratio = 0.5           # sample_ray's class split (config.py:128-129)
     c.face_sample_ratio = 0.
+    c.dataset_image_steps = 'host'      # the training datasets' undistort / resize / background: 'host' (upstream's cv2
+                                        # steps in the item) | 'device' (the item ships the decoded image and mask;
+                                        # nb_item_images runs the steps on the GPU, bit for bit)
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path

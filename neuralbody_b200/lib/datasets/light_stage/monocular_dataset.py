@@ -11,6 +11,9 @@ carries in place of the six ray keys the processed image `img` (H,W,3) float32, 
 other key is upstream's, including `msk`, `K` and `RT`.  neuralbody_b200's renderers sample the rays on the GPU
 (Renderer.train_rays).  Split 'test' carries the image and camera without the class map, and Renderer.camera_rays builds
 the view's rays and colours on the GPU (nb_image_rays_f64 with the float32-K kind).
+With `dataset_image_steps: 'device'` the item stops after decoding: it carries the decoded uint8 image and mask, K and D
+(train_item.device_fields) in place of the processed image and class map, and the renderer runs the undistort, resize,
+background and class map on the GPU (Renderer.item_images, nb_item_images).
 
 `make_dataset_class(base)` builds the subclass over any base with the reference's attributes (`data_root`, `split`, `cam`,
 `params`, `nrays`, `prepare_input`); `Dataset` is the one over the reference's own Dataset, resolved on first use.  OpenCV
@@ -38,13 +41,14 @@ def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
             cfg = get_active_cfg()
             cv = cv2 if cv2 is not None else _cv2()
             read = imread if imread is not None else _imread
+            if train_item.image_steps(cfg) == 'device':
+                return self._device_item(index, cfg, cv, read)
             # monocular_dataset.py:74-104
             img_path = os.path.join(self.data_root, 'image', '{}.jpg'.format(index))
             img = read(img_path).astype(np.float32) / 255.
             msk_path = os.path.join(self.data_root, 'mask', '{}.png'.format(index))
             msk = read(msk_path)
             frame_index = index
-            latent_index = index
             K = self.cam['K']
             D = self.cam['D']
             img = cv.undistort(img, K, D)
@@ -70,9 +74,39 @@ def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
                                                    cfg.body_sample_ratio, cfg.face_sample_ratio))
             else:
                 ret.update(train_item.test_fields(img, K, R, T, can_bounds))
+            return self._finish(ret, index, cv, Rh, Th, bounds, K, RT)
+
+        def _device_item(self, index, cfg, cv, read):
+            """`dataset_image_steps: 'device'`: the decoded image and mask and the camera in place of the processed image,
+            class map and `msk` (train_item.device_fields; Renderer.item_images writes `msk` back); the rest as the host
+            item."""
+            img_u8 = np.asarray(read(os.path.join(self.data_root, 'image', '{}.jpg'.format(index))))
+            msk_u8 = np.asarray(read(os.path.join(self.data_root, 'mask', '{}.png'.format(index))))
+            K, D = self.cam['K'], self.cam['D']
+            R = self.cam['R']
+            T = self.cam['T'][:, None]
+            RT = np.concatenate([R, T], axis=1).astype(np.float32)
+            coord, out_sh, can_bounds, bounds, Rh, Th = self.prepare_input(index)
+            H, W = int(img_u8.shape[0] * cfg.ratio), int(img_u8.shape[1] * cfg.ratio)
+            Ks = K.copy().astype(np.float32)
+            Ks[:2] = Ks[:2] * cfg.ratio
+            train = self.split == 'train'
+            bm = (bound_2d_mask or _bound_2d_mask)(can_bounds, Ks, np.concatenate([R, T], axis=1), H, W) if train else None
+            ret, meta = train_item.device_fields(img_u8, msk_u8, K, D, H, W, cfg.mask_bkgd, cfg.white_bkgd, True,
+                                                 train_item.CLASS_SNAPSHOT if train else None, bm)
+            ret.update({'coord': coord, 'out_sh': out_sh})
+            if train:
+                ret.update(train_item.camera_fields(Ks, R, T, can_bounds, self.nrays, cfg.body_sample_ratio,
+                                                    cfg.face_sample_ratio))
+            else:
+                ret.update(train_item.camera_fields(Ks, R, T, can_bounds))
+            ret['meta'].update(meta)
+            return self._finish(ret, index, cv, Rh, Th, bounds, Ks, RT)
+
+        def _finish(self, ret, index, cv, Rh, Th, bounds, K, RT):
             # :121-136
             R = cv.Rodrigues(Rh)[0].astype(np.float32)
-            ret.update({'bounds': bounds, 'R': R, 'Th': Th, 'latent_index': latent_index, 'frame_index': frame_index,
+            ret.update({'bounds': bounds, 'R': R, 'Th': Th, 'latent_index': index, 'frame_index': index,
                         'view_index': 0})
             Rh0 = self.params['pose'][index][:3]
             R0 = cv.Rodrigues(Rh0)[0].astype(np.float32)

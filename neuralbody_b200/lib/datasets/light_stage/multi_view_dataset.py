@@ -18,6 +18,9 @@ np.random.randint would raise (an empty body or bound list) the item raises the 
 evaluation views, whose upstream item carries every box-hit ray of the view and its colour) carries `img`, `train_cam`,
 `can_bounds` and `meta` without the class map; Renderer.camera_rays builds the rays, near, far, rgb and mask_at_box on
 the GPU (nb_image_rays_f64 with the image).
+With `dataset_image_steps: 'device'` the item stops after decoding: it carries the decoded uint8 image and mask, K and D
+(train_item.device_fields) in place of the processed image and class map, and the renderer runs the undistort, resize,
+background and class map on the GPU (Renderer.item_images, nb_item_images).
 
 `Dataset` subclasses the reference's own Dataset, resolved when it is first asked for; `make_dataset_class(base)` builds
 the same subclass over any base with the reference's attributes (`data_root`, `human`, `split`, `ims`, `cam_inds`,
@@ -50,6 +53,15 @@ def _bound_2d_mask(*args):
     return if_nerf_data_utils.get_bound_2d_mask(*args)
 
 
+def _frame(human, img_path):
+    """multi_view_dataset.py:159-165: (frame_index, the index prepare_input reads)."""
+    if human in ['CoreView_313', 'CoreView_315']:
+        i = int(os.path.basename(img_path).split('_')[4])
+        return i - 1, i
+    i = int(os.path.basename(img_path)[:-4])
+    return i, i
+
+
 def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
     """-> a subclass of `base` whose __getitem__ returns the image (and for split 'train' its pixel classes) in place of the
     rays.
@@ -61,6 +73,8 @@ def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
             cfg = get_active_cfg()
             cv = cv2 if cv2 is not None else _cv2()
             read = imread if imread is not None else _imread
+            if train_item.image_steps(cfg) == 'device':
+                return self._device_item(index, cfg, cv, read)
             # multi_view_dataset.py:121-152
             img_path = os.path.join(self.data_root, self.ims[index])
             img = read(img_path).astype(np.float32) / 255.
@@ -81,12 +95,7 @@ def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
                 if cfg.white_bkgd:
                     img[msk == 0] = 1
             K[:2] = K[:2] * cfg.ratio
-            if self.human in ['CoreView_313', 'CoreView_315']:
-                i = int(os.path.basename(img_path).split('_')[4])
-                frame_index = i - 1
-            else:
-                i = int(os.path.basename(img_path)[:-4])
-                frame_index = i
+            frame_index, i = _frame(self.human, img_path)
             coord, out_sh, can_bounds, bounds, Rh, Th = self.prepare_input(i)
             # what sample_ray_h36m (:154-155) reads
             ret = {'coord': coord, 'out_sh': out_sh}
@@ -96,6 +105,41 @@ def make_dataset_class(base, cv2=None, imread=None, bound_2d_mask=None):
                                                    cfg.body_sample_ratio, cfg.face_sample_ratio))
             else:
                 ret.update(train_item.test_fields(img, K, R, T, can_bounds))
+            return self._finish(ret, cfg, cv, Rh, Th, bounds, frame_index, cam_ind)
+
+        def _device_item(self, index, cfg, cv, read):
+            """`dataset_image_steps: 'device'`: the decoded image, upstream's get_mask and the camera in place of the
+            processed image and class map (train_item.device_fields); the rest as the host item."""
+            img_path = os.path.join(self.data_root, self.ims[index])
+            img_u8 = np.asarray(read(img_path))
+            if img_u8.shape[:2] != (cfg.H, cfg.W):
+                raise ValueError("the device image steps need the image at (cfg.H, cfg.W) = (%d, %d), where upstream's "
+                                 "first resize is a copy (got %s)" % (cfg.H, cfg.W, img_u8.shape[:2]))
+            msk = self.get_mask(index)
+            cam_ind = self.cam_inds[index]
+            K = np.array(self.cams['K'][cam_ind])
+            D = np.array(self.cams['D'][cam_ind])
+            R = np.array(self.cams['R'][cam_ind])
+            T = np.array(self.cams['T'][cam_ind]) / 1000.
+            H, W = int(img_u8.shape[0] * cfg.ratio), int(img_u8.shape[1] * cfg.ratio)
+            train = self.split == 'train'
+            Ks = K.copy()
+            Ks[:2] = Ks[:2] * cfg.ratio
+            frame_index, i = _frame(self.human, img_path)
+            coord, out_sh, can_bounds, bounds, Rh, Th = self.prepare_input(i)
+            bm = (bound_2d_mask or _bound_2d_mask)(can_bounds, Ks, np.concatenate([R, T], axis=1), H, W) if train else None
+            ret, meta = train_item.device_fields(img_u8, msk, K, D, H, W, cfg.mask_bkgd, cfg.white_bkgd, False,
+                                                 train_item.CLASS_H36M if train else None, bm)
+            ret.update({'coord': coord, 'out_sh': out_sh})
+            if train:
+                ret.update(train_item.camera_fields(Ks, R, T, can_bounds, self.nrays, cfg.body_sample_ratio,
+                                                    cfg.face_sample_ratio))
+            else:
+                ret.update(train_item.camera_fields(Ks, R, T, can_bounds))
+            ret['meta'].update(meta)
+            return self._finish(ret, cfg, cv, Rh, Th, bounds, frame_index, cam_ind)
+
+        def _finish(self, ret, cfg, cv, Rh, Th, bounds, frame_index, cam_ind):
             # :168-180
             R = cv.Rodrigues(Rh)[0].astype(np.float32)
             latent_index = (frame_index - cfg.begin_ith_frame) // cfg.frame_interval

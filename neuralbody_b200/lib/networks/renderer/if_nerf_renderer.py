@@ -645,7 +645,8 @@ class Renderer:
         cfg = get_active_cfg()
         keys = ('cam_RT', 'cam_K', 'can_bounds')
         meta = batch.get('meta')
-        if isinstance(meta, dict) and 'train_cam' in meta and 'img' in batch:   # the training datasets' test split
+        if isinstance(meta, dict) and 'train_cam' in meta and ('img' in batch or 'img_u8' in batch):   # the training
+            # datasets' test split
             return self._dataset_view_rays(batch, meta)
         src = meta if isinstance(meta, dict) and all(k in meta for k in keys) else batch
         if any(src[k].shape[0] != 1 for k in keys):
@@ -664,6 +665,8 @@ class Renderer:
         (1,H,W,3) and meta['train_cam'] / ['train_k_kind'] -> upstream's sample_ray(_h36m) test-split rays, bit for bit
         (rays.dataset_image_rays); also sets batch['rgb'] (1,n,3) and batch['mask_at_box'] (1,H*W) on the device."""
         from neuralbody_b200 import rays
+        if 'img' not in batch:
+            self.item_images(batch)
         img = batch['img']
         if img.shape[0] != 1:
             raise ValueError("a test-split batch renders one view (batch size 1, as upstream's test loader)")
@@ -689,6 +692,8 @@ class Renderer:
         calls this first and then edits the rays; they are constants, as upstream's are."""
         from neuralbody_b200 import rays
         meta = batch['meta']
+        if 'ray_class' not in batch:
+            self.item_images(batch)
         img, cmap = batch['img'], batch['ray_class']
         if img.device.type != "cuda":
             dev = torch.device("cuda", torch.cuda.current_device())
@@ -707,6 +712,38 @@ class Renderer:
         self._train_rays_pending = res
         return res
 
+    def item_images(self, batch):
+        """The image steps of a batch from the training datasets' `dataset_image_steps: 'device'` items (`img_u8`
+        (B,H0,W0,3), `msk_u8` (B,H0,W0) uint8, split 'train' also `bound_mask` (B,H,W), and in batch['meta'] on the host
+        `image_cam`, `image_n_dist`, `image_size`, `image_bkgd`, `image_class`, `image_msk`): undistort, resize, background
+        and class map on the device (neuralbody_b200.images.item_images, bit for bit with the host item's cv2 steps).  Writes
+        `img` (B,H,W,3) float32, for split 'train' `ray_class` (B,H,W) uint8, and for People-Snapshot `msk` (B,H,W) uint8
+        into the batch.  Raises ValueError when the items differ in size or steps.  Nothing synchronises with the host."""
+        from neuralbody_b200 import images
+        meta = batch['meta']
+        img_u8, msk_u8 = batch['img_u8'], batch['msk_u8']
+        dev = img_u8.device if img_u8.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+        same = {}
+        for k in ('image_n_dist', 'image_bkgd', 'image_class', 'image_msk'):
+            vals = set(torch.as_tensor(meta[k]).reshape(-1).tolist())
+            if len(vals) != 1:
+                raise ValueError("a batch's items must share %s (got %s)" % (k, sorted(vals)))
+            same[k] = int(vals.pop())
+        sizes = set(map(tuple, torch.as_tensor(meta['image_size']).reshape(-1, 2).tolist()))
+        if len(sizes) != 1:
+            raise ValueError("a batch's items must share the image size (got %s)" % sorted(sizes))
+        H, W = sizes.pop()
+        bound = batch['bound_mask'] if same['image_class'] else None
+        img, msk, cmap = images.item_images(img_u8.to(dev, non_blocking=True), msk_u8.to(dev, non_blocking=True),
+                                            torch.as_tensor(meta['image_cam']).reshape(-1, images.capi.NB_ITEM_CAM_DOUBLES).numpy(),
+                                            same['image_n_dist'], H, W, same['image_bkgd'], same['image_class'], bound)
+        batch['img'] = img
+        if cmap is not None:
+            batch['ray_class'] = cmap
+        if same['image_msk']:
+            batch['msk'] = msk
+        return batch
+
     def check_train_rays(self):
         """Raise RuntimeError when the last train_rays call failed (a view whose bound pixels' rays all miss the box, where
         upstream loops forever)."""
@@ -719,12 +756,13 @@ class Renderer:
         """if_clight_renderer.py:94-122.  `cfg.chunk` rays per launch (0 = everything in one
         launch; upstream hard-codes 2048 to bound activation memory, which the fused kernel
         never materialises).  A batch without `ray_o` but with the render camera (`cam_RT`, `cam_K`, `can_bounds`) gets
-        its rays from `camera_rays`; a training batch without `ray_o` but with the image (`img`, `ray_class`) gets them from
-        `train_rays`, issued before prepare_sp_input's host synchronisation and checked after it; a test-split batch of
-        those datasets (`img` without `ray_class`) gets the whole view's rays and colours from `camera_rays`."""
-        if 'ray_o' not in batch and 'ray_class' in batch:
+        its rays from `camera_rays`; a training batch without `ray_o` but with the image (`img`, `ray_class`, or the
+        decoded `img_u8` with `bound_mask`, which `item_images` processes first) gets them from `train_rays`, issued before
+        prepare_sp_input's host synchronisation and checked after it; a test-split batch of those datasets (`img` or
+        `img_u8` without a class map) gets the whole view's rays and colours from `camera_rays`."""
+        if 'ray_o' not in batch and ('ray_class' in batch or 'bound_mask' in batch):
             self.train_rays(batch)
-        if 'ray_o' not in batch and ('cam_RT' in batch or 'img' in batch):
+        if 'ray_o' not in batch and ('cam_RT' in batch or 'img' in batch or 'img_u8' in batch):
             ray_o, ray_d, near, far = self.camera_rays(batch)
         else:
             ray_o = batch['ray_o']

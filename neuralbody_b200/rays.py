@@ -197,6 +197,11 @@ _STATUS = {capi.NB_TRAIN_RAYS_ROUNDS: "no N_rand rays after %d sampling rounds: 
            capi.NB_TRAIN_RAYS_REPLAY: "the replayed draws do not fit the pixel lists"}
 
 
+class EmptyClassError(RuntimeError, ValueError):
+    """A failed nb_train_rays item whose round drew from an empty class list: where upstream's item raises ValueError
+    (np.random.randint), so it is a ValueError as well as the RuntimeError of any failed call."""
+
+
 class TrainRays:
     """The device outputs of one nb_train_rays call, (B, n_rays, ...) each, and its per-item status.  The status comes to
     pinned host memory with the stream's work; `check()` waits for it (free once something has synchronised the stream past
@@ -213,7 +218,7 @@ class TrainRays:
         self._event.synchronize()
         for b, s in enumerate(self._status_host.tolist()):
             if s != capi.NB_TRAIN_RAYS_OK:
-                raise RuntimeError("nb_train_rays: batch item %d: %s" % (b, _STATUS.get(s, "status %d" % s)))
+                raise (EmptyClassError if s == capi.NB_TRAIN_RAYS_EMPTY else RuntimeError)("nb_train_rays: batch item %d: %s" % (b, _STATUS.get(s, "status %d" % s)))
         return self
 
 

@@ -10,7 +10,10 @@ People-Snapshot-like one (1080 x 1080 at ratio 1.0, float32 K).  Per view it pri
   - drop-in: the class map, the empty-list check and the camera the drop-in item computes in its place;
   - the rays.train_rays call (CUDA events around the whole call: camera upload, workspace, the three scans, the list
     scatter, the sampler, the status copy) and the host-to-device copy of the item's image and class map;
-with the card's name and power limit.  One JSON line per view.
+with the card's name and power limit.  One JSON line per view.  Then (`item_steps`) per raw view (313-like 1024 x 1024 at
+ratio 0.5, Snapshot-like 1080 x 1080 at ratio 1, with distortion) the host ms of decoding, of the rest of a 'host' item
+(upstream's undistort, resize, background, class map, camera) and of the rest of a 'device' item, and the nb_item_images
+call (CUDA events), with the host CPU count.
 
 Then the loader (`loader_steps`): seeded synthetic data roots of the same two kinds around the synthetic body of
 tools/mesh_mono_case (313-like: four 1024 x 1024 views, ratio 0.5, float64 K; Snapshot-like: one 1080 x 1080 view, ratio
@@ -19,7 +22,9 @@ upstream's image steps (decode, undistort, INTER_AREA / INTER_NEAREST resize, ba
 sampler on the host (`upstream_sample`, the item carries the rays) or the drop-in's fields (`train_item.train_fields`, the
 GPU samples them).  A torch DataLoader at the configs' worker counts (8 for 313, 16 for Snapshot), batch size 1, pinned,
 feeds a c3-like step: Renderer.render (64 + 128 samples, training precision), the trainer's mse loss, backward, Adam.
-Upstream and drop-in loaders alternate in one process (A B A B); each reports steps/s over `--steps` steps after 8 warm-up
+A third item kind, `device` (`dataset_image_steps: 'device'`), stops after decoding and the mask's border and ships the
+decoded image and mask; Renderer.render runs nb_item_images on it.  The three loaders alternate in one process (A B C A B
+C); each reports steps/s over `--steps` steps after 8 warm-up
 steps (one JSON line per view kind, item kind and repeat).  `step_alone` lines time the same step on one item of each kind
 made ahead and kept in pinned memory: the rate the loader has to keep up with."""
 import json
@@ -118,12 +123,39 @@ class SynthTrainData:
         R, T = np.eye(3), np.zeros((3, 1))
         cb = self.scene_item["can_bounds"]
         ret = {k: v for k, v in self.scene_item.items() if k != "can_bounds"}
+        if self.mode == "device":
+            return self._device_item(img_path, msk_path)
         if self.mode == "upstream":
             rgb, ray_o, ray_d, near, far = TC.upstream_sample(img, cmap, K, R, T, cb, self.n_rand, 0.5, 0.0)
             ret.update({"rgb": rgb, "ray_o": ray_o, "ray_d": ray_d, "near": near, "far": far,
                         "mask_at_box": np.ones(len(near), bool)})
         else:
             ret.update(train_item.train_fields(img, cmap, K, R, T, cb, self.n_rand, 0.5, 0.0))
+        return ret
+
+    def _device_item(self, img_path, msk_path):
+        """`dataset_image_steps: 'device'`: decode and the mask's border on the host, the rest on the GPU."""
+        import cv2
+        img_u8 = cv2.imread(img_path)
+        msk = (cv2.imread(msk_path, cv2.IMREAD_GRAYSCALE) != 0).astype(np.uint8)
+        if self.h36m:
+            k = np.ones((5, 5), np.uint8)
+            msk[(cv2.dilate(msk.copy(), k) - cv2.erode(msk.copy(), k)) == 1] = 100
+        H, W = int(img_u8.shape[0] * self.ratio), int(img_u8.shape[1] * self.ratio)
+        s = img_u8.shape[0] // H
+        ys, xs = np.nonzero(msk[::s, ::s])
+        bound = np.zeros((H, W), np.uint8)          # stands in for get_bound_2d_mask
+        bound[max(ys.min() - 20, 0):ys.max() + 21, max(xs.min() - 20, 0):xs.max() + 21] = 1
+        K = self.K.copy()
+        Ks = K.copy()
+        Ks[:2] = Ks[:2] * self.ratio
+        ret = {k: v for k, v in self.scene_item.items() if k != "can_bounds"}
+        fields, meta = train_item.device_fields(img_u8, msk, K, np.zeros(5), H, W, True, False, False,
+                                                train_item.CLASS_H36M if self.h36m else train_item.CLASS_SNAPSHOT, bound)
+        ret.update(fields)
+        ret.update(train_item.camera_fields(Ks, np.eye(3), np.zeros((3, 1)), self.scene_item["can_bounds"], self.n_rand,
+                                            0.5, 0.0))
+        ret["meta"].update(meta)
         return ret
 
 
@@ -169,7 +201,7 @@ def loader_steps(reps, steps):
 
         for kind, paths, K, ratio, workers in views:
             # the step alone, on one pinned item of each kind made ahead: what the loader has to keep up with
-            for mode in ("upstream", "dropin"):
+            for mode in ("upstream", "dropin", "device"):
                 ds = SynthTrainData(paths, K, ratio, kind == "313", scene_item, mode)
                 one = torch.utils.data.default_collate([ds[0]])
                 one = {k: (v if k == "meta" else v.pin_memory()) for k, v in one.items()}
@@ -184,7 +216,7 @@ def loader_steps(reps, steps):
                 print(json.dumps({"step_alone": kind, "items": mode, "steps": steps, "ms_per_step": round(dt * 1e3 / steps, 2),
                                   "card": card()}), flush=True)
             for rep in range(reps):
-                for mode in ("upstream", "dropin"):
+                for mode in ("upstream", "dropin", "device"):
                     ds = SynthTrainData(paths, K, ratio, kind == "313", scene_item, mode, length=steps + 8)
                     loader = torch.utils.data.DataLoader(ds, batch_size=1, shuffle=True, num_workers=workers,
                                                          pin_memory=True)
@@ -200,6 +232,67 @@ def loader_steps(reps, steps):
                                       "steps": len(ds) - 8, "steps_per_s": round((len(ds) - 8) / dt, 2),
                                       "ms_per_step": round(dt * 1e3 / (len(ds) - 8), 2), "card": card()}), flush=True)
                     del loader
+
+
+def item_steps(kind, raw, ratio, d, reps, gpu):
+    """One raw view's host ms split into decode (cv2.imread of the image and mask) and the rest: upstream's image steps
+    with the drop-in's fields ('host' items), or the 'device' item's fields; and the nb_item_images call (CUDA events)."""
+    import cv2
+    rng = np.random.RandomState(1)
+    f = 1.1 * raw
+    K = np.array([[f, 0, raw / 2 + 3.1], [0, f, raw / 2 - 2.3], [0, 0, 1.]])
+    D = np.array([-0.3, 0.1, 0.001, -0.001, 0.0])
+    ip, mp = os.path.join(d, "raw_%s.png" % kind), os.path.join(d, "raw_%s_m.png" % kind)
+    yy, xx = np.mgrid[0:raw, 0:raw]
+    msk = ((((xx - raw / 2) / (0.18 * raw)) ** 2 + ((yy - raw / 2) / (0.42 * raw)) ** 2) < 1).astype(np.uint8)
+    cv2.imwrite(ip, (rng.rand(raw, raw, 3) * 255).astype(np.uint8))
+    cv2.imwrite(mp, msk)
+    H = W = int(raw * ratio)
+    bound = np.ones((H, W), np.uint8)
+    h36m = kind == "313"
+    cls = train_item.class_map_h36m if h36m else train_item.class_map_snapshot
+    Ks = K.copy()
+    Ks[:2] *= ratio
+    R, T, cb = np.eye(3), np.array([[0.], [0.], [3.]]), np.array([[-1, -1, 2], [1, 1, 4]], np.float32)
+    decode = med(lambda: (cv2.imread(ip), cv2.imread(mp, cv2.IMREAD_GRAYSCALE)), reps)
+    img_u8, msk_u8 = cv2.imread(ip), cv2.imread(mp, cv2.IMREAD_GRAYSCALE)
+
+    def host():
+        img = cv2.undistort(img_u8.astype(np.float32) / 255., K, D)
+        m = cv2.undistort(msk_u8, K, D)
+        img = cv2.resize(img, (W, H), interpolation=cv2.INTER_AREA)
+        m = cv2.resize(m, (W, H), interpolation=cv2.INTER_NEAREST)
+        img[m == 0] = 0
+        return train_item.train_fields(img, cls(m, bound), Ks, R, T, cb, 1024, 0.5, 0.0)
+
+    def device():
+        fields, meta = train_item.device_fields(img_u8, msk_u8, K, D, H, W, True, False, not h36m,
+                                                train_item.CLASS_H36M if h36m else train_item.CLASS_SNAPSHOT, bound)
+        return fields, meta, train_item.camera_fields(Ks, R, T, cb, 1024, 0.5, 0.0)
+    rec = {"item_steps": kind, "raw": raw, "ratio": ratio, "decode_ms": round(decode, 2),
+           "host_rest_ms": round(med(host, reps), 2), "device_item_rest_ms": round(med(device, reps), 2),
+           "cpus": os.cpu_count(), "card": card()}
+    if gpu:
+        import torch
+        from neuralbody_b200 import images
+        dev = torch.device("cuda:0")
+        n_dist, cam = images.item_camera(K, D)
+        gi = torch.from_numpy(img_u8[None].copy()).to(dev)
+        gm = torch.from_numpy(msk_u8[None].copy()).to(dev)
+        gb = torch.from_numpy(bound[None].copy()).to(dev)
+        rule = images.capi.NB_ITEM_CLASS_H36M if h36m else images.capi.NB_ITEM_CLASS_SNAPSHOT
+        call = lambda: images.item_images(gi, gm, cam[None], n_dist, H, W, 1, rule, gb)
+        call()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ts = []
+        for _ in range(reps):
+            e0.record()
+            call()
+            e1.record()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        rec["item_images_call_ms"] = round(float(np.median(ts)), 3)
+    return rec
 
 
 def main():
@@ -247,6 +340,8 @@ def main():
                     ts.append(e0.elapsed_time(e1))
                 rec["train_rays_call_ms"] = round(float(np.median(ts)), 3)
             print(json.dumps(rec), flush=True)
+        for kind, raw, ratio in (("313", 1024, 0.5), ("snapshot", 1080, 1.0)):
+            print(json.dumps(item_steps(kind, raw, ratio, d, a.reps, gpu)), flush=True)
     if gpu and not a.no_loader:
         loader_steps(2, a.steps)
 
