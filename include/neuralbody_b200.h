@@ -432,6 +432,52 @@ typedef struct nb_item_images_args {
 } nb_item_images_args;
 int nb_item_images(const nb_item_images_args* a, void* stream);
 
+/* The evaluator's per-view metrics (lib/evaluators/if_nerf.py upstream) on the device, from the rendered rays, the
+ * test split's colours and mask_at_box:
+ *   - scatter: ray k is the k-th set pixel of mask_at_box in row-major order (img[mask_at_box] = rgb); every other pixel
+ *     is white_bkgd (0 or 1).  n must equal the mask's count, else status NB_EVAL_COUNT (upstream's numpy raises);
+ *   - box: cv2.boundingRect of the mask (x, y, w, h; (0,0,0,0) for an empty mask), or the whole image with eval_whole_img;
+ *   - mse: eval_whole_img 0: the mean over the n x 3 ray values of fp32(fp32(pred - gt)^2), the terms summed in float64;
+ *     eval_whole_img 1: the mean over the float64 H x W x 3 images.  psnr = -10 log10(mse) in float64;
+ *   - ssim: scikit-image 0.14.2's compare_ssim(X, Y, multichannel=True) over the box in float64: per channel the 7 x 7
+ *     means of x, y, xx, yy, xy, cov_norm = 49/48, C1 = (0.01 * 2)^2, C2 = (0.03 * 2)^2 (a float image's data_range is 2),
+ *     S = (2 ux uy + C1)(2 vxy + C2) / ((ux^2 + uy^2 + C1)(vx + vy + C2)), the channel value the mean of S over the box
+ *     minus its 3-pixel border (those windows lie inside the box, so the filter's edge mode never enters), the result the
+ *     mean of the three.  A box side under 7 is status NB_EVAL_SMALL (upstream's "win_size exceeds image extent");
+ *   - crops: the box of each image as uint8 BGR, row-major, saturate_cast<uchar>(v * 255) with round-half-even (what
+ *     cv2.imwrite makes of upstream's float64 img[..., [2,1,0]] * 255), at the start of crop_pred / crop_gt.
+ * Fixed-order reductions and no floating-point atomics: the same inputs give the same bits.  `result` is written on the
+ * device; the caller reads it (and the crops) back once.  Validation (null pointers, sizes, flags, workspace) happens
+ * before anything is enqueued; six launches (the mask's box partials, a CUB scan, the ray sums, the first finish, the
+ * SSIM tiles with the crops, the SSIM finish); nothing synchronises with the host. */
+#define NB_EVAL_OK 0
+#define NB_EVAL_COUNT 1                /* n != the number of set pixels of mask_at_box */
+#define NB_EVAL_SMALL 2                /* a side of the box is under 7 pixels */
+typedef struct nb_eval_image_result {
+    int status;                        /* NB_EVAL_* */
+    int count;                         /* set pixels of mask_at_box */
+    int box[4];                        /* x, y, w, h of the region the SSIM and the crops cover */
+    double sq_sum;                     /* the float64 sum of the MSE's terms */
+    double mse, psnr, ssim;            /* NaN where the status says upstream raised before reaching them */
+    double ssim_channel[3];
+} nb_eval_image_result;
+typedef struct nb_eval_image_args {
+    int n;                             /* rays, 0 <= 3n < 2^31 */
+    int H, W;                          /* the view, H*W < 2^31 */
+    int white_bkgd;                    /* 0 / 1 */
+    int eval_whole_img;                /* 0 / 1 */
+    const float* rgb_pred;             /* device (n,3) */
+    const float* rgb_gt;               /* device (n,3) */
+    const unsigned char* mask_at_box;  /* device (H*W), nonzero = set */
+    void* workspace;                   /* device scratch of nb_eval_image_workspace_bytes(H, W, n) bytes */
+    size_t workspace_bytes;
+    nb_eval_image_result* result;      /* device */
+    unsigned char* crop_pred;          /* device, room for H*W*3 */
+    unsigned char* crop_gt;            /* device, room for H*W*3 */
+} nb_eval_image_args;
+size_t nb_eval_image_workspace_bytes(int H, int W, int n);   /* 0 for an invalid size */
+int nb_eval_image(const nb_eval_image_args* a, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

@@ -19,7 +19,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
-           "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images"]
+           "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_eval_image_workspace_bytes",
+           "nb_eval_image"]
 
 
 class nb_volume_level(C.Structure):
@@ -105,6 +106,21 @@ class nb_item_images_args(C.Structure):
                 ("bkgd", C.c_int), ("class_rule", C.c_int), ("img_u8", C.c_void_p), ("msk_u8", C.c_void_p),
                 ("cams", C.c_void_p), ("bound", C.c_void_p), ("img", C.c_void_p), ("msk", C.c_void_p),
                 ("class_map", C.c_void_p)]
+
+
+NB_EVAL_OK, NB_EVAL_COUNT, NB_EVAL_SMALL = 0, 1, 2
+
+
+class nb_eval_image_result(C.Structure):
+    _fields_ = [("status", C.c_int), ("count", C.c_int), ("box", C.c_int * 4), ("sq_sum", C.c_double), ("mse", C.c_double),
+                ("psnr", C.c_double), ("ssim", C.c_double), ("ssim_channel", C.c_double * 3)]
+
+
+class nb_eval_image_args(C.Structure):
+    _fields_ = [("n", C.c_int), ("H", C.c_int), ("W", C.c_int), ("white_bkgd", C.c_int), ("eval_whole_img", C.c_int),
+                ("rgb_pred", C.c_void_p), ("rgb_gt", C.c_void_p), ("mask_at_box", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t), ("result", C.c_void_p), ("crop_pred", C.c_void_p),
+                ("crop_gt", C.c_void_p)]
 
 
 class nb_image_rays_args(C.Structure):
@@ -220,6 +236,10 @@ def load(path=None):
     lib.nb_train_rays.argtypes = [C.POINTER(nb_train_rays_args), C.c_void_p]
     lib.nb_item_images.restype = C.c_int
     lib.nb_item_images.argtypes = [C.POINTER(nb_item_images_args), C.c_void_p]
+    lib.nb_eval_image_workspace_bytes.restype = C.c_size_t
+    lib.nb_eval_image_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    lib.nb_eval_image.restype = C.c_int
+    lib.nb_eval_image.argtypes = [C.POINTER(nb_eval_image_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

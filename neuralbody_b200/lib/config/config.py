@@ -110,6 +110,11 @@ def _defaults():
     c.dataset_image_steps = 'host'      # the training datasets' undistort / resize / background: 'host' (upstream's cv2
                                         # steps in the item) | 'device' (the item ships the decoded image and mask;
                                         # nb_item_images runs the steps on the GPU, bit for bit)
+    # evaluation (config.py:111, 120 upstream; the evaluator plugin as make_evaluator.py:5-9 selects it)
+    c.evaluator_module = "neuralbody_b200.lib.evaluators.if_nerf"
+    c.evaluator_path = os.path.join(_PKG_ROOT, "lib/evaluators/if_nerf.py")
+    c.result_dir = 'data/result'
+    c.eval_whole_img = False
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
