@@ -478,6 +478,36 @@ typedef struct nb_eval_image_args {
 size_t nb_eval_image_workspace_bytes(int H, int W, int n);   /* 0 for an invalid size */
 int nb_eval_image(const nb_eval_image_args* a, void* stream);
 
+/* The demo visualizers' frame (lib/visualizers/if_nerf_demo.py and if_nerf_perform.py upstream) on the device: the uint8
+ * BGR H x W x 3 array cv2.imwrite stores for upstream's float64 image img_pred[..., [2,1,0]] * 255, where
+ * img_pred[mask_at_box] = rgb_map over a background of white_bkgd (0 or 1):
+ *   - a set pixel takes the ray at the mask's exclusive prefix count (ray k is the k-th set pixel, row-major); with n = 1
+ *     every set pixel takes ray 0 (numpy broadcasts a (1,3) value);
+ *   - each value is saturate_cast<uchar>(v * 255): the float64 product rounded half to even, NaN or outside int32 to
+ *     INT_MIN, then clamped to [0, 255].
+ * A count other than n (and n != 1) is status NB_VIS_COUNT, upstream's numpy "shape mismatch"; the frame is then not
+ * written.  Validation (null pointers, sizes, white_bkgd, a 4-byte aligned frame, workspace) happens before anything is
+ * enqueued; two launches (a CUB scan of the mask, the frame with the status record); nothing synchronises with the host. */
+#define NB_VIS_OK 0
+#define NB_VIS_COUNT 1                 /* n != the number of set pixels of mask_at_box */
+typedef struct nb_vis_frame_result {
+    int status;                        /* NB_VIS_* */
+    int count;                         /* set pixels of mask_at_box */
+} nb_vis_frame_result;
+typedef struct nb_vis_frame_args {
+    int n;                             /* rays, 0 <= 3n < 2^31 */
+    int H, W;                          /* the view, H*W < 2^31 */
+    int white_bkgd;                    /* 0 / 1 */
+    const float* rgb_map;              /* device (n,3) */
+    const unsigned char* mask_at_box;  /* device (H*W), nonzero = set */
+    void* workspace;                   /* device scratch of nb_vis_frame_workspace_bytes(H, W) bytes */
+    size_t workspace_bytes;
+    nb_vis_frame_result* result;       /* device */
+    unsigned char* frame;              /* device (H,W,3) BGR, 4-byte aligned */
+} nb_vis_frame_args;
+size_t nb_vis_frame_workspace_bytes(int H, int W);   /* 0 for an invalid size */
+int nb_vis_frame(const nb_vis_frame_args* a, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

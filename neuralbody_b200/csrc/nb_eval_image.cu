@@ -10,11 +10,7 @@
 //   6. ssim_finish:   one CTA sums the tiles' S in a fixed order and writes the channel means and their mean.
 // No expression here may be contracted: every product and sum is an explicit _rn intrinsic, so pred == gt gives S = 1
 // exactly (2 ux uy and ux^2 + uy^2 round alike).  oracle/eval_metrics.py restates every output in numpy.
-#include <climits>
-
-#include <cub/device/device_scan.cuh>
-#include <thrust/iterator/transform_iterator.h>
-
+#include "nb_image_u8.cuh"
 #include "nb_internal.h"
 
 namespace nb {
@@ -26,14 +22,6 @@ constexpr int kEvalItems = 4096;         // elements per block before the cap
 constexpr int kTileX = 32, kTileY = 16;  // ssim_tiles: output pixels per CTA (32 x 8 threads, two rows each)
 constexpr int kWin = 7, kPad = 3;
 constexpr int kHaloX = kTileX + kWin - 1, kHaloY = kTileY + kWin - 1;
-
-struct NonZero {
-    __host__ __device__ int operator()(unsigned char m) const { return m != 0; }
-};
-
-inline cudaError_t scan_mask(void* scratch, size_t& bytes, const unsigned char* mask, int* offset, int n, cudaStream_t s) {
-    return cub::DeviceScan::ExclusiveSum(scratch, bytes, thrust::make_transform_iterator(mask, NonZero{}), offset, n, s);
-}
 
 inline int partial_blocks(long long items) {
     return (int)max(1LL, min((long long)kEvalMaxBlocks, (items + kEvalItems - 1) / kEvalItems));
@@ -47,12 +35,6 @@ struct Workspace {
     double2* sums;     // (kEvalMaxBlocks) fp32-term sum, float64-term sum
     double* ssim;      // (tiles, 3)
 };
-
-inline size_t scan_bytes(int n) {
-    size_t b = 0;
-    if (scan_mask(nullptr, b, nullptr, nullptr, n, 0) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return b;
-}
 
 inline int tiles(int H, int W) { return ((W + kTileX - 1) / kTileX) * ((H + kTileY - 1) / kTileY); }
 
@@ -187,13 +169,6 @@ __global__ void __launch_bounds__(kEvalThreads) finish_kernel(const __grid_const
     r->psnr = __dmul_rn(-10.0, log10(mse));
     r->ssim = nan;
     for (int c = 0; c < 3; ++c) r->ssim_channel[c] = nan;
-}
-
-// saturate_cast<uchar>(v * 255): cvRound (nearest-even; NaN or outside int32 -> INT_MIN), then clamped to [0, 255]
-__device__ __forceinline__ unsigned char to_u8(double v) {
-    const double r = rint(__dmul_rn(v, 255.0));
-    const int i = (r >= -2147483648.0 && r <= 2147483647.0) ? (int)r : INT_MIN;
-    return (unsigned char)min(max(i, 0), 255);
 }
 
 __global__ void __launch_bounds__(kEvalThreads) ssim_tiles_kernel(const __grid_constant__ nb_eval_image_args a,

@@ -115,6 +115,10 @@ def _defaults():
     c.evaluator_path = os.path.join(_PKG_ROOT, "lib/evaluators/if_nerf.py")
     c.result_dir = 'data/result'
     c.eval_whole_img = False
+    # the demo modes' visualizer plugin (make_visualizer.py:5-9; novel_view_cfg / rotate_smpl_cfg select if_nerf_demo,
+    # novel_pose_cfg if_nerf_perform)
+    c.visualizer_module = "neuralbody_b200.lib.visualizers.if_nerf_demo"
+    c.visualizer_path = os.path.join(_PKG_ROOT, "lib/visualizers/if_nerf_demo.py")
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path

@@ -15,13 +15,12 @@ Precision: the box and the PNG bytes are upstream's exactly; SSIM is upstream's 
 few float32 ulps of numpy's float32 pairwise mean; PSNR is -10 log10 of that in float64.  summarize() returns the means as
 a dict (upstream returns None, which Trainer.val cannot use)."""
 import os
-import queue
-import threading
 
 import numpy as np
 import torch
 
 from neuralbody_b200 import capi, metrics
+from neuralbody_b200.png_writer import PngWriter
 from neuralbody_b200.lib.config import get_active_cfg
 
 
@@ -33,43 +32,6 @@ def _colored(text, color):
     return colored(text, color)
 
 
-class _PngWriter:
-    """One daemon thread that writes (path, uint8 BGR array) pairs with cv2.imwrite from a small bounded queue."""
-
-    def __init__(self, depth=4):
-        self._q = queue.Queue(maxsize=depth)
-        self._error = None
-        self._thread = None
-
-    def _run(self):
-        import cv2
-        while True:
-            path, img = self._q.get()
-            try:
-                if self._error is None and not cv2.imwrite(path, img):
-                    raise IOError("cv2.imwrite could not write %s" % path)
-            except Exception as e:       # handed to the caller's thread
-                self._error = e
-            finally:
-                self._q.task_done()
-
-    def put(self, path, img):
-        self.check()
-        if self._thread is None:
-            self._thread = threading.Thread(target=self._run, name="if_nerf-png-writer", daemon=True)
-            self._thread.start()
-        self._q.put((path, img))
-
-    def join(self):
-        self._q.join()
-        self.check()
-
-    def check(self):
-        if self._error is not None:
-            e, self._error = self._error, None
-            raise e
-
-
 class Evaluator:
     def __init__(self):
         self.mse = []
@@ -78,7 +40,7 @@ class Evaluator:
         self._view = None        # metrics.ViewEval of the current view size
         self._host = None        # its pinned readback buffer
         self._index = None       # pinned (2,) int64: frame_index, cam_ind
-        self._writer = _PngWriter()
+        self._writer = PngWriter(name="if_nerf-png-writer")
 
     def _buffers(self, H, W, device):
         v = self._view
