@@ -508,6 +508,33 @@ typedef struct nb_vis_frame_args {
 size_t nb_vis_frame_workspace_bytes(int H, int W);   /* 0 for an invalid size */
 int nb_vis_frame(const nb_vis_frame_args* a, void* stream);
 
+/* The binary little-endian PLY body of a triangle mesh (nb_mcubes_emit's outputs), the bytes neuralbody_b200.mcubes.Mesh
+ * .export writes after its header "... end_header\n":
+ *   - nv vertex records of 24 bytes: the vertices array's own float64 bytes (x y z), in order;
+ *   - nf face records of 13 bytes: uchar 3, then the face's three indices as little-endian int32.
+ * `out` holds an nb_mesh_ply_result at its head and the body from NB_MESH_PLY_BODY_OFFSET on, so that one copy brings both
+ * back.  A face index < 0 or >= max(nv, 1) (the bound Mesh.export checks) is status NB_MESH_PLY_FACE; the body then holds
+ * that index's low 32 bits and must not be written out.  Nothing past NB_MESH_PLY_BODY_OFFSET + nb_mesh_ply_bytes(nv, nf)
+ * is written.  Validation (null pointers, counts, nv < 2^31, alignment, out_bytes) happens before anything is enqueued; a
+ * memset of the result record and one launch; nothing synchronises with the host. */
+#define NB_MESH_PLY_OK 0
+#define NB_MESH_PLY_FACE 1             /* a face index outside [0, max(nv, 1)) */
+#define NB_MESH_PLY_BODY_OFFSET 16
+typedef struct nb_mesh_ply_result {
+    int status;                        /* NB_MESH_PLY_* */
+    int reserved[3];
+} nb_mesh_ply_result;
+typedef struct nb_mesh_ply_args {
+    long long nv;                      /* vertices, 0 <= nv < 2^31 */
+    long long nf;                      /* faces, 0 <= nf <= 2^40 */
+    const double* vertices;            /* device (nv,3), 8-byte aligned; may be NULL when nv = 0 */
+    const long long* faces;            /* device (nf,3), 8-byte aligned; may be NULL when nf = 0 */
+    unsigned char* out;                /* device, 16-byte aligned: nb_mesh_ply_result, then the body */
+    size_t out_bytes;                  /* >= NB_MESH_PLY_BODY_OFFSET + nb_mesh_ply_bytes(nv, nf) */
+} nb_mesh_ply_args;
+size_t nb_mesh_ply_bytes(long long nv, long long nf);   /* 24 nv + 13 nf; 0 for invalid counts (and for an empty mesh) */
+int nb_mesh_ply(const nb_mesh_ply_args* a, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

@@ -20,7 +20,7 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
            "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_eval_image_workspace_bytes",
-           "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame"]
+           "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame", "nb_mesh_ply_bytes", "nb_mesh_ply"]
 
 
 class nb_volume_level(C.Structure):
@@ -134,6 +134,19 @@ class nb_vis_frame_args(C.Structure):
     _fields_ = [("n", C.c_int), ("H", C.c_int), ("W", C.c_int), ("white_bkgd", C.c_int), ("rgb_map", C.c_void_p),
                 ("mask_at_box", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
                 ("result", C.c_void_p), ("frame", C.c_void_p)]
+
+
+NB_MESH_PLY_OK, NB_MESH_PLY_FACE = 0, 1
+NB_MESH_PLY_BODY_OFFSET = 16
+
+
+class nb_mesh_ply_result(C.Structure):
+    _fields_ = [("status", C.c_int), ("reserved", C.c_int * 3)]
+
+
+class nb_mesh_ply_args(C.Structure):
+    _fields_ = [("nv", C.c_longlong), ("nf", C.c_longlong), ("vertices", C.c_void_p), ("faces", C.c_void_p),
+                ("out", C.c_void_p), ("out_bytes", C.c_size_t)]
 
 
 class nb_image_rays_args(C.Structure):
@@ -257,6 +270,10 @@ def load(path=None):
     lib.nb_vis_frame_workspace_bytes.argtypes = [C.c_int, C.c_int]
     lib.nb_vis_frame.restype = C.c_int
     lib.nb_vis_frame.argtypes = [C.POINTER(nb_vis_frame_args), C.c_void_p]
+    lib.nb_mesh_ply_bytes.restype = C.c_size_t
+    lib.nb_mesh_ply_bytes.argtypes = [C.c_longlong, C.c_longlong]
+    lib.nb_mesh_ply.restype = C.c_int
+    lib.nb_mesh_ply.argtypes = [C.POINTER(nb_mesh_ply_args), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

@@ -120,6 +120,8 @@ def _defaults():
     c.visualizer_module = "neuralbody_b200.lib.visualizers.if_nerf_demo"
     c.visualizer_path = os.path.join(_PKG_ROOT, "lib/visualizers/if_nerf_demo.py")
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
+    c.mesh_output = 'host'              # the mesh renderer's outputs: 'host' (upstream's float64 numpy cube and host mesh) |
+                                        # 'device' (the fp32 CUDA cube and a mcubes.DeviceMesh, nothing copied back)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
                                         # (meets the 1e-3 parity gate) | "tc_fp16" wgmma 1-pass (fastest, ~4e-3 on depth)

@@ -16,7 +16,14 @@ Differences to upstream: the inside points go through ONE density launch (nb_dec
 and marching cubes is this package's kernel (neuralbody_b200/mcubes.py), not PyMCubes: the same edge crossings
 interpolated the same way in double, but a watertight triangulation and grid-ordered output.  `'mesh'` is
 `trimesh.Trimesh(vertices, triangles)` when trimesh is importable (upstream's call), else neuralbody_b200.mcubes.Mesh,
-which has what lib/visualizers/if_nerf_mesh.py uses (`.vertices`, `.faces`, `.export(path)` as binary PLY)."""
+which has what lib/visualizers/if_nerf_mesh.py uses (`.vertices`, `.faces`, `.export(path)` as binary PLY).
+
+`cfg.mesh_output` (default 'host') picks where the outputs live.  'host' is upstream's contract above.  'device' leaves
+both on the GPU, so render() copies neither back: `'cube'` is the padded fp32 CUDA tensor (its values are the host cube's
+float64 values) and `'mesh'` a neuralbody_b200.mcubes.DeviceMesh, whose `.export(path)` writes the same PLY bytes and which
+this package's lib/visualizers/if_nerf_mesh.py writes off the visualize loop.  What still waits on the device is the
+inside points' selection (boolean indexing sizes its result; a mask-view batch also reads its world box) and marching
+cubes' count read."""
 import ctypes as C
 
 import numpy as np
@@ -28,6 +35,7 @@ from neuralbody_b200.lib.networks.renderer import if_nerf_renderer
 
 PAD = 10   # np.pad(cube, 10) of if_mesh_renderer.py:47
 MASK_KEYS = ('wbounds', 'RT', 'Ks', 'msks')
+MESH_OUTPUTS = ('host', 'device')
 
 
 def world_axes(wbounds, voxel_size):
@@ -87,6 +95,15 @@ def grid_inside(axes, RT, Ks, msks):
             a.RT, a.Ks = rt.data_ptr(), ks.data_ptr()
             capi.check(lib.nb_mesh_inside(C.byref(a), stream), "nb_mesh_inside")
     return inside
+
+
+def mesh_output(cfg):
+    """cfg.mesh_output, read with its default 'host' (upstream's cfg has no such key); any value but MESH_OUTPUTS is a
+    ValueError."""
+    mode = cfg.get('mesh_output', 'host')
+    if mode not in MESH_OUTPUTS:
+        raise ValueError("cfg.mesh_output must be one of %s (got %r)" % (", ".join(repr(m) for m in MESH_OUTPUTS), mode))
+    return mode
 
 
 class Renderer(if_nerf_renderer.Renderer):
@@ -150,7 +167,10 @@ class Renderer(if_nerf_renderer.Renderer):
 
     def render(self, batch):
         cfg = get_active_cfg()
+        mode = mesh_output(cfg)
         cube = self.density_cube(batch)
         verts, tris = mcubes.marching_cubes(cube, float(cfg.mesh_th))
+        if mode == 'device':
+            return {'cube': cube, 'mesh': mcubes.DeviceMesh(verts, tris)}
         mesh = mcubes.make_mesh(verts.cpu().numpy(), tris.cpu().numpy())
         return {'cube': cube.cpu().numpy().astype('float64'), 'mesh': mesh}

@@ -18,7 +18,14 @@ People-Snapshot one instead (tools/mesh_mono_case.py, the monocular mesh dataset
 1080 frame at ratio 0.5) with the dataset's float64 camera, so (a) projects the grid in float64 numpy and (b) runs
 nb_mesh_inside_f64.
 
-Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab | --from-masks [--monocular]]
+--vis measures `run.py --type visualize` with `vis_mesh True` per frame, render + visualize, alternating two paths frame by
+frame in one process: (a) `mesh_output: 'host'` and upstream's visualize body restated (`os.system('mkdir -p')`,
+`mesh.export(path)` on the loop thread); (b) `mesh_output: 'device'` and the drop-in lib/visualizers/if_nerf_mesh.py.  It
+reports the median ms per frame, each path's loop total in a loop of its own (the drop-in's final flush() included), the
+nb_mesh_ply kernel alone (CUDA events over back-to-back launches) and its bytes/s, whether (a) and (b) wrote identical
+files, and the card's name, power limit and SM clock read in the same run.  Files go to a temporary directory.
+
+Usage: python tools/bench_mesh.py [--steps 5] [--warmup 3] [--mesh-th 10] [--density-precision P | --ab | --from-masks [--monocular] | --vis]
 (upstream's default mesh_th = 50 lies above the synthetic body's sigma, p95 ~ 30, and would give an empty mesh)"""
 import argparse
 import json
@@ -40,8 +47,14 @@ PAD = 10
 
 
 def card_info(dev):
-    """Card name and power limit, read in the same run as the measurement."""
-    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    """Card name, power limit and SM clock, read in the same run as the measurement."""
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None, "sm_clock_mhz": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits", "-i",
+                              str(dev.index or 0)], capture_output=True, text=True, timeout=30).stdout.strip()
+        info["sm_clock_mhz"] = float(out.splitlines()[0])
+    except Exception:
+        pass
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -68,11 +81,16 @@ def main():
                     help="compare the host-built grid / inside (upstream's data path) with the device-built one")
     ap.add_argument("--monocular", action="store_true",
                     help="with --from-masks: the People-Snapshot frame (one view, float64 camera) instead of the 4-view one")
+    ap.add_argument("--vis", action="store_true",
+                    help="render + visualize per frame: host mode and upstream's visualize body against device mode and "
+                         "the drop-in visualizer")
     args = ap.parse_args()
     if args.monocular and not args.from_masks:
         ap.error("--monocular goes with --from-masks")
     if args.from_masks:
         return from_masks(args)
+    if args.vis:
+        return vis(args)
     arms = ("fp32", "tc_fp16x3") if args.ab else (args.density_precision,)
     if not torch.cuda.is_available():
         raise SystemExit("bench_mesh needs a CUDA device")
@@ -344,6 +362,134 @@ def from_masks(args):
         "host_cpus": os.cpu_count(), "numpy": np.__version__,
         "card": card_info(dev),
     }
+    print(json.dumps(line))
+
+
+def vis(args):
+    """--vis: arm (a) host mode + upstream's visualize body, arm (b) device mode + the drop-in visualizer; one JSON line."""
+    import contextlib
+    import ctypes as C
+    import filecmp
+    import tempfile
+    import time
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_mesh needs a CUDA device")
+    from oracle import mesh_case
+    from neuralbody_b200 import capi, mcubes
+    from neuralbody_b200.lib.config import cfg
+    from neuralbody_b200.lib.networks.make_network import make_network, load_source
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scene, _, batch = mesh_case.build_case("mesh_full")
+    cfg.num_train_frame = int(scene["weights"]["latent.weight"].shape[0])
+    cfg.voxel_size = list(scene["voxel_size"])
+    cfg.mesh_th = float(args.mesh_th)
+    cfg.density_precision = args.density_precision
+    net = make_network(cfg)
+    net.load_state_dict(scene["weights"], strict=False)
+    net = net.to(dev).eval()
+    net.set_feature_volume([v.to(dev) for v in scene["volumes"]])
+    lib_dir = os.path.join(ROOT, "neuralbody_b200", "lib")
+    ren = load_source("neuralbody_b200.lib.networks.renderer.if_mesh_renderer",
+                      os.path.join(lib_dir, "networks", "renderer", "if_mesh_renderer.py")).Renderer(net)
+    vis_mod = load_source("neuralbody_b200.lib.visualizers.if_nerf_mesh", os.path.join(lib_dir, "visualizers", "if_nerf_mesh.py"))
+    bd = {k: v.to(dev) for k, v in batch.items()}
+    tmp = tempfile.TemporaryDirectory()
+    dirs = {"a": os.path.join(tmp.name, "a"), "b": os.path.join(tmp.name, "b")}
+
+    def upstream_visualize(output, b):
+        """lib/visualizers/if_nerf_mesh.py:28-36 of the reference, restated."""
+        mesh = output['mesh']
+        result_dir = os.path.join(cfg.result_dir, 'mesh')
+        os.system('mkdir -p {}'.format(result_dir))
+        i = b['frame_index'].item()
+        mesh.export(os.path.join(result_dir, '{:04d}.ply'.format(i)))
+
+    cfg.result_dir = dirs["b"]
+    with contextlib.redirect_stdout(sys.stderr):             # its "results are saved at" line: stdout keeps the JSON
+        drop_in = vis_mod.Visualizer()
+
+    def frame(arm, i):
+        """One frame of `arm` -> host ms from the render call to visualize()'s return."""
+        b = dict(bd, frame_index=torch.tensor([i], device=dev))
+        cfg.mesh_output = "host" if arm == "a" else "device"
+        cfg.result_dir = dirs[arm]
+        t = time.perf_counter()
+        with torch.no_grad():
+            out = ren.render(b)
+        (upstream_visualize if arm == "a" else drop_in.visualize)(out, b)
+        return (time.perf_counter() - t) * 1e3
+
+    for i in range(args.warmup):
+        frame("a", i)
+        frame("b", i)
+    drop_in.flush()
+    torch.cuda.synchronize(dev)
+    rows = {"a": [], "b": []}
+    for i in range(args.steps):
+        for arm in ("a", "b"):
+            rows[arm].append(frame(arm, args.warmup + i))
+    t = time.perf_counter()
+    drop_in.flush()
+    flush_ms = (time.perf_counter() - t) * 1e3
+    names = ["%04d.ply" % i for i in range(args.steps + args.warmup)]
+    identical = all(filecmp.cmp(os.path.join(dirs["a"], "mesh", n), os.path.join(dirs["b"], "mesh", n), shallow=False)
+                    for n in names)
+    # each path's loop total in a loop of its own, the drop-in's final flush() included
+    loops = {}
+    for arm in ("a", "b"):
+        torch.cuda.synchronize(dev)
+        t = time.perf_counter()
+        for i in range(args.steps):
+            frame(arm, i)
+        if arm == "b":
+            drop_in.flush()
+        loops[arm] = (time.perf_counter() - t) * 1e3
+
+    # nb_mesh_ply alone on this frame's mesh: back-to-back launches between two CUDA events
+    cfg.mesh_output = "device"
+    with torch.no_grad():
+        mesh = ren.render(dict(bd, frame_index=torch.tensor([0], device=dev)))["mesh"]
+    out = torch.empty(capi.NB_MESH_PLY_BODY_OFFSET + mesh.body_bytes(), dtype=torch.uint8, device=dev)
+    a = capi.nb_mesh_ply_args()
+    a.nv, a.nf, a.vertices, a.faces = mesh.nv, mesh.nf, mesh.vertices.data_ptr(), mesh.faces.data_ptr()
+    a.out, a.out_bytes = out.data_ptr(), out.numel()
+    lib, stream = capi.load(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    launches = 200
+    for _ in range(20):
+        capi.check(lib.nb_mesh_ply(C.byref(a), stream), "nb_mesh_ply")
+    kernel_ms = []
+    for _ in range(5):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(launches):
+            lib.nb_mesh_ply(C.byref(a), stream)
+        e1.record()
+        torch.cuda.synchronize(dev)
+        kernel_ms.append(e0.elapsed_time(e1) / launches)
+    k_ms = float(np.median(kernel_ms))
+    moved = 24 * mesh.nv + 24 * mesh.nf + mesh.body_bytes()      # vertices and faces read once, the body written once
+    med = {arm: float(np.median(r)) for arm, r in rows.items()}
+    line = {
+        "metric": "mesh_vis_frame_ms", "value": med["b"], "unit": "ms", "higher_is_better": False,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "data": "synthetic",
+        "config": {"workload": "run.py --type visualize with vis_mesh True on the full-size synth-313 frame: render (5 mm "
+                               "world grid %s, density %s, marching cubes at mesh_th = %g) + visualize, one PLY per frame"
+                               % (tuple(batch["inside"].shape[1:]), args.density_precision, cfg.mesh_th),
+                   "a": "mesh_output 'host' + upstream's visualize body (os.system mkdir -p, mesh.export on the loop)",
+                   "b": "mesh_output 'device' + lib/visualizers/if_nerf_mesh.py (nb_mesh_ply, pinned copy, writer thread)"},
+        "vertices": mesh.nv, "triangles": mesh.nf, "ply_bytes": len(mcubes.ply_header(mesh.nv, mesh.nf)) + mesh.body_bytes(),
+        "frame_ms_median": med, "frame_ms_all": rows, "speedup_frame": med["a"] / med["b"],
+        "b_final_flush_ms": flush_ms,
+        "loop_total_ms": {"a": loops["a"], "b_incl_flush": loops["b"], "frames": args.steps},
+        "files_identical": bool(identical), "files_compared": len(names),
+        "nb_mesh_ply_kernel": {"ms_median": k_ms, "ms_all": kernel_ms, "launches_per_sample": launches,
+                               "bytes_moved": moved, "tbs": moved / (k_ms * 1e-3) / 1e12,
+                               "fraction_of_hbm_datasheet": moved / (k_ms * 1e-3) / 1e12 / HBM_TBS_DATASHEET},
+        "host_cpus": os.cpu_count(),
+        "card": card_info(dev),
+    }
+    tmp.cleanup()
     print(json.dumps(line))
 
 
