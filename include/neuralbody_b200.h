@@ -635,6 +635,19 @@ int    nb_render_bwd_inputs(const nb_render_bwd_args* args, const float* d_disp_
  * splits > 1 splits the reduction over CTAs and ACCUMULATES into c (zero it first).  bias (N) / mask (M,N) may be NULL. */
 int nb_debug_gemm_tf32x3(const float* a, const float* b, float* c, int M, int N, int K, int a_k_contiguous, int b_k_contiguous,
                          int splits, const float* bias, int relu, const float* mask, void* stream);
+/* The render's compositing (raw2outputs) in isolation, on caller-made raw records instead of the decoder's.  The ray fields
+ * of `a` are read and validated as nb_render_fwd reads them (batch, n_rays, n_samples <= 1024, ray_o, ray_d, near, far, t_vals,
+ * t_rand, z_vals, white_bkgd, the four maps, weights, out_ray_stride); no frame field is read.  raw: device (B,n,S,4) (rgb
+ * logits, sigma).  Writes the maps and weights a render writes from those records, with the same kernel, one launch per frame. */
+int nb_debug_composite(const nb_render_args* a, const float* raw, void* stream);
+/* Its backward as the training backward runs it: d_raw (B,n,S,4) = d loss / d(rgb logits, sigma) from the five map
+ * cotangents (device, dense, any NULL; see nb_render_bwd_maps).  With `rec` (device (B,n,S,8): per sample d loss / d(world
+ * point) 3 | d loss / d(view direction) 3 | 2 unused, standing in for the decoder's part) it also ACCUMULATES d_ray_o, d_ray_d,
+ * d_near, d_far and d_z_vals of `grads` (as nb_render_bwd_inputs; d_R, d_Th, d_bounds must be NULL).  n_samples <= 256.  Sizes and
+ * pointers are validated before anything is enqueued. */
+int nb_debug_composite_bwd(const nb_render_args* a, const float* raw, const float* d_rgb_map, const float* d_depth_map,
+                           const float* d_acc_map, const float* d_disp_map, const float* d_weights, const float* rec,
+                           const nb_render_input_grads* grads, float* d_raw, void* stream);
 
 #ifdef __cplusplus
 }

@@ -15,7 +15,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_pack_volume", "nb_packed_weights_bytes", "nb_pack_weights", "nb_render_fwd",
            "nb_render_fwd_launches", "nb_render_fwd_workspace_bytes", "nb_render_bwd", "nb_render_bwd_frame", "nb_render_bwd_rays",
            "nb_render_bwd_maps", "nb_render_bwd_inputs", "nb_render_save_bytes",
-           "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_decode_density", "nb_decode_density_workspace_bytes",
+           "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_debug_composite",
+           "nb_debug_composite_bwd", "nb_decode_density", "nb_decode_density_workspace_bytes",
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
@@ -226,6 +227,11 @@ def load(path=None):
     lib.nb_render_bwd_workspace_bytes_for.argtypes = [C.POINTER(nb_render_args)]
     lib.nb_debug_gemm_tf32x3.restype = C.c_int
     lib.nb_debug_gemm_tf32x3.argtypes = [C.c_void_p] * 3 + [C.c_int] * 6 + [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.nb_debug_composite.restype = C.c_int
+    lib.nb_debug_composite.argtypes = [C.POINTER(nb_render_args), C.c_void_p, C.c_void_p]
+    lib.nb_debug_composite_bwd.restype = C.c_int
+    lib.nb_debug_composite_bwd.argtypes = [C.POINTER(nb_render_args)] + [C.c_void_p] * 7 + [C.POINTER(nb_render_input_grads),
+                                                                                            C.c_void_p, C.c_void_p]
     lib.nb_decode_density.restype = C.c_int
     lib.nb_decode_density.argtypes = [C.POINTER(nb_render_args), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     lib.nb_decode_density_workspace_bytes.restype = C.c_size_t

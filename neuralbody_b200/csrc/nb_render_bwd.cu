@@ -828,3 +828,58 @@ extern "C" int nb_render_bwd_inputs(const nb_render_bwd_args* a, const float* d_
     if (e != cudaSuccess) { set_error("nb_render_bwd: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
     return NB_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ diagnostics
+// The per-ray stages around the decoder on caller-made raw records: composite_kernel (the maps and weights of a render) and
+// composite_bwd_kernel / ray_grad_kernel (d raw, and the ray and depth gradients) exactly as the render calls launch them.
+// tests/test_ray_stages_gpu.py compares them with a float64 raw2outputs.
+static int debug_composite_params(const nb_render_args* a, const float* raw, const char* who, int max_samples, RenderParams* p) {
+    if (!a || !raw) { set_error("%s: null args or raw", who); return NB_ERR_BAD_ARG; }
+    if (a->batch <= 0) { set_error("%s: batch must be > 0", who); return NB_ERR_BAD_ARG; }
+    *p = RenderParams{};
+    p->batch = a->batch;
+    const int st = fill_ray_params(a, who, p);
+    if (st != NB_OK) return st;
+    if (a->n_samples > max_samples) { set_error("%s: n_samples <= %d supported (got %d)", who, max_samples, a->n_samples); return NB_ERR_UNSUPPORTED; }
+    p->stats = nullptr; p->trace = nullptr; p->save = nullptr;
+    return NB_OK;
+}
+
+extern "C" int nb_debug_composite(const nb_render_args* a, const float* raw, void* stream) {
+    RenderParams p;
+    const int st = debug_composite_params(a, raw, "nb_debug_composite", kListMaxSamples, &p);
+    if (st != NB_OK) return st;
+    if (p.n_rays == 0) return NB_OK;
+    for (int b = 0; b < p.batch; ++b) {
+        p.frame = b;
+        p.raw_ws = reinterpret_cast<float4*>(const_cast<float*>(raw)) + (size_t)b * p.n_rays * p.n_samples;
+        launch_composite(p, (cudaStream_t)stream);
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("nb_debug_composite: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
+    return NB_OK;
+}
+
+extern "C" int nb_debug_composite_bwd(const nb_render_args* a, const float* raw, const float* d_rgb_map, const float* d_depth_map,
+                                      const float* d_acc_map, const float* d_disp_map, const float* d_weights, const float* rec,
+                                      const nb_render_input_grads* in, float* d_raw, void* stream) {
+    const char* who = "nb_debug_composite_bwd";
+    RenderParams p;
+    int st = debug_composite_params(a, raw, who, bwd::kBwdMaxSamples, &p);
+    if (st != NB_OK) return st;
+    if (!d_raw) { set_error("%s: d_raw is null", who); return NB_ERR_BAD_ARG; }
+    const nb_render_input_grads none{};
+    if (!in) in = &none;
+    if (in->d_R || in->d_Th || in->d_bounds) { set_error("%s: d_R, d_Th and d_bounds need the decoder (nb_render_bwd_inputs)", who); return NB_ERR_BAD_ARG; }
+    const GradRequest req{{d_rgb_map, d_depth_map, d_acc_map, d_disp_map, d_weights}, nullptr, nullptr, in->d_ray_o, in->d_ray_d,
+                          {in->d_near, in->d_far, in->d_z_vals}, nullptr};
+    if (req.records() && !rec) { set_error("%s: the ray and depth gradients need the per-sample record", who); return NB_ERR_BAD_ARG; }
+    if (a->z_vals && (in->d_near || in->d_far)) { set_error("%s: d_near / d_far need depths derived from near / far (z_vals was given)", who); return NB_ERR_BAD_ARG; }
+    if (p.n_rays == 0) return NB_OK;
+    const cudaStream_t s = (cudaStream_t)stream;
+    launch_composite_bwd(p, raw, req, d_raw, 4, s);
+    if (req.records()) launch_ray_grad(p, raw, req, rec, 8, s);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); return NB_ERR_CUDA; }
+    return NB_OK;
+}
