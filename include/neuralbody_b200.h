@@ -432,6 +432,32 @@ typedef struct nb_item_images_args {
 } nb_item_images_args;
 int nb_item_images(const nb_item_images_args* a, void* stream);
 
+/* The demo and mesh datasets' mask views after decoding (get_mask of multi_view_demo / multi_view_perform /
+ * multi_view_mesh_dataset.py, the masks of monocular_demo / monocular_mesh_dataset.py upstream) on the device, for nv
+ * views of one size, each with its own camera, bit for bit with OpenCV's host steps:
+ *   - with `binarise`, the source is (m != 0) (upstream's (msk_cihp != 0).astype(np.uint8)), else the decoded values;
+ *   - cv2.undistort(src, K, D) at the source size: nb_item_images' map and its 15-bit fixed-point uint8 remap;
+ *   - with dilate = 5, cv2.dilate(., np.ones((5, 5))): the maximum over the 5 x 5 window, pixels outside the image not
+ *     taking part (the default border);
+ *   - the resize to (H, W): a copy, or an exact 2x reduction by INTER_NEAREST (source pixel (2y, 2x)).
+ * Pass 1 undistorts every view at the source size into the workspace, pass 2 dilates and picks the output pixels.
+ * Validation (null pointers, sizes, the geometry, n_dist, dilate, the workspace size) happens before anything is
+ * enqueued; two launches; nothing synchronises with the host. */
+typedef struct nb_mask_views_args {
+    int nv, H0, W0;                  /* the decoded views' size, W0 <= NB_ITEM_MAX_W */
+    int H, W;                        /* the output size: (H0, W0), or exactly (H0 / 2, W0 / 2) */
+    int n_dist;                      /* the distortion model's coefficient count: 4, 5 or 8 */
+    int binarise;                    /* 1: undistort (m != 0); 0: the decoded values */
+    int dilate;                      /* 0 (none) or 5 (a 5 x 5 window) */
+    const unsigned char* msk_u8;     /* device (nv,H0,W0) */
+    const double* cams;              /* device (nv, NB_ITEM_CAM_DOUBLES): each view's K and D at the source size */
+    void* workspace;                 /* device, nb_mask_views_workspace_bytes(nv, H0, W0) bytes */
+    size_t workspace_bytes;
+    unsigned char* msks;             /* device (nv,H,W) */
+} nb_mask_views_args;
+size_t nb_mask_views_workspace_bytes(int nv, int H0, int W0);   /* 0 for an invalid size */
+int nb_mask_views(const nb_mask_views_args* a, void* stream);
+
 /* The evaluator's per-view metrics (lib/evaluators/if_nerf.py upstream) on the device, from the rendered rays, the
  * test split's colours and mask_at_box:
  *   - scatter: ray k is the k-th set pixel of mask_at_box in row-major order (img[mask_at_box] = rgb); every other pixel

@@ -20,7 +20,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
-           "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_eval_image_workspace_bytes",
+           "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_mask_views_workspace_bytes",
+           "nb_mask_views", "nb_eval_image_workspace_bytes",
            "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame", "nb_mesh_ply_bytes", "nb_mesh_ply"]
 
 
@@ -107,6 +108,12 @@ class nb_item_images_args(C.Structure):
                 ("bkgd", C.c_int), ("class_rule", C.c_int), ("img_u8", C.c_void_p), ("msk_u8", C.c_void_p),
                 ("cams", C.c_void_p), ("bound", C.c_void_p), ("img", C.c_void_p), ("msk", C.c_void_p),
                 ("class_map", C.c_void_p)]
+
+
+class nb_mask_views_args(C.Structure):
+    _fields_ = [("nv", C.c_int), ("H0", C.c_int), ("W0", C.c_int), ("H", C.c_int), ("W", C.c_int), ("n_dist", C.c_int),
+                ("binarise", C.c_int), ("dilate", C.c_int), ("msk_u8", C.c_void_p), ("cams", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("msks", C.c_void_p)]
 
 
 NB_EVAL_OK, NB_EVAL_COUNT, NB_EVAL_SMALL = 0, 1, 2
@@ -268,6 +275,10 @@ def load(path=None):
     lib.nb_train_rays.argtypes = [C.POINTER(nb_train_rays_args), C.c_void_p]
     lib.nb_item_images.restype = C.c_int
     lib.nb_item_images.argtypes = [C.POINTER(nb_item_images_args), C.c_void_p]
+    lib.nb_mask_views_workspace_bytes.restype = C.c_size_t
+    lib.nb_mask_views_workspace_bytes.argtypes = [C.c_int] * 3
+    lib.nb_mask_views.restype = C.c_int
+    lib.nb_mask_views.argtypes = [C.POINTER(nb_mask_views_args), C.c_void_p]
     lib.nb_eval_image_workspace_bytes.restype = C.c_size_t
     lib.nb_eval_image_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.nb_eval_image.restype = C.c_int

@@ -1,7 +1,11 @@
 """The training datasets' image steps after decoding on the device (nb_item_images): undistort, the resize by cfg.ratio
 (a copy or an exact 2x reduction), the background and the sampler's class map, bit for bit with OpenCV's host steps
 (oracle/item_images.py restates them).  Items of the `dataset_image_steps: 'device'` kind carry the decoded image and
-mask and the camera; Renderer.item_images runs this on a collated batch."""
+mask and the camera; Renderer.item_images runs this on a collated batch.
+
+`mask_views` is the demo and mesh datasets' counterpart for their mask views (nb_mask_views): the optional binarisation,
+the undistort, the optional 5 x 5 dilation and the INTER_NEAREST resize, per view with its own camera;
+Renderer.mask_views runs it on a collated batch."""
 import ctypes as C
 
 import numpy as np
@@ -82,3 +86,44 @@ def item_images(img_u8, msk_u8, cams, n_dist, H, W, bkgd=capi.NB_ITEM_BKGD_NONE,
         capi.check(lib.nb_item_images(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                    "nb_item_images")
         return img, msk, cmap
+
+
+def mask_views(msk_u8, cams, n_dist, H, W, binarise, dilate):
+    """nb_mask_views on one item's views: msk_u8 (nv,H0,W0) uint8 CUDA tensor as decoded, cams (nv, NB_ITEM_CAM_DOUBLES)
+    float64 on the host (stacked `item_camera` results; `n_dist` the largest of their coefficient counts: the rest are
+    zero), the output size (a copy or an exact 2x reduction, see `reduction`), `binarise` (undistort m != 0) and `dilate`
+    (0 or 5).  Everything is validated before the launch; nothing synchronises with the host.  -> msks (nv,H,W) uint8."""
+    lib = capi.load()
+    if not torch.is_tensor(msk_u8) or msk_u8.device.type != "cuda":
+        raise ValueError("msk_u8 must be a CUDA tensor")
+    if msk_u8.dim() != 3 or msk_u8.dtype != torch.uint8:
+        raise ValueError("msk_u8 must be (nv,H0,W0) uint8 (got %s %s)" % (tuple(msk_u8.shape), msk_u8.dtype))
+    dev = msk_u8.device
+    nv, H0, W0 = (int(s) for s in msk_u8.shape)
+    if nv < 1 or W0 > capi.NB_ITEM_MAX_W:
+        raise ValueError("mask_views takes at least one view up to %d pixels wide (got %d views of %dx%d)"
+                         % (capi.NB_ITEM_MAX_W, nv, H0, W0))
+    reduction(H0, W0, H, W)
+    cams = np.ascontiguousarray(cams, dtype=np.float64)
+    if cams.shape != (nv, capi.NB_ITEM_CAM_DOUBLES):
+        raise ValueError("cams must be (nv, %d) (got %s)" % (capi.NB_ITEM_CAM_DOUBLES, cams.shape))
+    if int(n_dist) not in (4, 5, 8) or int(dilate) not in (0, 5) or int(binarise) not in (0, 1):
+        raise ValueError("n_dist must be 4, 5 or 8, dilate 0 or 5 and binarise 0 or 1 (got %s, %s, %s)"
+                         % (n_dist, dilate, binarise))
+    with torch.cuda.device(dev):
+        a = capi.nb_mask_views_args()
+        a.nv, a.H0, a.W0, a.H, a.W = nv, H0, W0, int(H), int(W)
+        a.n_dist, a.binarise, a.dilate = int(n_dist), int(binarise), int(dilate)
+        msk_u8 = msk_u8.contiguous()
+        a.msk_u8 = msk_u8.data_ptr()
+        cams_dev = torch.from_numpy(cams).pin_memory().to(dev, non_blocking=True)
+        a.cams = cams_dev.data_ptr()
+        ws = None
+        if a.dilate:
+            a.workspace_bytes = lib.nb_mask_views_workspace_bytes(nv, H0, W0)
+            ws = torch.empty(a.workspace_bytes, dtype=torch.uint8, device=dev)
+            a.workspace = ws.data_ptr()
+        out = torch.empty((nv, int(H), int(W)), dtype=torch.uint8, device=dev)
+        a.msks = out.data_ptr()
+        capi.check(lib.nb_mask_views(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "nb_mask_views")
+        return out

@@ -7,7 +7,10 @@ and the float32 `can_bounds` (2,3) of the rotated body. neuralbody_b200's render
 and mask_at_box from them on the GPU (nb_image_rays). `meta` holds the same three arrays: upstream's visualize loop
 (run.py) moves every key but `meta` to the GPU, so the renderer reads the camera there with no copy back to the host.
 Every other key is upstream's, including the mask `msk` (decoded, undistorted and resized on the host by upstream's own
-calls) and `RT` / `K`, the same camera as the masked renderer reads it.
+calls) and `RT` / `K`, the same camera as the masked renderer reads it.  With `dataset_image_steps: 'device'` the item
+stops after decoding the mask: it ships `msks_u8` (1,H0,W0) uint8 as read in place of `msk`, and the camera K, D and the
+recipe (no binarisation, no dilation, the INTER_NEAREST resize by cfg.ratio) under `meta`; the `_msk` renderer builds
+the same `msk` on the GPU (Renderer.mask_views, nb_mask_views).
 
 `make_dataset_class(base)` builds the subclass over any base with the reference's attributes (`data_root`, `cam`,
 `params`, `prepare_input`); `Dataset` is the one over the reference's own Dataset, resolved on first use.  OpenCV and
@@ -19,6 +22,7 @@ import os
 import numpy as np
 
 from neuralbody_b200.lib.config import get_active_cfg
+from neuralbody_b200.lib.datasets import mask_item, train_item
 
 REFERENCE_MODULE = "lib.datasets.light_stage.monocular_demo_dataset"
 
@@ -54,14 +58,19 @@ def make_dataset_class(base, cv2=None, imread=None):
             view_index = index
             coord, out_sh, can_bounds, bounds, Rh, Th = self.prepare_input(i, index)
             msk = read(os.path.join(self.data_root, 'mask', '{}.png'.format(i)))
-            msk = cv.undistort(msk, K, D)
             H, W = int(msk.shape[0] * cfg.ratio), int(msk.shape[1] * cfg.ratio)
-            msk = cv.resize(msk, (W, H), interpolation=cv.INTER_NEAREST)
+            if train_item.image_steps(cfg) == 'device':
+                msk_keys, mask_meta = mask_item.mask_fields([msk], [K], [D], H, W, False, 0)
+            else:
+                msk = cv.undistort(msk, K, D)
+                msk = cv.resize(msk, (W, H), interpolation=cv.INTER_NEAREST)
+                msk_keys, mask_meta = {'msk': msk}, {}
             K = K.copy().astype(np.float32)
             K[:2] = K[:2] * cfg.ratio
             RT = np.concatenate([R, T], axis=1).astype(np.float32)
             # :116-142 without the rays
-            ret = {'coord': coord, 'out_sh': out_sh, 'msk': msk}
+            ret = {'coord': coord, 'out_sh': out_sh}
+            ret.update(msk_keys)
             R = cv.Rodrigues(Rh)[0].astype(np.float32)
             ret.update({'bounds': bounds, 'R': R, 'Th': Th, 'latent_index': latent_index, 'frame_index': frame_index,
                         'view_index': view_index})
@@ -73,6 +82,7 @@ def make_dataset_class(base, cv2=None, imread=None):
             ret.update({'cam_RT': RT, 'cam_K': K, 'can_bounds': can_bounds})
             # a host copy for the renderer: upstream's visualize loop moves every key but 'meta' to the GPU
             ret['meta'] = {'cam_RT': ret['cam_RT'], 'cam_K': ret['cam_K'], 'can_bounds': can_bounds}
+            ret['meta'].update(mask_meta)
             return ret
 
     return Dataset

@@ -13,6 +13,11 @@ neuralbody_b200's if_mesh_renderer builds the grid axes and the test from them a
 The image is neither decoded nor resized: nothing downstream of the mesh item reads it.  The output size is therefore
 taken from the mask, which has the image's size in People-Snapshot (upstream takes it from the image).
 
+With `dataset_image_steps: 'device'` (default 'host') the item stops after decoding the mask: it ships `msks_u8`
+(1,H0,W0) uint8 as read in place of `msks`, and the camera K, D and the recipe (no binarisation, no dilation, the
+INTER_NEAREST resize by cfg.ratio) under `meta` (lib/datasets/mask_item.py); the mesh renderer builds the same `msks` on
+the GPU (Renderer.mask_views, nb_mask_views).
+
 `Dataset` subclasses the reference's own Dataset, resolved when it is first asked for (so this module imports without the
 reference tree); `make_dataset_class(base)` builds the same subclass over any base with the reference's attributes
 (`data_root`, `cam`, `begin_ith_frame`, `prepare_input`).  OpenCV and imageio are imported only when an item is built.
@@ -24,6 +29,7 @@ import os
 import numpy as np
 
 from neuralbody_b200.lib.config import get_active_cfg
+from neuralbody_b200.lib.datasets import mask_item, train_item
 
 REFERENCE_MODULE = "lib.datasets.light_stage.monocular_mesh_dataset"
 
@@ -55,13 +61,19 @@ def make_dataset_class(base, cv2=None, imread=None):
             msk = read(os.path.join(self.data_root, 'mask', '{}.png'.format(index)))
             K = self.cam['K']
             D = self.cam['D']
-            msk = cv.undistort(msk, K, D)
+            device = train_item.image_steps(cfg) == 'device'
+            if not device:
+                msk = cv.undistort(msk, K, D)
             R = self.cam['R']
             T = self.cam['T'][:, None]
             coord, out_sh, can_bounds, bounds, Rh, Th = self.prepare_input(index)
             # :72-79, without the image
             H, W = int(msk.shape[0] * cfg.ratio), int(msk.shape[1] * cfg.ratio)
-            msk = cv.resize(msk, (W, H), interpolation=cv.INTER_NEAREST)
+            if device:
+                msk_keys, mask_meta = mask_item.mask_fields([msk], [K], [D], H, W, False, 0)
+            else:
+                msk = cv.resize(msk, (W, H), interpolation=cv.INTER_NEAREST)
+                msk_keys, mask_meta = {'msks': np.asarray(msk, dtype=np.uint8)[None]}, None
             K = K.copy()
             K[:2] = K[:2] * cfg.ratio
             ret = {'coord': coord, 'out_sh': out_sh}
@@ -70,9 +82,11 @@ def make_dataset_class(base, cv2=None, imread=None):
             ret.update({'wbounds': can_bounds, 'bounds': bounds, 'R': R_smpl, 'Th': Th, 'latent_index': latent_index,
                         'frame_index': frame_index})
             # what prepare_inside_pts (:35-48) reads: one view, the camera in its own dtype
-            ret['msks'] = np.asarray(msk, dtype=np.uint8)[None]
+            ret.update(msk_keys)
             ret['Ks'] = K[None]
             ret['RT'] = np.concatenate([R, T], axis=1)[None]
+            if mask_meta is not None:
+                ret['meta'] = mask_meta
             return ret
 
     return Dataset

@@ -113,7 +113,10 @@ class Renderer(if_nerf_renderer.Renderer):
     def density_cube(self, batch):
         """The padded density cube on the device (fp32: it holds the fp32 sigma and zeros, so it is exact as upstream's
         float64 cube), shape (X + 20, Y + 20, Z + 20).  The grid comes from the batch's `pts` / `inside` when both are
-        there, else from its mask views (`wbounds`, `RT`, `Ks`, `msks`; see `grid_from_masks`)."""
+        there, else from its mask views (`wbounds`, `RT`, `Ks`, `msks`; see `grid_from_masks`).  A batch of 'device' items
+        carries the decoded views (`msks_u8`) in place of `msks`: mask_views builds them on the device first."""
+        if 'pts' not in batch and 'msks' not in batch and 'msks_u8' in batch:
+            self.mask_views(batch)
         if 'pts' in batch and 'inside' in batch:
             wpts, inside = self.grid_from_points(batch)
         elif all(k in batch for k in MASK_KEYS):

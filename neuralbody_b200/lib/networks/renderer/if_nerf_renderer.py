@@ -744,6 +744,31 @@ class Renderer:
             batch['msk'] = msk
         return batch
 
+    # the batch key mask_views writes: upstream's masked renderers read the views as `msks` (1,nv,H,W); the single-view
+    # renderer (if_nerf_renderer_msk) reads `msk` (1,H,W)
+    MASK_VIEWS_KEY = 'msks'
+
+    def mask_views(self, batch):
+        """The mask steps of a batch from the demo and mesh datasets' `dataset_image_steps: 'device'` items (`msks_u8`
+        (1,nv,H0,W0) uint8 as decoded, and in batch['meta'] on the host `mask_cams`, `mask_n_dist`, `mask_size`,
+        `mask_binarise`, `mask_dilate`): binarise, undistort, dilate and resize on the device (neuralbody_b200.images.
+        mask_views, bit for bit with upstream's cv2 steps).  Writes `msks` (1,nv,H,W) uint8 into the batch, or `msk` (1,H,W)
+        for the single-view renderer (MASK_VIEWS_KEY).  B = 1, as upstream's loaders.  Nothing synchronises with the host."""
+        from neuralbody_b200 import images
+        meta, msk_u8 = batch['meta'], batch['msks_u8']
+        if msk_u8.dim() != 4 or msk_u8.shape[0] != 1:
+            raise ValueError("batch['msks_u8'] must be (1,nv,H0,W0) (B = 1, as upstream); got %s" % (tuple(msk_u8.shape),))
+        if self.MASK_VIEWS_KEY == 'msk' and msk_u8.shape[1] != 1:
+            raise ValueError("the single-view renderer takes one mask view (got %d)" % msk_u8.shape[1])
+        dev = msk_u8.device if msk_u8.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+        one = lambda k: int(torch.as_tensor(meta[k]).reshape(-1)[0])
+        H, W = (int(v) for v in torch.as_tensor(meta['mask_size']).reshape(-1)[:2])
+        cams = torch.as_tensor(meta['mask_cams']).reshape(-1, images.capi.NB_ITEM_CAM_DOUBLES).numpy()
+        out = images.mask_views(msk_u8[0].to(dev, non_blocking=True), cams, one('mask_n_dist'), H, W,
+                                one('mask_binarise'), one('mask_dilate'))
+        batch[self.MASK_VIEWS_KEY] = out[None] if self.MASK_VIEWS_KEY == 'msks' else out
+        return batch
+
     def check_train_rays(self):
         """Raise RuntimeError when the last train_rays call failed (a view whose bound pixels' rays all miss the box, where
         upstream loops forever)."""

@@ -36,7 +36,10 @@ class Renderer(if_nerf_renderer.Renderer):
         return inside
 
     def get_pixel_value(self, ray_o, ray_d, near, far, feature_volume, sp_input, batch):
-        """if_clight_renderer_mmsk.py:63-94."""
+        """if_clight_renderer_mmsk.py:63-94.  A batch of 'device' items carries the decoded views (`msks_u8`) in place of
+        `msks`: mask_views builds them on the device first."""
+        if 'msks' not in batch and 'msks_u8' in batch:
+            self.mask_views(batch)
         if 'Ks' not in batch or 'RT' not in batch or 'msks' not in batch:
             raise KeyError("the masked renderer needs batch['RT'], batch['Ks'] and batch['msks'] "
                            "(lib/datasets/light_stage/multi_view_demo_dataset.py:107-129)")

@@ -15,6 +15,8 @@ from neuralbody_b200.lib.networks.renderer import if_nerf_renderer_mmsk
 
 
 class Renderer(if_nerf_renderer_mmsk.Renderer):
+    MASK_VIEWS_KEY = 'msk'
+
     def __init__(self, net):
         super(Renderer, self).__init__(net)
 
@@ -35,7 +37,10 @@ class Renderer(if_nerf_renderer_mmsk.Renderer):
         return batch['msk'][0][pts2d[:, 1], pts2d[:, 0]][None].bool()
 
     def get_pixel_value(self, ray_o, ray_d, near, far, feature_volume, sp_input, batch):
-        """if_clight_renderer_mmsk.py:63-94 with the single-view predicate above."""
+        """if_clight_renderer_mmsk.py:63-94 with the single-view predicate above.  A batch of 'device' items carries the
+        decoded view (`msks_u8`) in place of `msk`: mask_views builds it on the device first."""
+        if 'msk' not in batch and 'msks_u8' in batch:
+            self.mask_views(batch)
         for k in ('R0_snap', 'Th0_snap', 'RT', 'K', 'msk'):
             if k not in batch:
                 raise KeyError("the single-view masked renderer needs batch['%s'] "
