@@ -21,6 +21,8 @@ _PRECISIONS = {"fp32": capi.NB_PRECISION_FP32, "tc_fp16": capi.NB_PRECISION_TC_F
                "tc_fp16x3": capi.NB_PRECISION_TC_FP16X3}
 # the fields of nb_decoder_weights that point at the 17 tensors of Network.decoder_tensors(), in that order
 _DECODER_FIELDS = tuple(f[0] for f in capi.nb_decoder_weights._fields_[:17])
+# samples per ray nb_render_bwd takes (kBwdMaxSamples, nb_render_bwd.cu): the most a differentiable call may render
+_BWD_MAX_SAMPLES = 256
 
 
 def _input_grad_slots(B, n, S):
@@ -101,6 +103,21 @@ class Renderer:
         if name == "tc_tf32x3" and S <= 256 and B * n * S < (1 << 28) and self.lib.nb_has_precision(capi.NB_PRECISION_TC_TF32X3):
             return capi.NB_PRECISION_TC_TF32X3
         return capi.NB_PRECISION_FP32
+
+    def _needs_grad(self, feature_volume, inputs):
+        """True when autograd is recording and any decoder tensor, volume or input tensor (`inputs`, None allowed) requires
+        grad: the call then runs the training precision under `_FusedRender`."""
+        return torch.is_grad_enabled() and (any(t.requires_grad for t in self.net.decoder_tensors()) or
+                                            any(v.requires_grad for v in feature_volume) or
+                                            any(torch.is_tensor(t) and t.requires_grad for t in inputs))
+
+    @staticmethod
+    def _check_grad_samples(S, what):
+        """A differentiable call is refused before anything is enqueued when its backward could not run: nb_render_bwd
+        takes rays of at most _BWD_MAX_SAMPLES samples, and finding out inside loss.backward() would waste the forward."""
+        if S > _BWD_MAX_SAMPLES:
+            raise NotImplementedError("a differentiable render supports at most %d samples per ray (the backward's limit); %s "
+                                      "has %d" % (_BWD_MAX_SAMPLES, what, S))
 
     def _volume_dtype(self, precision):
         name = str(self._opt("render_volume_dtype", "auto"))
@@ -247,9 +264,9 @@ class Renderer:
         inputs = [sp_input['R'], sp_input['Th'], ray_o, ray_d, near if z_vals is None else None,
                   far if z_vals is None else None, sp_input['bounds'], z_vals]
         inputs = [t if torch.is_tensor(t) else None for t in inputs]
-        needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in params) or
-                                                  any(v.requires_grad for v in feature_volume) or
-                                                  any(t is not None and t.requires_grad for t in inputs))
+        needs_grad = self._needs_grad(feature_volume, inputs)
+        if needs_grad:
+            self._check_grad_samples(S, "this call" if z_vals is None else "z_vals")
         precision = self._train_precision(B, n, S) if needs_grad else self._precision("render_precision", "tc_fp16x3")
         skip_empty = bool(self._opt("render_skip_empty", True))
         if precision != capi.NB_PRECISION_FP32 and (S > 1024 or n * S >= (1 << 28)):
@@ -618,6 +635,9 @@ class Renderer:
         S = int(cfg.N_samples)
         dev = ray_o.device
         B, n = int(ray_o.shape[0]), int(ray_o.shape[1])
+        if self._needs_grad(feature_volume, [sp_input['R'], sp_input['Th'], ray_o, ray_d, near, far, sp_input['bounds']]):
+            # the fine pass would be refused only after the coarse pass and the sampler ran
+            self._check_grad_samples(S + Ni, "the fine pass (N_samples + render_importance)")
         if t_rand is None and float(cfg.perturb) > 0. and self.net.training:
             t_rand = self._draw_t_rand(B, n, S, dev)
         if u is None and float(cfg.perturb) != 0.:

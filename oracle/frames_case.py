@@ -101,8 +101,21 @@ def fragile_samples(scene, t_rand):
     zero.  A sample with all-zero features has sigma(empty) < 0 and weight 0: no gradient flows through it."""
     from oracle import neuralbody_oracle as O
     sc = to_double(scene)
-    B, n, S = t_rand.shape
-    pts, _ = O.get_sampling_points(sc["ray_o"], sc["ray_d"], sc["near"], sc["far"], S, 1.0, True, t_rand.double())
+    _, z_vals = O.get_sampling_points(sc["ray_o"], sc["ray_d"], sc["near"], sc["far"], t_rand.shape[2], 1.0, True,
+                                      t_rand.double())
+    return sample_conditions(scene, z_vals)["fragile"]
+
+
+def sample_conditions(scene, z_vals, scale=None, kinks=True):
+    """What fragile_samples decides, for the samples at the depths z_vals (B,n,S) along the scene's rays, in float64.
+    Returns dict of (B,n,S) tensors: 'fragile', 'occupied' (a non-zero feature), 'face' (distance in cells to the nearest
+    trilinear cell face of any level), and 'scale': the rms pre-activation of each ReLU layer over the occupied samples, the
+    unit of RELU_MARGIN.  `scale` given: judge against those rms values instead, so that a subset of samples (redrawn ones)
+    is held to the margins of the whole set it belongs to.  kinks=False: 'occupied' and 'face' only (no decoder run)."""
+    from oracle import neuralbody_oracle as O
+    sc = to_double(scene)
+    B, n, S = z_vals.shape
+    pts = sc["ray_o"][:, :, None] + sc["ray_d"][:, :, None] * z_vals.double()[..., None]   # get_sampling_points' pts
     pts = pts.reshape(B, n * S, 3)
     sp = O.prepare_sp_input(sc)
     grid = O.get_grid_coords(O.pts_to_can_pts(pts, sp["R"], sp["Th"]), sp["bounds"], sp["out_sh"], sc["voxel_size"])
@@ -114,6 +127,8 @@ def fragile_samples(scene, t_rand):
     w = sc["weights"]
     feats = O.interpolate_features(grid, sc["volumes"])                               # (B, 352, P)
     occupied = (feats != 0).any(1)
+    if not kinks:
+        return {"occupied": occupied.view(B, n, S), "face": face.view(B, n, S)}
     pre = []
     h = feats
     for name in ("fc_0", "fc_1", "fc_2"):
@@ -127,11 +142,15 @@ def fragile_samples(scene, t_rand):
     f = torch.cat((f, O.positional_embed(viewdir, 4).transpose(1, 2), O.positional_embed(pts, 10).transpose(1, 2)), 1)
     pre.append(O._conv(w, "view_fc", f))
     kink = torch.zeros((B, n * S), dtype=torch.bool)
-    for z in pre:
+    rms_of = []
+    for i, z in enumerate(pre):
         live = occupied[:, None].expand_as(z)
         rms = float(z[live].pow(2).mean().sqrt()) if bool(live.any()) else 1.0
+        rms = rms if scale is None else scale[i]
+        rms_of.append(rms)
         kink |= (z.abs() < RELU_MARGIN * rms).any(1)
-    return (occupied & ((face < FACE_MARGIN) | kink)).view(B, n, S)
+    return {"fragile": (occupied & ((face < FACE_MARGIN) | kink)).view(B, n, S), "occupied": occupied.view(B, n, S),
+            "face": face.view(B, n, S), "scale": rms_of}
 
 
 def well_conditioned(scene, t_rand, gen):
