@@ -561,6 +561,33 @@ typedef struct nb_mesh_ply_args {
 size_t nb_mesh_ply_bytes(long long nv, long long nf);   /* 24 nv + 13 nf; 0 for invalid counts (and for an empty mesh) */
 int nb_mesh_ply(const nb_mesh_ply_args* a, void* stream);
 
+/* The image losses of upstream's training wrapper (lib/train/trainers/if_nerf_clight.py:24-32) on the device, without the
+ * host wait of a boolean-mask index:
+ *   img_loss  = mean over the set rays' elements of (rgb_map - rgb)^2   (mask = mask_at_box)
+ *   img_loss0 = mean over all elements of (rgb0 - rgb)^2                (mask = NULL)
+ * nb_image_loss_fwd writes the loss (float32; the sum in float64, then one rounding) and the number of elements averaged,
+ * 3 x the set rays, in ONE launch: per-CTA partials over a grid that depends on `rays` only, finished in CTA order by the
+ * last CTA (an integer ticket), so the loss is the same bits on every run; no floating-point atomics.  No element gives a
+ * NaN loss, as torch.mean of an empty tensor.  nb_image_loss_bwd writes d_pred (rays,3), the cotangent autograd computes
+ * on the GPU for upstream's expression, bit for bit: g * (1.0f / (float)count), times 2 * (pred - gt), in fp32 in that
+ * order, on the set rays (plus 0, the index backward's scatter into zeros, when there is a mask) and exact 0 elsewhere; g is
+ * the device scalar d_loss and count the forward's.  Validation happens before anything is enqueued; both enqueue one
+ * launch on the caller's stream (none for rays = 0 in the backward); nothing allocates or synchronises.  The workspace is
+ * zeroed once when allocated and the forward leaves it so; calls that share one must be ordered (one stream). */
+typedef struct nb_image_loss_args {
+    int rays;                          /* B*n rays of 3 channels, 0 <= 3 rays < 2^31 */
+    const float* pred;                 /* device (rays,3): rgb_map or rgb0 */
+    const float* gt;                   /* device (rays,3): batch['rgb'] */
+    const unsigned char* mask;         /* device (rays), nonzero = set (bool or uint8); NULL = every ray */
+    void* workspace;                   /* device, 256-byte aligned, nb_image_loss_workspace_bytes(); forward only */
+    size_t workspace_bytes;
+    float* loss;                       /* device scalar; written by the forward */
+    long long* count;                  /* device scalar: elements averaged; written by the forward, read by the backward */
+} nb_image_loss_args;
+size_t nb_image_loss_workspace_bytes(void);
+int nb_image_loss_fwd(const nb_image_loss_args* a, void* stream);
+int nb_image_loss_bwd(const nb_image_loss_args* a, const float* d_loss, float* d_pred, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

@@ -22,7 +22,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
            "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_mask_views_workspace_bytes",
            "nb_mask_views", "nb_eval_image_workspace_bytes",
-           "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame", "nb_mesh_ply_bytes", "nb_mesh_ply"]
+           "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame", "nb_mesh_ply_bytes", "nb_mesh_ply",
+           "nb_image_loss_workspace_bytes", "nb_image_loss_fwd", "nb_image_loss_bwd"]
 
 
 class nb_volume_level(C.Structure):
@@ -155,6 +156,11 @@ class nb_mesh_ply_result(C.Structure):
 class nb_mesh_ply_args(C.Structure):
     _fields_ = [("nv", C.c_longlong), ("nf", C.c_longlong), ("vertices", C.c_void_p), ("faces", C.c_void_p),
                 ("out", C.c_void_p), ("out_bytes", C.c_size_t)]
+
+
+class nb_image_loss_args(C.Structure):
+    _fields_ = [("rays", C.c_int), ("pred", C.c_void_p), ("gt", C.c_void_p), ("mask", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t), ("loss", C.c_void_p), ("count", C.c_void_p)]
 
 
 class nb_image_rays_args(C.Structure):
@@ -291,6 +297,12 @@ def load(path=None):
     lib.nb_mesh_ply_bytes.argtypes = [C.c_longlong, C.c_longlong]
     lib.nb_mesh_ply.restype = C.c_int
     lib.nb_mesh_ply.argtypes = [C.POINTER(nb_mesh_ply_args), C.c_void_p]
+    lib.nb_image_loss_workspace_bytes.restype = C.c_size_t
+    lib.nb_image_loss_workspace_bytes.argtypes = []
+    lib.nb_image_loss_fwd.restype = C.c_int
+    lib.nb_image_loss_fwd.argtypes = [C.POINTER(nb_image_loss_args), C.c_void_p]
+    lib.nb_image_loss_bwd.restype = C.c_int
+    lib.nb_image_loss_bwd.argtypes = [C.POINTER(nb_image_loss_args), C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):
