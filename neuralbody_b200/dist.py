@@ -139,9 +139,12 @@ class FrameGatherer:
         g = FrameGatherer(n_rays, world, rank, device)
         for v in views:
             out = g.begin()                      # dict of slab views for Renderer.render_rays(out=...), compute stream
-            renderer.render_rays(..., out=out)
+            renderer.render_rays(..., out=out)   # or, with cfg.render_importance > 0 (coarse + fine sampling):
+            #   renderer.render_rays_hierarchical(..., out=out)   -- the fine pass's maps go into the slab
             frame = g.finish()                   # enqueues all-gather + un-permute (+ D2H on rank `host_rank`) on the side stream
         g.drain()                                # frames of the last views are complete after this
+
+    Rays are independent in both passes, so the gathered frame holds the same bits as one unsharded render of the view.
 
     `finish` returns the (B, n_rays, 6) device frame of THIS view (valid once the side stream has run; `drain` or
     `frame_ready(i).synchronize()`); with `host=True` the view's owner also copies it into a pinned host buffer.  The owner is

@@ -624,28 +624,50 @@ class Renderer:
             z = lower + (upper - lower) * t_rand.to(device=dev, dtype=torch.float32)
         return z
 
-    def render_rays_hierarchical(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, u=None):
+    def render_rays_hierarchical(self, ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=None, u=None, masks=None,
+                                 out=None):
         """Coarse pass (cfg.N_samples) -> importance samples from its weights -> fine pass over the merged depths with the SAME
         network, as the reference's NeRF-baseline renderer does (volume_renderer.py:60-118; Neural Body's own renderer has no
         fine pass, SURVEY 8f-4).  `cfg.render_importance` = N_importance; det = (cfg.perturb == 0) as upstream.
         Both passes are nb_render_fwd launches (the fine one with nb_render_args.z_vals); under autograd each is a
-        `_FusedRender` node and the importance samples are detached, as upstream."""
+        `_FusedRender` node and the importance samples are detached, as upstream.
+        `masks`: the mask views of render_rays (f-1, B = 1), applied in both passes, so the weights that drive the sampler are
+        the masked coarse weights (upstream's masked get_pixel_value as the coarse network of volume_renderer.py).  `out`:
+        the fine pass's rgb / disp / acc / depth maps go there (dense maps or columns of one record, as render_rays takes
+        them, e.g. a dist.FrameGatherer slab).  Without autograd the coarse pass's depth map and weights are scratch from the
+        renderer's pool; with perturb == 0 the call draws nothing on the host and does not synchronise with it."""
         cfg = get_active_cfg()
         Ni = int(self._opt("render_importance", 0))
         S = int(cfg.N_samples)
         dev = ray_o.device
         B, n = int(ray_o.shape[0]), int(ray_o.shape[1])
-        if self._needs_grad(feature_volume, [sp_input['R'], sp_input['Th'], ray_o, ray_d, near, far, sp_input['bounds']]):
+        needs_grad = self._needs_grad(feature_volume, [sp_input['R'], sp_input['Th'], ray_o, ray_d, near, far, sp_input['bounds']])
+        if needs_grad:
             # the fine pass would be refused only after the coarse pass and the sampler ran
             self._check_grad_samples(S + Ni, "the fine pass (N_samples + render_importance)")
+            if out is not None:
+                raise NotImplementedError("`out` maps are an inference feature: a differentiable render returns its own maps")
         if t_rand is None and float(cfg.perturb) > 0. and self.net.training:
             t_rand = self._draw_t_rand(B, n, S, dev)
         if u is None and float(cfg.perturb) != 0.:
             u = torch.rand((B * n, Ni)).view(B, n, Ni).to(dev)          # nerf_net_utils.py:70 (CPU generator, like upstream)
-        coarse = self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=t_rand,
+        scratch = None
+        if not needs_grad:
+            # the coarse maps the caller gets back (rgb0 / disp0 / acc0) are its own; the coarse depth map and the (B,n,S)
+            # weights only feed the sampler, so they live in one pooled record, handed back once the sampler is enqueued
+            scratch = self._pool_take("coarse", B * n * (S + 1), torch.float32, dev)
+            cout = {'rgb_map': torch.empty((B, n, 3), dtype=torch.float32, device=dev),
+                    'disp_map': torch.empty((B, n), dtype=torch.float32, device=dev),
+                    'acc_map': torch.empty((B, n), dtype=torch.float32, device=dev),
+                    'depth_map': scratch[:B * n].view(B, n),
+                    'weights': scratch[B * n:B * n * (S + 1)].view(B, n, S)}
+        coarse = self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, t_rand=t_rand, masks=masks,
+                                  out=None if scratch is None else cout,
                                   want_weights=True)          # the coarse weights drive the importance sampling
         z_all, z_smp = self.importance_z_vals(near, far, coarse['weights'], S, Ni, t_rand=t_rand, u=u)
-        fine = dict(self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, z_vals=z_all))
+        # stream-ordered reuse: the next call's coarse pass on this stream runs after the sampler has read the weights
+        self._pool_give("coarse", scratch)
+        fine = dict(self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, z_vals=z_all, masks=masks, out=out))
         fine['rgb0'], fine['disp0'], fine['acc0'] = coarse['rgb_map'], coarse['disp_map'], coarse['acc_map']
         fine['z_std'] = torch.std(z_smp, dim=-1, unbiased=False)
         return fine

@@ -37,7 +37,8 @@ class Renderer(if_nerf_renderer.Renderer):
 
     def get_pixel_value(self, ray_o, ray_d, near, far, feature_volume, sp_input, batch):
         """if_clight_renderer_mmsk.py:63-94.  A batch of 'device' items carries the decoded views (`msks_u8`) in place of
-        `msks`: mask_views builds them on the device first."""
+        `msks`: mask_views builds them on the device first.  With `cfg.render_importance > 0` the view gets the coarse + fine
+        passes of `render_rays_hierarchical`, both masked, and the dict also carries rgb0 / disp0 / acc0 / z_std."""
         if 'msks' not in batch and 'msks_u8' in batch:
             self.mask_views(batch)
         if 'Ks' not in batch or 'RT' not in batch or 'msks' not in batch:
@@ -47,4 +48,6 @@ class Renderer(if_nerf_renderer.Renderer):
         H, W = int(cfg.H * cfg.ratio), int(cfg.W * cfg.ratio)
         if tuple(batch['msks'].shape[-2:]) != (H, W):
             raise ValueError("batch['msks'] is %s but cfg.H*ratio x cfg.W*ratio = %dx%d" % (tuple(batch['msks'].shape), H, W))
+        if int(self._opt("render_importance", 0)) > 0:
+            return self.render_rays_hierarchical(ray_o, ray_d, near, far, feature_volume, sp_input, masks=batch)
         return self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, masks=batch)

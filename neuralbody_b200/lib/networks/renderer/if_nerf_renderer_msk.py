@@ -38,7 +38,8 @@ class Renderer(if_nerf_renderer_mmsk.Renderer):
 
     def get_pixel_value(self, ray_o, ray_d, near, far, feature_volume, sp_input, batch):
         """if_clight_renderer_mmsk.py:63-94 with the single-view predicate above.  A batch of 'device' items carries the
-        decoded view (`msks_u8`) in place of `msk`: mask_views builds it on the device first."""
+        decoded view (`msks_u8`) in place of `msk`: mask_views builds it on the device first.  With `cfg.render_importance > 0`
+        both passes of `render_rays_hierarchical` take the view, the snapshot transform included."""
         if 'msk' not in batch and 'msks_u8' in batch:
             self.mask_views(batch)
         for k in ('R0_snap', 'Th0_snap', 'RT', 'K', 'msk'):
@@ -51,4 +52,6 @@ class Renderer(if_nerf_renderer_mmsk.Renderer):
             raise ValueError("batch['msk'] is %s but cfg.H*ratio x cfg.W*ratio = %dx%d" % (tuple(batch['msk'].shape), H, W))
         masks = {"msks": batch['msk'][:, None], "RT": batch['RT'][:, None], "Ks": batch['K'][:, None],
                  "R0_snap": batch['R0_snap'], "Th0_snap": batch['Th0_snap']}
+        if int(self._opt("render_importance", 0)) > 0:
+            return self.render_rays_hierarchical(ray_o, ray_d, near, far, feature_volume, sp_input, masks=masks)
         return self.render_rays(ray_o, ray_d, near, far, feature_volume, sp_input, masks=masks)
