@@ -588,6 +588,58 @@ size_t nb_image_loss_workspace_bytes(void);
 int nb_image_loss_fwd(const nb_image_loss_args* a, void* stream);
 int nb_image_loss_bwd(const nb_image_loss_args* a, const float* d_loss, float* d_pred, void* stream);
 
+/* The reference's SparseConvNet encode (lib/networks/latent_xyzc.py:30-39,166-274; spconv 1.2.1 semantics, restated in
+ * oracle/spconv_oracle.py) as sparse convolutions over the active sites, forward and backward (opt-in from Python:
+ * `sparse_encode: 'cuda'`).  17 layers in the reference's order (conv0 x2, down0, conv1 x2, down1, conv2 x3, down2, conv3
+ * x3, down3, conv4 x3), each SubMConv3d(k=3) or SparseConv3d(k=3, s=2, p=1) without bias, then BatchNorm1d over the active
+ * rows and ReLU; the outputs of layers 4, 8, 12 and 16 are net1..net4.
+ *   - input: point i sits at coord[i] = (b, z, y, x) with feature code[i % n_vert]; several points on one site: the highest
+ *     index wins; a point outside [0, batch) x out_sh is ignored.  Strided output extent floor((in - 1) / 2) + 1 per axis;
+ *     a site is active iff its 3x3x3 window holds an active input.
+ *   - BatchNorm: training = 1 normalises with the batch statistics (biased variance), then updates running_mean /
+ *     running_var (unbiased) with `momentum` and adds 1 to num_batches_tracked; training = 0 uses the running statistics.
+ *   - volumes[l]: (batch, C_l, D_l, H_l, W_l) fp32 with C = 32, 64, 128, 128 and the extents of strided levels 1..4; written
+ *     whole, exact 0 off the active set.
+ * fp32 FFMA arithmetic, float64 BatchNorm sums.  The row counts never leave the device: buffers are sized from bounds
+ * (level 0 <= n_points, level l+1 <= min(8 x level l, B D_l H_l W_l)) in the workspace, whose size depends on
+ * (batch, n_points, out_sh) only.  nb_spconv_bwd takes the same arguments and the workspace the forward call filled,
+ * unchanged, and the cotangents of the four volumes; it WRITES every gradient (d_code, the conv weights, the BatchNorm
+ * weights and biases); weight and BatchNorm sums use atomics, so the gradients are not bit-reproducible.  Validation (null
+ * pointers, batch, n_points, n_vert, out_sh, training, eps, momentum, workspace) happens before anything is enqueued;
+ * nothing allocates or synchronises with the host. */
+#define NB_SPCONV_LAYERS 17
+#define NB_SPCONV_CODE_DIM 16           /* the code embedding's width, c = nn.Embedding(6890, 16) */
+typedef struct nb_spconv_args {
+    int batch;                          /* B frames */
+    int n_points;                       /* rows of coord (B * 6890 upstream) */
+    int n_vert;                         /* rows of code (6890) */
+    int out_sh[3];                      /* D, H, W of the input grid */
+    const int* coord;                   /* device (n_points, 4) int32 (b, z, y, x) */
+    const float* code;                  /* device (n_vert, 16) */
+    const float* weight[NB_SPCONV_LAYERS];        /* device (3, 3, 3, Cin, Cout) each, spconv's layout */
+    const float* bn_weight[NB_SPCONV_LAYERS];     /* device (Cout) */
+    const float* bn_bias[NB_SPCONV_LAYERS];       /* device (Cout) */
+    float* running_mean[NB_SPCONV_LAYERS];        /* device (Cout); updated when training */
+    float* running_var[NB_SPCONV_LAYERS];         /* device (Cout); updated when training */
+    long long* num_batches_tracked[NB_SPCONV_LAYERS];   /* device scalar; training only (may be NULL otherwise) */
+    int training;                       /* 1: batch statistics, 0: running statistics */
+    float momentum, eps;                /* BatchNorm1d(eps=1e-3, momentum=0.01) upstream */
+    void* workspace;                    /* device, 256-byte aligned, nb_spconv_workspace_bytes() */
+    size_t workspace_bytes;
+    float* volumes[NB_NUM_LEVELS];      /* device, written */
+    int* row_counts;                    /* device int32[5] or NULL: active sites of the input grid and of levels 1..4 */
+} nb_spconv_args;
+typedef struct nb_spconv_grads {
+    const float* d_volumes[NB_NUM_LEVELS];        /* device, shaped as volumes; NULL = zero cotangent */
+    float* d_code;                                /* device (n_vert, 16), written */
+    float* d_weight[NB_SPCONV_LAYERS];            /* device, shaped as weight, written */
+    float* d_bn_weight[NB_SPCONV_LAYERS];         /* device (Cout), written */
+    float* d_bn_bias[NB_SPCONV_LAYERS];           /* device (Cout), written */
+} nb_spconv_grads;
+size_t nb_spconv_workspace_bytes(int batch, int n_points, const int out_sh[3]);   /* 0 for an invalid size */
+int nb_spconv_fwd(const nb_spconv_args* a, void* stream);
+int nb_spconv_bwd(const nb_spconv_args* a, const nb_spconv_grads* g, void* stream);
+
 /* number of kernels nb_render_fwd enqueues per FRAME of a call: 1 for NB_PRECISION_FP32 (the single fused exact kernel),
  * 3 for the tensor-core inference precisions (classify, decoder, composite; plus one 32-byte memset per call), 9 for
  * NB_PRECISION_TC_TF32X3 (colour-matrix build, classify, gather, 4 GEMMs, rgb head, composite). */

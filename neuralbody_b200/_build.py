@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(HERE, "libneuralbody_b200.so")
 SOURCES = ["nb_capi.cu", "nb_render_f32.cu", "nb_render_tc_list.cu", "nb_render_bwd.cu", "nb_train.cu", "nb_sample_pdf.cu",
            "nb_mcubes.cu", "nb_mesh_inside_f64.cu", "nb_image_rays.cu", "nb_image_rays_f64.cu",
            "nb_train_rays.cu", "nb_item_images.cu", "nb_mask_views.cu", "nb_eval_image.cu", "nb_vis_frame.cu", "nb_mesh_ply.cu",
-           "nb_image_loss.cu"]
+           "nb_image_loss.cu", "nb_spconv.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 OBJ_DIR = os.path.join(HERE, "build")
 

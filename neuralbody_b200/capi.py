@@ -23,7 +23,8 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_mask_views_workspace_bytes",
            "nb_mask_views", "nb_eval_image_workspace_bytes",
            "nb_eval_image", "nb_vis_frame_workspace_bytes", "nb_vis_frame", "nb_mesh_ply_bytes", "nb_mesh_ply",
-           "nb_image_loss_workspace_bytes", "nb_image_loss_fwd", "nb_image_loss_bwd"]
+           "nb_image_loss_workspace_bytes", "nb_image_loss_fwd", "nb_image_loss_bwd", "nb_spconv_workspace_bytes",
+           "nb_spconv_fwd", "nb_spconv_bwd"]
 
 
 class nb_volume_level(C.Structure):
@@ -161,6 +162,24 @@ class nb_mesh_ply_args(C.Structure):
 class nb_image_loss_args(C.Structure):
     _fields_ = [("rays", C.c_int), ("pred", C.c_void_p), ("gt", C.c_void_p), ("mask", C.c_void_p), ("workspace", C.c_void_p),
                 ("workspace_bytes", C.c_size_t), ("loss", C.c_void_p), ("count", C.c_void_p)]
+
+
+NB_SPCONV_LAYERS = 17
+_SpLayers = C.c_void_p * NB_SPCONV_LAYERS
+
+
+class nb_spconv_args(C.Structure):
+    _fields_ = [("batch", C.c_int), ("n_points", C.c_int), ("n_vert", C.c_int), ("out_sh", C.c_int * 3),
+                ("coord", C.c_void_p), ("code", C.c_void_p), ("weight", _SpLayers), ("bn_weight", _SpLayers),
+                ("bn_bias", _SpLayers), ("running_mean", _SpLayers), ("running_var", _SpLayers),
+                ("num_batches_tracked", _SpLayers), ("training", C.c_int), ("momentum", C.c_float), ("eps", C.c_float),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("volumes", C.c_void_p * NB_NUM_LEVELS),
+                ("row_counts", C.c_void_p)]
+
+
+class nb_spconv_grads(C.Structure):
+    _fields_ = [("d_volumes", C.c_void_p * NB_NUM_LEVELS), ("d_code", C.c_void_p), ("d_weight", _SpLayers),
+                ("d_bn_weight", _SpLayers), ("d_bn_bias", _SpLayers)]
 
 
 class nb_image_rays_args(C.Structure):
@@ -303,6 +322,12 @@ def load(path=None):
     lib.nb_image_loss_fwd.argtypes = [C.POINTER(nb_image_loss_args), C.c_void_p]
     lib.nb_image_loss_bwd.restype = C.c_int
     lib.nb_image_loss_bwd.argtypes = [C.POINTER(nb_image_loss_args), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.nb_spconv_workspace_bytes.restype = C.c_size_t
+    lib.nb_spconv_workspace_bytes.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_int)]
+    lib.nb_spconv_fwd.restype = C.c_int
+    lib.nb_spconv_fwd.argtypes = [C.POINTER(nb_spconv_args), C.c_void_p]
+    lib.nb_spconv_bwd.restype = C.c_int
+    lib.nb_spconv_bwd.argtypes = [C.POINTER(nb_spconv_args), C.POINTER(nb_spconv_grads), C.c_void_p]
     if lib.nb_abi_version() != 5:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):

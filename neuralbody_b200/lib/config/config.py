@@ -122,6 +122,8 @@ def _defaults():
     c.mesh_th = 50                      # isovalue of the mesh renderer's marching cubes, on raw sigma (config.py:45)
     c.mesh_output = 'host'              # the mesh renderer's outputs: 'host' (upstream's float64 numpy cube and host mesh) |
                                         # 'device' (the fp32 CUDA cube and a mcubes.DeviceMesh, nothing copied back)
+    c.sparse_encode = 'reference'       # the SparseConvNet encode: 'reference' (upstream's spconv module) | 'dense' (the
+                                        # dense-PyTorch emulation) | 'cuda' (sparse convolutions on the GPU, nb_spconv)
     # H100 renderer options (new)
     c.render_precision = "tc_fp16x3"    # "fp32" exact FFMA kernel | "tc_fp16x3" wgmma, 3-pass hi/lo density path
                                         # (meets the 1e-3 parity gate) | "tc_fp16" wgmma 1-pass (fastest, ~4e-3 on depth)

@@ -4,11 +4,14 @@
 (`fc_0.weight (256,352,1)` ... `rgb_fc.weight (3,128,1)`, `latent.weight`, `c.weight`),
 so reference checkpoints load with `load_state_dict(..., strict=False)`.
 
-What is NOT here, by the scope contract (SURVEY.md 8, north star): the SparseConvNet
-encode (`xyzc_net`, latent_xyzc.py:166-274) stays on the reference path.  Attach the
-reference's own module as `net.xyzc_net` when spconv is installed, hand the dense
-volumes in with `set_feature_volume()` (what the synthetic scenes do), or opt into the
-dense-PyTorch emulation with `attach_dense_encoder()` (f-2(ii), parity unpinned).
+The SparseConvNet encode (`xyzc_net`, latent_xyzc.py:166-274) stays on the reference path by
+default (SURVEY.md 8): attach the reference's own module as `net.xyzc_net` when spconv is
+installed, or hand the dense volumes in with `set_feature_volume()` (what the synthetic scenes
+do).  Two opt-in encoders need no spconv, selected by the yaml key `sparse_encode` when the
+network is built ('reference' (default) | 'dense' | 'cuda') or from Python: the dense-PyTorch
+emulation (`attach_dense_encoder()`, f-2(ii), parity unpinned) and the sparse CUDA
+convolutions (`attach_cuda_encoder()`, csrc/nb_spconv.cu), both with the reference module's
+parameter names.
 
 The decoder arithmetic itself (`calculate_density_color`, :91-126) is not evaluated by
 PyTorch modules here: the Renderer packs these parameters and runs the fused CUDA kernel.
@@ -38,6 +41,13 @@ class Network(nn.Module):
         self.view_fc = nn.Conv1d(346, 128, 1)
         self.rgb_fc = nn.Conv1d(128, 3, 1)
         self._feature_volume = None
+        encoder = cfg.get('sparse_encode', 'reference') if hasattr(cfg, 'get') else getattr(cfg, 'sparse_encode', 'reference')
+        if encoder == 'dense':
+            self.attach_dense_encoder()
+        elif encoder == 'cuda':
+            self.attach_cuda_encoder()
+        elif encoder != 'reference':
+            raise ValueError("sparse_encode must be 'reference', 'dense' or 'cuda' (got %r)" % (encoder,))
 
     # ---- encode: reference path or supplied volumes
     def set_feature_volume(self, volumes):
@@ -52,11 +62,18 @@ class Network(nn.Module):
         self.xyzc_net = DenseSparseConvNet().to(self.c.weight.device)
         return self.xyzc_net
 
+    def attach_cuda_encoder(self):
+        """Opt-in: run the encode as sparse convolutions on the GPU (lib/networks/sparse_encode_cuda.py, nb_spconv_fwd /
+        nb_spconv_bwd), forward and backward; the same parameter names as the emulation and the reference module."""
+        from neuralbody_b200.lib.networks.sparse_encode_cuda import CudaSparseConvNet
+        self.xyzc_net = CudaSparseConvNet().to(self.c.weight.device)
+        return self.xyzc_net
+
     def encode_sparse_voxels(self, sp_input):
         """latent_xyzc.py:30-39."""
         if self._feature_volume is not None:
             return self._feature_volume
-        if type(self.xyzc_net).__name__ == "DenseSparseConvNet":
+        if type(self.xyzc_net).__name__ in ("DenseSparseConvNet", "CudaSparseConvNet"):
             coord = sp_input['coord']
             code = self.c(torch.arange(0, 6890).to(coord.device))
             return self.xyzc_net.encode(code, coord, sp_input['out_sh'], sp_input['batch_size'])

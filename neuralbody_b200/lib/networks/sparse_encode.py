@@ -1,6 +1,8 @@
 """f-2(ii): dense-PyTorch emulation of the reference's SparseConvNet encode (lib/networks/latent_xyzc.py:30-39,166-274),
-for machines without spconv -- OPT-IN (`Network.attach_dense_encoder()`); by the scope contract the encode stays on the
-reference's spconv path and this package's hot path starts at the four dense volumes it returns.
+for machines without spconv -- OPT-IN (`Network.attach_dense_encoder()` or `sparse_encode: 'dense'`); by default the encode
+stays on the reference's spconv path and this package's hot path starts at the four dense volumes it returns.  The same
+encode runs as sparse convolutions on the GPU in CudaSparseConvNet (sparse_encode_cuda.py, `sparse_encode: 'cuda'`,
+also opt-in), which is tested against this module in float64.
 
 PARITY UNPINNED: spconv 1.2.1 (commit abf0acf, INSTALL.md:14-22) is not in this image, so this module cannot be checked
 against it.  It follows spconv's published semantics, restated independently as a brute-force sparse oracle in
