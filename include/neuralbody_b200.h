@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NB_ABI_VERSION 5
+#define NB_ABI_VERSION 6
 
 #define NB_OK               0
 #define NB_ERR_BAD_ARG     (-1)
@@ -275,30 +275,6 @@ int nb_mesh_inside(const nb_mesh_inside_args* a, void* stream);
  * clipped.  The view loop and `inside` are nb_mesh_inside's.  Validated as nb_mesh_inside, before anything is enqueued. */
 int nb_mesh_inside_f64(const nb_mesh_inside_args* a, const double* RT, const double* Ks, void* stream);
 
-/* f-2: ray generation on the device.  Replaces the per-view numpy of get_rays (lib/utils/if_nerf/if_nerf_data_utils.py:8-21)
- * and get_near_far (:54-69) as called from image_rays (lib/utils/render_utils.py:120-137): fp64 arithmetic like upstream, fp32
- * results.  Writes ALL H*W pixels (row-major) plus mask_at_box; the caller compacts with the mask (upstream: ray_o[mask_at_box]).
- * K_inv, R, T: the view's inverse intrinsics / world->camera rotation / translation (host memory, row-major doubles);
- * bounds: host (2,3) doubles, the world box (can_bounds). */
-typedef struct nb_camera {
-    double K_inv[9];
-    double R[9];
-    double T[3];
-    double bounds[6];
-    int H, W;
-} nb_camera;
-int nb_gen_rays(const nb_camera* cam, float* ray_o /* device (H*W,3) */, float* ray_d /* device (H*W,3) */,
-                float* near /* device (H*W) */, float* far /* device (H*W) */, unsigned char* mask_at_box /* device (H*W) */,
-                void* stream);
-/* Same arithmetic for ONE RANK'S SHARD of a ray-sharded render (SURVEY 8e): pixel chunk c (of `chunk` consecutive pixels)
- * belongs to rank c % world; local ray j of rank `rank` is pixel ((j / chunk) * world + rank) * chunk + j % chunk.  Writes
- * n_local rays with a FIXED shape (no mask compaction, so nothing synchronises with the host): a ray that misses the box --
- * upstream drops it, image_rays :131-132 -- or lies past the last pixel becomes a dead ray (near = far = 0: every sample
- * sits at the camera centre, outside the volume, and is skipped) with mask_at_box = 0. */
-int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, int n_local,
-                        float* ray_o /* device (n_local,3) */, float* ray_d, float* near, float* far,
-                        unsigned char* mask_at_box /* device (n_local) */, void* stream);
-
 /* The demo datasets' per-view rays (render_utils.image_rays, lib/utils/render_utils.py:120-137, as called by
  * multi_view_demo_dataset.py:151, multi_view_perform_dataset.py:148 and monocular_demo_dataset.py:113) on the device, bit for
  * bit: get_rays (if_nerf_data_utils.py:8-21) in the camera's scalar type with the product and sum order numpy's BLAS uses
@@ -310,7 +286,15 @@ int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, in
  * Writes mask_at_box (H*W) and the first n entries of ray_o / ray_d (n,3) and near / far (n), n = the number of pixels whose
  * ray enters the box, and n itself to `count` (device int32).  The caller reads count once (the one host synchronisation:
  * upstream's n varies per view).  Validation (null pointers, H, W >= 1, H*W < 2^31, workspace size) happens before anything is
- * enqueued; three launches (the box test, a CUB scan, the compacting write). */
+ * enqueued; three launches (the box test, a CUB scan, the compacting write).
+ * Shard mode (world >= 1): ONE RANK'S SHARD of a ray-sharded render (SURVEY 8e) in one launch, with a FIXED shape, so nothing
+ * synchronises with the host.  Pixel chunk c (of `chunk` consecutive pixels) belongs to rank c % world; local ray j < n_local
+ * is pixel ((j / chunk) * world + rank) * chunk + j % chunk, and its ray_o, ray_d, near, far and mask_at_box are the bits the
+ * compacting call writes for that pixel.  A ray that misses the box (upstream drops it, image_rays :131-132) keeps ray_o /
+ * ray_d with near = far = 0; a slot past the last pixel is o = 0, d = (0, 0, 1), near = far = 0.  Both are dead rays (every
+ * sample sits at the camera centre, outside the volume, and is skipped) with mask_at_box = 0.  ray_o / ray_d (n_local,3),
+ * near / far / mask_at_box (n_local); workspace and count are not read; image and rgb must be NULL.  rank in [0, world),
+ * chunk >= 1 and n_local >= 0 are validated with the rest before anything is enqueued; n_local = 0 enqueues nothing. */
 typedef struct nb_image_rays_args {
     int H, W;
     float bounds[6];             /* can_bounds (2,3): world box min, max */
@@ -327,6 +311,7 @@ typedef struct nb_image_rays_args {
     float* rgb;                  /* device, room for H*W (n,3); set with image */
     int k_f32;                   /* nb_image_rays_f64 only, nonzero: K is float32 (K_inv's values are float32's and
                                     xy1 @ inv(K).T runs in float32, as for People-Snapshot's get_camera R and T) */
+    int rank, world, chunk, n_local;  /* world = 0: the compacting call; world >= 1: shard mode (above) */
 } nb_image_rays_args;
 size_t nb_image_rays_workspace_bytes(int H, int W);   /* 0 for an invalid size */
 /* float32 camera (monocular_demo_dataset.py:109-112: RT and K cast to float32) */

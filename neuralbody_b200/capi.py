@@ -17,7 +17,7 @@ EXPORTS = ["nb_abi_version", "nb_last_error", "nb_has_precision", "nb_packed_vol
            "nb_render_bwd_maps", "nb_render_bwd_inputs", "nb_render_save_bytes",
            "nb_render_bwd_workspace_bytes", "nb_render_save_bytes_for", "nb_render_bwd_workspace_bytes_for", "nb_debug_gemm_tf32x3", "nb_debug_composite",
            "nb_debug_composite_bwd", "nb_decode_density", "nb_decode_density_workspace_bytes",
-           "nb_decode_density_list", "nb_gen_rays", "nb_gen_rays_sharded", "nb_sample_pdf", "nb_sample_pdf_src",
+           "nb_decode_density_list", "nb_sample_pdf", "nb_sample_pdf_src",
            "nb_mcubes_workspace_bytes", "nb_mcubes_count", "nb_mcubes_emit", "nb_mesh_inside",
            "nb_mesh_inside_f64", "nb_image_rays_workspace_bytes", "nb_image_rays", "nb_image_rays_f64",
            "nb_train_rays_workspace_bytes", "nb_train_rays", "nb_item_images", "nb_mask_views_workspace_bytes",
@@ -36,11 +36,6 @@ class nb_decoder_weights(C.Structure):
         "fc0_w", "fc0_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "alpha_w", "alpha_b", "feature_w", "feature_b",
         "latent_w", "latent_b", "view_w", "view_b", "rgb_w", "rgb_b", "latent", "latent_index")] + \
         [("num_train_frame", C.c_int), ("batch", C.c_int)]
-
-
-class nb_camera(C.Structure):
-    _fields_ = [("K_inv", C.c_double * 9), ("R", C.c_double * 9), ("T", C.c_double * 3), ("bounds", C.c_double * 6),
-                ("H", C.c_int), ("W", C.c_int)]
 
 
 LevelDims = (C.c_int * 4) * NB_NUM_LEVELS
@@ -186,7 +181,8 @@ class nb_image_rays_args(C.Structure):
     _fields_ = [("H", C.c_int), ("W", C.c_int), ("bounds", C.c_float * 6), ("workspace", C.c_void_p),
                 ("workspace_bytes", C.c_size_t), ("ray_o", C.c_void_p), ("ray_d", C.c_void_p), ("near", C.c_void_p),
                 ("far", C.c_void_p), ("mask_at_box", C.c_void_p), ("count", C.c_void_p), ("image", C.c_void_p),
-                ("rgb", C.c_void_p), ("k_f32", C.c_int)]
+                ("rgb", C.c_void_p), ("k_f32", C.c_int), ("rank", C.c_int), ("world", C.c_int), ("chunk", C.c_int),
+                ("n_local", C.c_int)]
 
 
 class nb_render_bwd_args(C.Structure):
@@ -270,10 +266,6 @@ def load(path=None):
     lib.nb_decode_density_workspace_bytes.argtypes = [C.c_int, C.c_int]
     lib.nb_decode_density_list.restype = C.c_int
     lib.nb_decode_density_list.argtypes = [C.POINTER(nb_render_args), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.nb_gen_rays.restype = C.c_int
-    lib.nb_gen_rays.argtypes = [C.POINTER(nb_camera)] + [C.c_void_p] * 6
-    lib.nb_gen_rays_sharded.restype = C.c_int
-    lib.nb_gen_rays_sharded.argtypes = [C.POINTER(nb_camera)] + [C.c_int] * 4 + [C.c_void_p] * 6
     lib.nb_sample_pdf.restype = C.c_int
     lib.nb_sample_pdf.argtypes = [C.POINTER(nb_importance_args), C.c_void_p]
     lib.nb_sample_pdf_src.restype = C.c_int
@@ -328,7 +320,7 @@ def load(path=None):
     lib.nb_spconv_fwd.argtypes = [C.POINTER(nb_spconv_args), C.c_void_p]
     lib.nb_spconv_bwd.restype = C.c_int
     lib.nb_spconv_bwd.argtypes = [C.POINTER(nb_spconv_args), C.POINTER(nb_spconv_grads), C.c_void_p]
-    if lib.nb_abi_version() != 5:
+    if lib.nb_abi_version() != 6:
         raise RuntimeError("libneuralbody_b200.so ABI version mismatch")
     if path in (_build.LIB_PATH, os.environ.get("NB_LIB_PATH")):
         _lib = lib

@@ -194,64 +194,6 @@ __global__ void sigma_empty_kernel(nb_decoder_weights w, float* __restrict__ f32
     }
 }
 
-// f-2: get_rays + get_near_far (if_nerf_data_utils.py:8-21, 54-69), one thread per pixel, fp64 like the numpy original.
-__device__ __forceinline__ bool gen_ray(const nb_camera& cam, int pix, float (&of)[3], float (&df)[3], float& near, float& far) {
-    const double i = (double)(float)(pix % cam.W), j = (double)(float)(pix / cam.W);   // np.arange(..., dtype=float32)
-    // rays_o = -R^T T
-    double o[3], pc[3], pw[3], d[3];
-    for (int a = 0; a < 3; ++a) o[a] = -(cam.R[0 * 3 + a] * cam.T[0] + cam.R[1 * 3 + a] * cam.T[1] + cam.R[2 * 3 + a] * cam.T[2]);
-    // pixel_camera = xy1 @ K_inv^T ; pixel_world = (pixel_camera - T) @ R
-    for (int a = 0; a < 3; ++a) pc[a] = i * cam.K_inv[a * 3 + 0] + j * cam.K_inv[a * 3 + 1] + cam.K_inv[a * 3 + 2] - cam.T[a];
-    for (int a = 0; a < 3; ++a) pw[a] = pc[0] * cam.R[0 * 3 + a] + pc[1] * cam.R[1 * 3 + a] + pc[2] * cam.R[2 * 3 + a];
-    for (int a = 0; a < 3; ++a) d[a] = pw[a] - o[a];
-    // the dataset casts to float32 BEFORE get_near_far (multi_view_demo_dataset.py / image_rays: ray_o.astype(np.float32))
-    for (int a = 0; a < 3; ++a) { of[a] = (float)o[a]; df[a] = (float)d[a]; }
-    const float nrm = ray_norm(df[0], df[1], df[2]);
-    float tnear = -INFINITY, tfar = INFINITY;
-    for (int a = 0; a < 3; ++a) {
-        float v = __fdiv_rn(df[a], nrm);
-        if (v < 1e-5f && v > -1e-10f) v = 1e-5f;
-        if (v > -1e-5f && v < 1e-10f) v = -1e-5f;
-        const float t0 = __fdiv_rn(__fsub_rn((float)cam.bounds[a], of[a]), v), t1 = __fdiv_rn(__fsub_rn((float)cam.bounds[3 + a], of[a]), v);
-        tnear = fmaxf(tnear, fminf(t0, t1));
-        tfar = fminf(tfar, fmaxf(t0, t1));
-    }
-    near = __fdiv_rn(tnear, nrm);
-    far = __fdiv_rn(tfar, nrm);
-    return tnear < tfar;
-}
-
-__global__ void gen_rays_kernel(nb_camera cam, float* __restrict__ ray_o, float* __restrict__ ray_d, float* __restrict__ near,
-                                float* __restrict__ far, unsigned char* __restrict__ mask) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= cam.H * cam.W) return;
-    float of[3], df[3], tn, tf;
-    const bool hit = gen_ray(cam, idx, of, df, tn, tf);
-    for (int a = 0; a < 3; ++a) { ray_o[idx * 3 + a] = of[a]; ray_d[idx * 3 + a] = df[a]; }
-    near[idx] = tn;
-    far[idx] = tf;
-    mask[idx] = hit ? 1 : 0;
-}
-
-// one rank's interleaved shard, fixed shape: misses and pixels past the image become dead rays (near = far = 0)
-__global__ void gen_rays_sharded_kernel(nb_camera cam, int rank, int world, int chunk, int n_local, float* __restrict__ ray_o,
-                                        float* __restrict__ ray_d, float* __restrict__ near, float* __restrict__ far,
-                                        unsigned char* __restrict__ mask) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n_local) return;
-    const long long pix = ((long long)(j / chunk) * world + rank) * chunk + j % chunk;
-    float of[3] = {0.f, 0.f, 0.f}, df[3] = {0.f, 0.f, 1.f}, tn = 0.f, tf = 0.f;
-    bool hit = false;
-    if (pix < (long long)cam.H * cam.W) {
-        hit = gen_ray(cam, (int)pix, of, df, tn, tf);
-        if (!hit) tn = tf = 0.f;
-    }
-    for (int a = 0; a < 3; ++a) { ray_o[j * 3 + a] = of[a]; ray_d[j * 3 + a] = df[a]; }
-    near[j] = tn;
-    far[j] = tf;
-    mask[j] = hit ? 1 : 0;
-}
-
 // fp16 split of an fp32 value: hi = fp16(x), lo = fp16(x - hi): hi + lo carries ~21 mantissa bits.
 __device__ __forceinline__ __half f16_hi(float x) { return __float2half_rn(x); }
 __device__ __forceinline__ __half f16_lo(float x) { return __float2half_rn(x - __half2float(__float2half_rn(x))); }
@@ -496,33 +438,6 @@ int fill_ray_params(const nb_render_args* a, const char* who, RenderParams* out)
 }  // namespace nb
 
 extern "C" {
-
-int nb_gen_rays(const nb_camera* cam, float* ray_o, float* ray_d, float* near, float* far, unsigned char* mask_at_box, void* stream) {
-    if (!cam || !ray_o || !ray_d || !near || !far || !mask_at_box || cam->H <= 0 || cam->W <= 0) {
-        set_error("nb_gen_rays: null argument or empty image");
-        return NB_ERR_BAD_ARG;
-    }
-    const int n = cam->H * cam->W;
-    gen_rays_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*cam, ray_o, ray_d, near, far, mask_at_box);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("nb_gen_rays: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    return NB_OK;
-}
-
-int nb_gen_rays_sharded(const nb_camera* cam, int rank, int world, int chunk, int n_local, float* ray_o, float* ray_d, float* near,
-                        float* far, unsigned char* mask_at_box, void* stream) {
-    if (!cam || !ray_o || !ray_d || !near || !far || !mask_at_box || cam->H <= 0 || cam->W <= 0 || world <= 0 || rank < 0 ||
-        rank >= world || chunk <= 0 || n_local < 0) {
-        set_error("nb_gen_rays_sharded: null argument, empty image or bad rank / world / chunk");
-        return NB_ERR_BAD_ARG;
-    }
-    if (n_local == 0) return NB_OK;
-    gen_rays_sharded_kernel<<<(n_local + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*cam, rank, world, chunk, n_local, ray_o, ray_d,
-                                                                                      near, far, mask_at_box);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("nb_gen_rays_sharded: %s", cudaGetErrorString(e)); return NB_ERR_CUDA; }
-    return NB_OK;
-}
 
 int nb_decode_density(const nb_render_args* a, const float* points, int n_points, float* sigma, void* stream) {
     if (!a || !points || !sigma || n_points < 0) { set_error("nb_decode_density: null argument"); return NB_ERR_BAD_ARG; }

@@ -3,7 +3,8 @@
 // the pixels (numpy 2.3 / OpenBLAS 0.3.30; tools/demo_case.py spells them out and tests/golden/demo_*.npz pin them), then
 // get_near_far in float32.  No expression here may be contracted: every product and sum is an explicit _rn intrinsic.
 // The kernels are instantiated over the camera's scalar type: float in nb_image_rays.cu, double in nb_image_rays_f64.cu,
-// one instance per object.  nb_gen_rays / nb_gen_rays_sharded (nb_capi.cu) do not use this file.
+// one instance per object.  The same image_ray writes the compacted view (mask, scan, emit) and one rank's fixed-shape shard
+// of it (shard mode), and nb_train_rays shares its camera_ray_d.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -121,6 +122,29 @@ __global__ void __launch_bounds__(kRayThreads) image_rays_emit_kernel(const __gr
         for (int a = 0; a < 3; ++a) rgb[(size_t)q * 3 + a] = image[(size_t)p * 3 + a];
 }
 
+// shard mode: local ray j of rank `rank` is pixel ((j / chunk) * world + rank) * chunk + j % chunk.  A miss keeps its ray with
+// near = far = 0, a slot past the last pixel is o = 0, d = (0, 0, 1), near = far = 0; both have mask 0.
+template <typename TK, typename TR>
+__global__ void __launch_bounds__(kRayThreads) image_rays_shard_kernel(const __grid_constant__ ImageCam<TK, TR> c, int rank,
+                                                                       int world, int chunk, int n_local,
+                                                                       float* __restrict__ ray_o, float* __restrict__ ray_d,
+                                                                       float* __restrict__ near, float* __restrict__ far,
+                                                                       unsigned char* __restrict__ mask) {
+    const unsigned j = blockIdx.x * kRayThreads + threadIdx.x;     // n_local < 2^31: no unsigned wrap in the last block
+    if (j >= (unsigned)n_local) return;
+    const long long pix = ((long long)(j / (unsigned)chunk) * world + rank) * chunk + j % (unsigned)chunk;
+    float of[3] = {0.f, 0.f, 0.f}, df[3] = {0.f, 0.f, 1.f}, tn = 0.f, tf = 0.f;
+    bool hit = false;
+    if (pix < (long long)c.H * c.W) {
+        hit = image_ray(c, (int)pix, of, df, tn, tf);
+        if (!hit) tn = tf = 0.f;
+    }
+    for (int a = 0; a < 3; ++a) { ray_o[(size_t)j * 3 + a] = of[a]; ray_d[(size_t)j * 3 + a] = df[a]; }
+    near[j] = tn;
+    far[j] = tf;
+    mask[j] = hit ? 1 : 0;
+}
+
 // bit `shift` of a per-pixel byte map (mask_at_box: bit 0; the training sampler's class map: bits 0-2)
 struct MaskBit {
     int shift;
@@ -149,13 +173,23 @@ inline int image_rays_pixels(int H, int W) {   // H*W, or -1 when it is not in [
 template <typename TK, typename TR>
 int image_rays_launch(const char* who, const nb_image_rays_args* a, const TR* K_inv, const TR* R, const TR* Tv, const TR* o,
                       void* stream) {
-    if (!a || !K_inv || !R || !Tv || !o || !a->workspace || !a->ray_o || !a->ray_d || !a->near || !a->far ||
-        !a->mask_at_box || !a->count) {
+    const bool shard = a && a->world != 0;
+    if (!a || !K_inv || !R || !Tv || !o || !a->ray_o || !a->ray_d || !a->near || !a->far || !a->mask_at_box ||
+        (!shard && (!a->workspace || !a->count))) {
         set_error("%s: null argument", who);
+        return NB_ERR_BAD_ARG;
+    }
+    if (shard && (a->image || a->rgb)) {
+        set_error("%s: image and rgb must be NULL in shard mode", who);
         return NB_ERR_BAD_ARG;
     }
     if (!a->image != !a->rgb) {
         set_error("%s: image and rgb must both be set or both be NULL", who);
+        return NB_ERR_BAD_ARG;
+    }
+    if (shard && (a->rank < 0 || a->rank >= a->world || a->chunk < 1 || a->n_local < 0)) {
+        set_error("%s: shard mode needs 0 <= rank < world, chunk >= 1 and n_local >= 0 (got rank %d, world %d, chunk %d, "
+                  "n_local %d)", who, a->rank, a->world, a->chunk, a->n_local);
         return NB_ERR_BAD_ARG;
     }
     const int n = image_rays_pixels(a->H, a->W);
@@ -163,22 +197,31 @@ int image_rays_launch(const char* who, const nb_image_rays_args* a, const TR* K_
         set_error("%s: H and W must be >= 1 with H*W < 2^31 (got %d x %d)", who, a->H, a->W);
         return NB_ERR_BAD_ARG;
     }
-    const size_t need = nb_image_rays_workspace_bytes(a->H, a->W);
-    if (need == 0 || a->workspace_bytes < need) {
+    const size_t need = shard ? 0 : nb_image_rays_workspace_bytes(a->H, a->W);   // shard mode has no workspace
+    if (!shard && (need == 0 || a->workspace_bytes < need)) {
         set_error("%s: workspace_bytes too small (%zu < %zu)", who, a->workspace_bytes, need);
         return NB_ERR_BAD_ARG;
     }
+    if (shard && a->n_local == 0) return NB_OK;
     ImageCam<TK, TR> c;
     for (int k = 0; k < 9; ++k) { c.K_inv[k] = (TK)K_inv[k]; c.R[k] = R[k]; }
     for (int k = 0; k < 3; ++k) { c.T_[k] = Tv[k]; c.o[k] = o[k]; }
     for (int k = 0; k < 6; ++k) c.bounds[k] = a->bounds[k];
     c.H = a->H; c.W = a->W;
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (shard) {
+        const unsigned blocks = (unsigned)(((long long)a->n_local + kRayThreads - 1) / kRayThreads);
+        image_rays_shard_kernel<TK, TR><<<blocks, kRayThreads, 0, s>>>(c, a->rank, a->world, a->chunk, a->n_local, a->ray_o,
+                                                                       a->ray_d, a->near, a->far, a->mask_at_box);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); return NB_ERR_CUDA; }
+        return NB_OK;
+    }
     unsigned char* ws = (unsigned char*)a->workspace;
     int* offset = (int*)ws;
     const size_t scratch = align256((size_t)n * sizeof(int));
     size_t sb = need - scratch;
     const unsigned blocks = (unsigned)(((long long)n + kRayThreads - 1) / kRayThreads);   // 64-bit: n may be 2^31 - 1
-    const cudaStream_t s = (cudaStream_t)stream;
     image_rays_mask_kernel<TK, TR><<<blocks, kRayThreads, 0, s>>>(c, a->mask_at_box);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess)

@@ -8,53 +8,6 @@ import torch
 from . import capi
 
 
-def _camera(RT, K, bounds, H, W):
-    RT = np.asarray(RT, dtype=np.float64)
-    cam = capi.nb_camera()
-    kinv = np.linalg.inv(np.asarray(K, dtype=np.float64))
-    for i, v in enumerate(kinv.reshape(-1)):
-        cam.K_inv[i] = float(v)
-    for i, v in enumerate(RT[:3, :3].reshape(-1)):
-        cam.R[i] = float(v)
-    for i, v in enumerate(RT[:3, 3].reshape(-1)):
-        cam.T[i] = float(v)
-    for i, v in enumerate(np.asarray(bounds, dtype=np.float32).astype(np.float64).reshape(-1)):
-        cam.bounds[i] = float(v)
-    cam.H, cam.W = int(H), int(W)
-    return cam
-
-
-class ShardedRays:
-    """Fixed-shape device buffers for one rank's interleaved shard of an H x W view (nb_gen_rays_sharded): nothing is
-    compacted, so generating the rays of the next view never synchronises with the host.  Rays that miss the box (upstream
-    drops them, render_utils.py:131-132) are dead rays with mask 0."""
-
-    def __init__(self, H, W, rank=0, world=1, chunk=256, device="cuda:0"):
-        self.H, self.W, self.rank, self.world, self.chunk = int(H), int(W), int(rank), int(world), int(chunk)
-        n = self.H * self.W
-        n_chunks = (n + chunk - 1) // chunk
-        self.n_local = ((n_chunks + world - 1) // world) * chunk
-        dev = torch.device(device)
-        self.ray_o = torch.empty((1, self.n_local, 3), dtype=torch.float32, device=dev)
-        self.ray_d = torch.empty((1, self.n_local, 3), dtype=torch.float32, device=dev)
-        self.near = torch.empty((1, self.n_local), dtype=torch.float32, device=dev)
-        self.far = torch.empty((1, self.n_local), dtype=torch.float32, device=dev)
-        self.mask = torch.empty((1, self.n_local), dtype=torch.uint8, device=dev)
-        self.lib = capi.load()
-
-    def generate(self, RT, K, bounds):
-        """Enqueue the ray generation of one view on the current stream; returns self (ray_o, ray_d, near, far, mask)."""
-        cam = _camera(RT, K, bounds, self.H, self.W)
-        dev = self.ray_o.device
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            capi.check(self.lib.nb_gen_rays_sharded(C.byref(cam), self.rank, self.world, self.chunk, self.n_local,
-                                                    self.ray_o.data_ptr(), self.ray_d.data_ptr(), self.near.data_ptr(),
-                                                    self.far.data_ptr(), self.mask.data_ptr(), C.c_void_p(stream)),
-                       "nb_gen_rays_sharded")
-        return self
-
-
 def _host(*xs):
     """numpy copies of numpy arrays / tensors.  The device tensors among them come over in ONE copy (widened to float64,
     which holds float32 values exactly, and narrowed back), so a camera left on the GPU costs one host synchronisation."""
@@ -80,17 +33,67 @@ def camera_image_rays(RT, K, bounds, H, W, device="cuda:0"):
     given on the host costs one host synchronisation (reading n), one given as device tensors two (one copy of all of it
     to the host, then n)."""
     RT, K, bounds = _host(RT, K, bounds)
+    f64, host = _camera_operands(RT, K)
+    if bounds.dtype != np.float32 or bounds.shape != (2, 3):
+        raise ValueError("bounds must be the float32 (2,3) can_bounds (got %s %s)" % (bounds.dtype, bounds.shape))
+    return _image_rays_call(host, f64, False, bounds, H, W, device)
+
+
+def _camera_operands(RT, K):
+    """The host operands of nb_image_rays / nb_image_rays_f64 for the numpy camera RT (3,4) or (4,4), K (3,3), both float32
+    or both float64: -> (f64, [K_inv, R, T, o]) in the camera's dtype, inv(K) and the camera centre -np.dot(R.T, T) by
+    upstream's own numpy expressions (get_rays :10 and :16)."""
     if RT.dtype != K.dtype or RT.dtype not in (np.float32, np.float64):
         raise ValueError("the camera must be all float32 or all float64 (got RT %s, K %s)" % (RT.dtype, K.dtype))
     if RT.shape not in ((3, 4), (4, 4)) or K.shape != (3, 3):
         raise ValueError("RT must be (3,4) or (4,4) and K (3,3) (got %s and %s)" % (RT.shape, K.shape))
-    if bounds.dtype != np.float32 or bounds.shape != (2, 3):
-        raise ValueError("bounds must be the float32 (2,3) can_bounds (got %s %s)" % (bounds.dtype, bounds.shape))
-    f64 = RT.dtype == np.float64
     R, T = RT[:3, :3], RT[:3, 3]
-    host = [np.ascontiguousarray(x, dtype=RT.dtype).reshape(-1)
-            for x in (np.linalg.inv(K), R, T, -np.dot(R.T, T).ravel())]   # get_rays :10 and :16, as upstream evaluates them
-    return _image_rays_call(host, f64, False, bounds, H, W, device)
+    return RT.dtype == np.float64, [np.ascontiguousarray(x, dtype=RT.dtype).reshape(-1)
+                                    for x in (np.linalg.inv(K), R, T, -np.dot(R.T, T).ravel())]
+
+
+def _image_rays_enqueue(a, host, f64, dev):
+    """Enqueue nb_image_rays_f64 (f64) or nb_image_rays with the args `a` and the host operands `host` (K_inv, R, T, o) on
+    the current stream of `dev`."""
+    lib = capi.load()
+    ct = C.c_double if f64 else C.c_float
+    fn, name = (lib.nb_image_rays_f64, "nb_image_rays_f64") if f64 else (lib.nb_image_rays, "nb_image_rays")
+    with torch.cuda.device(dev):
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        capi.check(fn(C.byref(a), *[x.ctypes.data_as(C.POINTER(ct)) for x in host], stream), name)
+
+
+class ShardedRays:
+    """Fixed-shape device buffers for one rank's interleaved shard of an H x W view (nb_image_rays' shard mode): nothing is
+    compacted, so generating the rays of the next view from a camera on the host never synchronises with it.  A box-hit ray
+    carries the bits camera_image_rays gives its pixel; rays that miss the box (upstream drops them, render_utils.py:131-132)
+    are dead rays with mask 0."""
+
+    def __init__(self, H, W, rank=0, world=1, chunk=256, device="cuda:0"):
+        self.H, self.W, self.rank, self.world, self.chunk = int(H), int(W), int(rank), int(world), int(chunk)
+        n = self.H * self.W
+        n_chunks = (n + chunk - 1) // chunk
+        self.n_local = ((n_chunks + world - 1) // world) * chunk
+        dev = torch.device(device)
+        self.ray_o = torch.empty((1, self.n_local, 3), dtype=torch.float32, device=dev)
+        self.ray_d = torch.empty((1, self.n_local, 3), dtype=torch.float32, device=dev)
+        self.near = torch.empty((1, self.n_local), dtype=torch.float32, device=dev)
+        self.far = torch.empty((1, self.n_local), dtype=torch.float32, device=dev)
+        self.mask = torch.empty((1, self.n_local), dtype=torch.uint8, device=dev)
+        self.lib = capi.load()
+        self._args = a = capi.nb_image_rays_args()
+        a.H, a.W, a.rank, a.world, a.chunk, a.n_local = self.H, self.W, self.rank, self.world, self.chunk, self.n_local
+        a.ray_o, a.ray_d, a.near, a.far = (t.data_ptr() for t in (self.ray_o, self.ray_d, self.near, self.far))
+        a.mask_at_box = self.mask.data_ptr()
+
+    def generate(self, RT, K, bounds):
+        """Enqueue the ray generation of one view on the current stream; returns self (ray_o, ray_d, near, far, mask).  RT
+        and K as camera_image_rays takes them (a float64 camera runs nb_image_rays_f64, a float32 one nb_image_rays);
+        bounds, the world box (2,3), is cast to float32."""
+        f64, host = _camera_operands(*_host(RT, K))
+        self._args.bounds[:] = np.asarray(bounds, dtype=np.float32).reshape(-1).tolist()
+        _image_rays_enqueue(self._args, host, f64, self.ray_o.device)
+        return self
 
 
 def _image_rays_call(host, f64, k_f32, bounds, H, W, device, image=None):
@@ -101,8 +104,6 @@ def _image_rays_call(host, f64, k_f32, bounds, H, W, device, image=None):
     nbytes = lib.nb_image_rays_workspace_bytes(H, W)
     if nbytes == 0:
         raise ValueError("bad image size %d x %d" % (H, W))
-    ct = C.c_double if f64 else C.c_float
-    ptrs = [x.ctypes.data_as(C.POINTER(ct)) for x in host]
     dev = torch.device(device)
     n = H * W
     with torch.cuda.device(dev):
@@ -128,9 +129,7 @@ def _image_rays_call(host, f64, k_f32, bounds, H, W, device, image=None):
             rgb = torch.empty((n, 3), dtype=torch.float32, device=dev)
             a.image, a.rgb = image.data_ptr(), rgb.data_ptr()
         a.k_f32 = 1 if k_f32 else 0
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        fn, name = (lib.nb_image_rays_f64, "nb_image_rays_f64") if f64 else (lib.nb_image_rays, "nb_image_rays")
-        capi.check(fn(C.byref(a), *ptrs, stream), name)
+        _image_rays_enqueue(a, host, f64, dev)
         m = int(count.item())
         out = (ray_o[:m], ray_d[:m], near[:m], far[:m], mask.bool())
         return out if rgb is None else out + (rgb[:m],)
@@ -148,26 +147,6 @@ def dataset_image_rays(cam, k_kind, H, W, image, device="cuda:0"):
     host = [np.ascontiguousarray(cam[a:b]) for a, b in ((0, 9), (9, 18), (18, 21), (21, 24))]
     return _image_rays_call(host, True, int(k_kind) == capi.NB_SCALAR_F32, cam[24:30].astype(np.float32), H, W, device,
                             image=image)
-
-
-def image_rays(RT, K, bounds, H, W, device="cuda:0"):
-    """RT (3,4) or (4,4) world->camera, K (3,3), bounds (2,3) world box -> ray_o, ray_d (n,3), near, far (n,), mask_at_box
-    (H*W,) bool, all torch tensors on `device`; n = mask_at_box.sum() (order = row-major pixel order, as upstream)."""
-    lib = capi.load()
-    dev = torch.device(device)
-    cam = _camera(RT, K, bounds, H, W)
-    n = int(H) * int(W)
-    with torch.cuda.device(dev):
-        ray_o = torch.empty((n, 3), dtype=torch.float32, device=dev)
-        ray_d = torch.empty((n, 3), dtype=torch.float32, device=dev)
-        near = torch.empty((n,), dtype=torch.float32, device=dev)
-        far = torch.empty((n,), dtype=torch.float32, device=dev)
-        mask = torch.empty((n,), dtype=torch.uint8, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        capi.check(lib.nb_gen_rays(C.byref(cam), ray_o.data_ptr(), ray_d.data_ptr(), near.data_ptr(), far.data_ptr(),
-                                   mask.data_ptr(), C.c_void_p(stream)), "nb_gen_rays")
-        m = mask.bool()
-        return ray_o[m], ray_d[m], near[m], far[m], m
 
 
 def train_camera(K, R, T, can_bounds):

@@ -64,7 +64,7 @@ def test_depth_entry_points_exported_and_bound(built_lib):
     for name in ("nb_render_bwd_inputs", "nb_sample_pdf_src"):
         assert hasattr(lib, name) and name in capi.EXPORTS, name
     bound = capi.load()
-    assert bound.nb_abi_version() == 5
+    assert bound.nb_abi_version() == 6
     assert bound.nb_render_bwd_inputs.restype is ctypes.c_int and len(bound.nb_render_bwd_inputs.argtypes) == 5
     assert bound.nb_sample_pdf_src.restype is ctypes.c_int and len(bound.nb_sample_pdf_src.argtypes) == 3
     assert [f[0] for f in capi.nb_render_input_grads._fields_] == ["d_R", "d_Th", "d_ray_o", "d_ray_d", "d_near", "d_far",

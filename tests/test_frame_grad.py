@@ -40,7 +40,7 @@ def test_frame_entry_point_exported_and_bound(built_lib):
     assert hasattr(lib, "nb_render_bwd_frame")
     assert "nb_render_bwd_frame" in capi.EXPORTS
     bound = capi.load()
-    assert bound.nb_abi_version() == 5
+    assert bound.nb_abi_version() == 6
     assert bound.nb_render_bwd_frame.restype is ctypes.c_int
     assert len(bound.nb_render_bwd_frame.argtypes) == 4
 

@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(lib, name), "include/neuralbody_b200.h declares %s but the library does not export it" % name
     from neuralbody_b200 import capi
     assert sorted(capi.EXPORTS) == declared
-    assert capi.load().nb_abi_version() == 5
+    assert capi.load().nb_abi_version() == 6
 
 
 def test_struct_layouts_match_header(built_lib):
@@ -40,7 +40,7 @@ def test_struct_layouts_match_header(built_lib):
     import tempfile
     from neuralbody_b200 import capi
     src = ('#include <stdio.h>\n#include "neuralbody_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu\\n", sizeof(nb_volume_level), '
-           'sizeof(nb_decoder_weights), sizeof(nb_render_args), sizeof(nb_importance_args), sizeof(nb_camera));return 0;}\n')
+           'sizeof(nb_decoder_weights), sizeof(nb_render_args), sizeof(nb_importance_args), sizeof(nb_image_rays_args));return 0;}\n')
     with tempfile.TemporaryDirectory() as d:
         c = os.path.join(d, "p.c")
         open(c, "w").write(src)
@@ -48,7 +48,8 @@ def test_struct_layouts_match_header(built_lib):
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
         sizes = [int(x) for x in subprocess.check_output([exe]).split()]
     assert sizes == [ctypes.sizeof(capi.nb_volume_level), ctypes.sizeof(capi.nb_decoder_weights),
-                     ctypes.sizeof(capi.nb_render_args), ctypes.sizeof(capi.nb_importance_args), ctypes.sizeof(capi.nb_camera)]
+                     ctypes.sizeof(capi.nb_render_args), ctypes.sizeof(capi.nb_importance_args),
+                     ctypes.sizeof(capi.nb_image_rays_args)]
 
 
 def test_size_queries_without_gpu(built_lib):

@@ -49,6 +49,34 @@ def test_bad_arguments_are_rejected_before_any_launch(name, ct):
 
 
 @pytest.mark.parametrize("name,ct", [("nb_image_rays", C.c_float), ("nb_image_rays_f64", C.c_double)])
+def test_bad_shard_arguments_are_rejected_before_any_launch(name, ct):
+    L = lib()
+    fn = getattr(L, name)
+    K, R, T, o = cam(ct)
+
+    def shard(**kw):
+        a = args()
+        a.workspace, a.workspace_bytes, a.count = None, 0, None      # shard mode reads neither
+        a.rank, a.world, a.chunk, a.n_local = 1, 2, 64, 128
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    for kw in ({"rank": -1}, {"rank": 2}, {"world": -1}, {"world": -2, "rank": -1}, {"chunk": 0}, {"chunk": -64},
+               {"n_local": -1}):
+        assert fn(C.byref(shard(**kw)), K, R, T, o, None) == -1, kw
+        assert b"shard mode needs" in L.nb_last_error(), kw
+    for kw in ({"image": 256, "rgb": 256}, {"image": 256}, {"rgb": 256}):
+        assert fn(C.byref(shard(**kw)), K, R, T, o, None) == -1, kw
+        assert b"NULL in shard mode" in L.nb_last_error(), kw
+    for field in ("ray_o", "ray_d", "near", "far", "mask_at_box"):
+        assert fn(C.byref(shard(**{field: None})), K, R, T, o, None) == -1, field
+        assert b"null" in L.nb_last_error()
+    assert fn(C.byref(shard(H=0)), K, R, T, o, None) == -1 and b"H and W" in L.nb_last_error()
+    assert fn(C.byref(shard(n_local=0)), K, R, T, o, None) == 0     # nothing to write: nothing enqueued
+
+
+@pytest.mark.parametrize("name,ct", [("nb_image_rays", C.c_float), ("nb_image_rays_f64", C.c_double)])
 def test_short_workspace_is_rejected(name, ct):
     L = lib()
     need = L.nb_image_rays_workspace_bytes(48, 64)

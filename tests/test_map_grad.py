@@ -63,7 +63,7 @@ def test_map_entry_point_exported_and_bound(built_lib):
     assert hasattr(lib, "nb_render_bwd_maps")
     assert "nb_render_bwd_maps" in capi.EXPORTS
     bound = capi.load()
-    assert bound.nb_abi_version() == 5
+    assert bound.nb_abi_version() == 6
     assert bound.nb_render_bwd_maps.restype is ctypes.c_int
     assert len(bound.nb_render_bwd_maps.argtypes) == 8
 

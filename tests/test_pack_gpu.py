@@ -75,39 +75,12 @@ def test_pack_weights_fold_matches_fp64_torch():
     assert bc.shape == (2, 128)
 
 
-def test_gen_rays_matches_reference_numpy():
-    """f-2: nb_gen_rays vs get_rays / get_near_far (restated literally in oracle/synth.py)."""
-    from oracle import synth
-    from neuralbody_b200 import rays
-    scene, _, _ = golden_case("eval_s64")
-    cb = scene["can_bounds"][0].numpy()
-    center = 0.5 * (cb[0] + cb[1]).astype(np.float64)
-    for az, f in ((20.0, 150.0), (133.0, 90.0)):
-        R, T = synth.look_at_camera(center, 0.9, az)
-        H = W = 96
-        K = np.array([[f, 0, W / 2.0], [0, f * 1.1, H / 2.0], [0, 0, 1.0]])
-        ro, rd = synth.get_rays(H, W, K, R, T)
-        ro = ro.reshape(-1, 3).astype(np.float32); rd = rd.reshape(-1, 3).astype(np.float32)
-        near, far, mask = synth.get_near_far(cb, ro, rd)
-        RT = np.concatenate([R, T], 1)
-        g_ro, g_rd, g_near, g_far, g_mask = rays.image_rays(RT, K, cb, H, W)
-        gm = g_mask.cpu().numpy()
-        assert (gm != mask).mean() < 1e-3                    # grazing rays may flip
-        both = mask & gm
-        sel_ref = both[mask]; sel_gpu = both[gm]
-        np.testing.assert_allclose(g_ro.cpu().numpy()[sel_gpu], ro[mask][sel_ref], rtol=1e-6, atol=1e-6)
-        np.testing.assert_allclose(g_rd.cpu().numpy()[sel_gpu], rd[mask][sel_ref], rtol=1e-5, atol=1e-6)
-        np.testing.assert_allclose(g_near.cpu().numpy()[sel_gpu], near.astype(np.float32)[sel_ref], rtol=1e-5, atol=1e-5)
-        np.testing.assert_allclose(g_far.cpu().numpy()[sel_gpu], far.astype(np.float32)[sel_ref], rtol=1e-5, atol=1e-5)
-        assert 0 < mask.sum() < H * W
-
-
 def test_sharded_ray_generation_matches_the_full_image():
-    """nb_gen_rays_sharded: rank r's fixed-shape shard holds exactly the pixels the interleaved plan gives it; box-hit rays carry
-    the bits nb_gen_rays writes, the others are dead rays (near = far = 0, mask 0)."""
-    import ctypes as C
+    """ShardedRays (nb_image_rays' shard mode), for a float64 and a float32 camera: rank r's fixed-shape shard holds exactly
+    the pixels the interleaved plan gives it; box-hit rays carry the bits camera_image_rays writes, the others are dead rays
+    (near = far = 0, mask 0), and a slot past the last pixel is o = 0, d = (0, 0, 1)."""
     from oracle import synth
-    from neuralbody_b200 import capi, rays, dist as nbdist
+    from neuralbody_b200 import rays, dist as nbdist
     scene, _, _ = golden_case("eval_s64")
     cb = scene["can_bounds"][0].numpy()
     center = 0.5 * (cb[0] + cb[1]).astype(np.float64)
@@ -115,24 +88,31 @@ def test_sharded_ray_generation_matches_the_full_image():
     H, W = 50, 70                                   # 3500 pixels: not a multiple of world * chunk
     K = np.array([[95.0, 0, W / 2.0], [0, 99.0, H / 2.0], [0, 0, 1.0]])
     RT = np.concatenate([R, T], 1)
-    ro, rd, near, far, m = rays.image_rays(RT, K, cb, H, W)
-    full = {k: torch.zeros((H * W,) + s, device="cuda") for k, s in (("ray_o", (3,)), ("ray_d", (3,)), ("near", ()), ("far", ()))}
-    full["ray_o"][m], full["ray_d"][m], full["near"][m], full["far"][m] = ro, rd, near, far
-    assert 0 < int(m.sum()) < H * W
     world, chunk = 3, 64
-    seen = torch.zeros(H * W, dtype=torch.bool, device="cuda")
-    for rank in range(world):
-        sh = rays.ShardedRays(H, W, rank, world, chunk).generate(RT, K, cb)
-        idx, per = nbdist.shard_indices(H * W, rank, world, chunk)
-        assert sh.n_local == per
-        j = torch.arange(per, device="cuda")
-        pix = ((j // chunk) * world + rank) * chunk + j % chunk
-        ok = pix < H * W
-        hit = torch.zeros(per, dtype=torch.bool, device="cuda")
-        hit[ok] = m[pix[ok]]
-        assert torch.equal(sh.mask[0].bool(), hit)
-        for k in ("ray_o", "ray_d", "near", "far"):
-            assert torch.equal(getattr(sh, k)[0][hit], full[k][pix[hit]]), k
-        assert float(sh.near[0][~hit].abs().max()) == 0.0 and float(sh.far[0][~hit].abs().max()) == 0.0
-        seen[pix[ok]] = True
-    assert bool(seen.all())
+    for dt in (np.float64, np.float32):
+        ro, rd, near, far, m = rays.camera_image_rays(RT.astype(dt), K.astype(dt), cb, H, W)
+        full = {k: torch.zeros((H * W,) + s, device="cuda") for k, s in (("ray_o", (3,)), ("ray_d", (3,)), ("near", ()),
+                                                                          ("far", ()))}
+        full["ray_o"][m], full["ray_d"][m], full["near"][m], full["far"][m] = ro, rd, near, far
+        assert 0 < int(m.sum()) < H * W
+        seen = torch.zeros(H * W, dtype=torch.bool, device="cuda")
+        past_slots = 0
+        for rank in range(world):
+            sh = rays.ShardedRays(H, W, rank, world, chunk).generate(RT.astype(dt), K.astype(dt), cb)
+            idx, per = nbdist.shard_indices(H * W, rank, world, chunk)
+            assert sh.n_local == per
+            j = torch.arange(per, device="cuda")
+            pix = ((j // chunk) * world + rank) * chunk + j % chunk
+            ok = pix < H * W
+            hit = torch.zeros(per, dtype=torch.bool, device="cuda")
+            hit[ok] = m[pix[ok]]
+            assert torch.equal(sh.mask[0].bool(), hit), dt
+            for k in ("ray_o", "ray_d", "near", "far"):
+                assert torch.equal(getattr(sh, k)[0][hit], full[k][pix[hit]]), (dt, k)
+            assert float(sh.near[0][~hit].abs().max()) == 0.0 and float(sh.far[0][~hit].abs().max()) == 0.0
+            past = ~ok
+            assert torch.equal(sh.ray_o[0][past], torch.zeros((int(past.sum()), 3), device="cuda"))
+            assert torch.equal(sh.ray_d[0][past], torch.tensor([0.0, 0.0, 1.0], device="cuda").expand(int(past.sum()), 3))
+            past_slots += int(past.sum())
+            seen[pix[ok]] = True
+        assert bool(seen.all()) and past_slots > 0

@@ -65,7 +65,7 @@ def test_ray_entry_point_exported_and_bound(built_lib):
     assert hasattr(lib, "nb_render_bwd_rays")
     assert "nb_render_bwd_rays" in capi.EXPORTS
     bound = capi.load()
-    assert bound.nb_abi_version() == 5
+    assert bound.nb_abi_version() == 6
     assert bound.nb_render_bwd_rays.restype is ctypes.c_int
     assert len(bound.nb_render_bwd_rays.argtypes) == 6
 
